@@ -1,5 +1,5 @@
 """Alias package: `import dalm...` resolves to dalm_b200's drop-in modules, so code written against the reference's
-import paths (dalm.models.*, dalm.training.*, dalm.cli, dalm.utils) runs unchanged on the B200 build.
+import paths (dalm.models.*, dalm.training.*, dalm.cli, dalm.utils) runs unchanged on the H100 build.
 
 `dalm.X` IS `dalm_b200.X` (the same module object, executed once): the finder hands the import machinery a spec whose
 loader returns the already-imported real module from `create_module` and does nothing in `exec_module`, so module

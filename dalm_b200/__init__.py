@@ -1,4 +1,4 @@
-"""dalm_b200 — B200-native drop-in for DALM's RAG-e2e / retriever-only training step.
+"""dalm_b200 — H100-native drop-in for DALM's RAG-e2e / retriever-only training step.
 
 Public surface mirrors the reference package `dalm` for this path:
   dalm_b200.models.rag_e2e_base_model.{AutoModelForRagE2E, Mode}

@@ -1,6 +1,6 @@
 """ctypes binding of libdalm_b200.so (the C ABI declared in include/dalm_b200.h).
 
-There is no CPU or PyTorch fallback: if the shared library is missing, or a kernel is invoked without an sm_100
+There is no CPU or PyTorch fallback: if the shared library is missing, or a kernel is invoked without an sm_90
 device, this module raises.
 """
 from __future__ import annotations
@@ -39,13 +39,11 @@ SIGNATURES = {
     "dalm_b200_gemm_set_raster": [_I],
     "dalm_b200_gemm_set_l2_hints": [_I],
     "dalm_b200_attention_fwd": [_P, _L, _P, _L, _P, _L, _P, _P, _L, _P, _I, _I, _I, _I, _I, _F, _I, *_DROP, _P],
+    "dalm_b200_attention_tc_fwd": [_P, _L, _P, _L, _P, _L, _P, _P, _L, _P, _I, _I, _I, _I, _I, _F, _I, *_DROP, _P],
+    "dalm_b200_attention_tc_bwd": [_P, _L, _P, _L, _P, _L, _P, _P, _L, _P, _P, _L, _P, _P, _L, _P, _L, _P, _L,
+                                   _I, _I, _I, _I, _I, _F, _I, *_DROP, _P],
     "dalm_b200_attention_bwd": [_P, _L, _P, _L, _P, _L, _P, _P, _L, _P, _P, _L, _P, _P, _L, _P, _L, _P, _L,
                                 _I, _I, _I, _I, _I, _F, _I, *_DROP, _P],
-    "dalm_b200_attention_tc_fwd": [_P, _L, _L, _I, _P, _L, _L, _I, _P, _L, _L, _I, _P, _P, _L, _P, _I, _I, _I, _I, _I, _F, _I, *_DROP, _P],
-    "dalm_b200_attention_tc_set_debug": [_P],
-    "dalm_b200_attention_tc_set_mode": [_I],
-    "dalm_b200_attention_tc_bwd": [_P, _L, _L, _P, _L, _L, _P, _L, _L, _P, _P, _L, _P, _P, _L, _L, _P, _P, _L, _P, _L, _P, _L,
-                                   _I, _I, _I, _I, _I, _F, _I, *_DROP, _P],
     "dalm_b200_layernorm_fwd": [_P, _P, _P, _P, _P, _L, _P, _P, _I, _I, _F, *_DROP, _P],
     "dalm_b200_layernorm_bwd": [_P, _P, _P, _P, _P, _P, _L, _P, _P, _L, _I, _I, *_DROP, _P],
     "dalm_b200_layernorm_bwd_res": [_P, _P, _P, _P, _P, _P, _L, _P, _P, _P, _L, _I, _I, _P],
@@ -93,8 +91,6 @@ _RESTYPES = {
     "dalm_b200_gemm_clear_cache": None,
     "dalm_b200_gemm_set_raster": None,
     "dalm_b200_gemm_set_l2_hints": None,
-    "dalm_b200_attention_tc_set_debug": None,
-    "dalm_b200_attention_tc_set_mode": None,
 }
 
 _lib = None

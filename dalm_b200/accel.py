@@ -150,7 +150,8 @@ class GradientSync:
         if world > 1 and self.large and nccl:
             reserve = int(os.environ.get("NCCL_MAX_CTAS", "0") or 0)
             if reserve > 0:                                    # leave NCCL's CTAs their SMs (see ops.GEMM_MAX_CTAS): applied from the
-                self.gemm_cap = max(148 - reserve, 64)         # first bucket of a backward until the step's last collective is queued
+                sms = torch.cuda.get_device_properties(device).multi_processor_count
+                self.gemm_cap = max(sms - reserve, 64)         # first bucket of a backward until the step's last collective is queued
         if world > 1 and self.large:
             if torch.cuda.is_available() and torch.device(device).type == "cuda":
                 self.side = torch.cuda.Stream(device=device)

@@ -11,7 +11,7 @@ from typing_extensions import Annotated
 
 from . import __version__
 
-cli = typer.Typer(add_completion=False, help="B200-native DALM training step")
+cli = typer.Typer(add_completion=False, help="H100-native DALM training step")
 
 
 class DALMSchedulerType(str, Enum):
@@ -210,7 +210,7 @@ def qa_gen(                                   # reference cli.py:280-309: same a
     sample_size: Annotated[int, typer.Option(help="Number of examples to process.")] = 1000,
     as_csv: Annotated[bool, typer.Option(help="Save the files as CSV.")] = True,
 ) -> None:
-    """(reference command — QA-pair data generation — not part of the B200 hot-path build; exits with status 2)"""
+    """(reference command — QA-pair data generation — not part of the H100 hot-path build; exits with status 2)"""
     _out_of_scope("qa-gen")
 
 

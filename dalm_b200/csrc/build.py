@@ -1,4 +1,4 @@
-"""Build libdalm_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libdalm_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python -m dalm_b200.csrc.build [--force]
 """
@@ -10,11 +10,11 @@ import sys
 from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SOURCES = ["api.cu", "loss.cu", "gemm_tcgen05.cu", "attention.cu", "rowwise.cu", "lora.cu", "attention_tc.cu", "dense_grad.cu", "topk.cu", "nf4.cu", "decode.cu"]
+SOURCES = ["api.cu", "loss.cu", "gemm_wgmma.cu", "attention.cu", "rowwise.cu", "lora.cu", "dense_grad.cu", "topk.cu", "nf4.cu", "decode.cu"]
 HEADERS = ["common.cuh", "ptx.cuh"]
 LIB = os.path.join(HERE, "libdalm_b200.so")
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]
 
@@ -52,7 +52,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     with ThreadPoolExecutor(max_workers=min(8, len(SOURCES))) as ex:
         objs = list(ex.map(compile_one, SOURCES))
-    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [nvcc, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -1,5 +1,5 @@
-// dalm_b200 — shared device/host helpers for the sm_100a kernels.
-// Everything in csrc/ is compiled with: nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3
+// dalm_b200 — shared device/host helpers for the sm_90a kernels.
+// Everything in csrc/ is compiled with: nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -34,10 +34,12 @@ void count_launch(int n = 1);                 // bumps the global launch counter
     }                                                                                     \
   } while (0)
 
-constexpr int kNumSMs = 148;   // B200: 2 dies x 74 SMs
+// SM count and L2 size of the device the library first runs on (read once; persistent grids and L2 heuristics use them)
+int num_sms();
+long long l2_bytes();
 
 // cached TMA descriptor of a row-major [rows, cols] bf16 (or fp32) matrix with row stride ld; box = {128 bytes, box_rows},
-// 128B swizzle (defined in gemm_tcgen05.cu)
+// 128B swizzle (defined in gemm_wgmma.cu)
 int get_tmap(const void* ptr, long long rows, long long cols, long long ld, int box_rows, ::CUtensorMap_st* out, int f32 = 0);
 
 // ---------------------------------------------------------------------------------------------

@@ -13,9 +13,8 @@
 // each row's current column) lives in device memory: a decode step is then the SAME launch sequence with the same
 // arguments for every token and can be captured once as a CUDA graph and replayed (292 launches per token at Llama-2-7B).
 // The host reads back one "is anyone still generating" counter every few steps.
-// Measured (profiles/README.md, r01_decode_bench.jsonl): a decode step costs ~3.3 ms + 0.029 ms x cached tokens; the second
-// term is attn_decode_kernel's PV pass (pass 3 below walks the keys serially per thread, one dependent 2-byte load each):
-// the known limiter of this file, first item of the next round.
+// A decode step's cost grows with the cached tokens through attn_decode_kernel's PV pass (pass 3 below walks the keys serially
+// per thread, one dependent 2-byte load each); attn_decode_par_kernel below parallelises that pass and is the default.
 #include "common.cuh"
 #include <limits.h>
 #include <stdlib.h>
@@ -125,12 +124,10 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const __nv_bfloat16* _
   if (g == 0) out[(size_t)b * ldo + h * D + d] = __float2bfloat16(acc / sum);
 }
 
-// DEFAULT decode attention: the kernel above with a parallel PV pass. Measured on the first kernel: 0.9 us per cached key per
-// layer, because its pass 3 walks the keys serially per thread with the V load behind `if (p != 0)` (profiles/README.md,
-// r01_decode_bench.jsonl line 4). Here 128 threads = KG key groups x D/8 lanes, every lane loads 16 bytes of V unconditionally
+// DEFAULT decode attention: the kernel above with a parallel PV pass (the first kernel's pass 3 walks the keys serially per
+// thread with the V load behind `if (p != 0)`). Here 128 threads = KG key groups x D/8 lanes, every lane loads 16 bytes of V unconditionally
 // (masked keys carry p = 0; their cache rows are initialised memory) and the KG partial rows meet in shared memory.
-// Measured (profiles/r02b_decode_bench.jsonl, Llama-2-7B shape, 16 x 192 -> 256 tokens): 13.3 / 9.1 ms (graph / eager) per token
-// step with the first kernel -> 4.55 / 5.0 ms = 3 514 tokens/s = 0.50 of the HBM floor. DALM_B200_DECODE_ATTN=1 selects the first
+// DALM_B200_DECODE_ATTN=1 selects the first
 // kernel (kept as the cross-check of tests/test_generate_gpu.py).
 // one explicit 16-byte read-only load -> 8 floats (the struct-typed loads above are split into 32-bit loads by the compiler)
 __device__ __forceinline__ void load8_nc(const __nv_bfloat16* p, float* f) {
@@ -279,9 +276,8 @@ __global__ void __launch_bounds__(256) greedy_step_kernel(const __nv_bfloat16* _
 
 // ------------------------------------------------------------------------------------------------------------
 // Weight-streaming GEMM for the decode step: out[m, n] = act(sum_k A[m,k] W[n,k]) + resid[m,n] with M <= 16 token rows.
-// HBM-bound: every weight is read exactly once (N*K*2 bytes), the activations (16 x K bf16) stay in L2. The 128-row tcgen05
-// tile of the training GEMM wastes 7/8 of its A tile here and runs N = 4096 on 64 CTAs (measured 10.2 ms per token at
-// Llama-2-7B against a 2.3 ms HBM floor), so this path uses one `mma.sync.m16n8k16` row tile = the whole batch instead:
+// HBM-bound: every weight is read exactly once (N*K*2 bytes), the activations (16 x K bf16) stay in L2. The 128-row wgmma
+// tile of the training GEMM wastes 7/8 of its A tile here and runs N = 4096 on 64 CTAs, so this path uses one `mma.sync.m16n8k16` row tile = the whole batch instead:
 //   CTA = 16 output columns (2 n-tiles) x all of K, 256 threads; the 8 warps interleave over 32-wide k-chunks (split-K inside
 //   the CTA), partial sums meet in shared memory. Each lane loads 16 bytes (8 consecutive k) of one weight row and of two
 //   activation rows per chunk straight from global memory into MMA fragments: lane (g, t) takes k = chunk*32 + 8t .. +7, and

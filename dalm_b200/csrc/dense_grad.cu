@@ -1,6 +1,6 @@
 // dalm_b200 — parameter-gradient kernels of FULL fine-tuning (reference default `use_peft=None`: every parameter of the
 // HF model the wrapper holds is trainable, dalm/models/rag_e2e_base_model.py:45-59 + train_rage2e.py:336). The dense
-// weight gradients dW = dY^T X are tcgen05 GEMMs (gemm_tcgen05.cu, layout 2); what is left is HBM-bound row/column work:
+// weight gradients dW = dY^T X are wgmma GEMMs (gemm_wgmma.cu, layout 2); what is left is HBM-bound row/column work:
 //   col_reduce      bias gradients (column sums of dY) and LayerNorm / RMSNorm gain+bias gradients (sum_m dy, sum_m dy*zhat)
 //   embed_scatter   word / position embedding gradients (scatter-add of the embedding-LayerNorm input gradient)
 //   masked_add      g = (a_f32 + b_bf16) * dropout_mask  (gradient through the embedding dropout)
@@ -143,7 +143,7 @@ extern "C" int dalm_b200_col_reduce(const float* dy_f32, const void* dy_bf16, lo
   DALM_REQUIRE(out_sum || out_prod, "col_reduce: no output");
   DALM_REQUIRE(!out_prod || (z && rstd), "col_reduce: out_prod needs z and rstd");
   const int colblocks = (H + kCrCols - 1) / kCrCols;
-  int splits = (4 * kNumSMs + colblocks - 1) / colblocks;
+  int splits = (4 * num_sms() + colblocks - 1) / colblocks;
   const int max_splits = (M + 63) / 64;
   if (splits > max_splits) splits = max_splits;
   if (splits < 1) splits = 1;

@@ -5,7 +5,7 @@
 //
 // Both are HBM-bound (X is read exactly once: 38 MB per call at cfg-3) with a trivial amount of math, so they use
 // warp-level mma.sync (m16n8k16, the 16-row tile IS the LoRA rank) fed by cp.async double buffering instead of the
-// tcgen05 path: there is no reuse to stage, only bytes to stream.
+// wgmma path: there is no reuse to stage, only bytes to stream.
 // Replaces the two skinny GEMMs per adapted Linear that peft's LoRA layer adds per pass (reference
 // dalm/models/rag_e2e_base_model.py:61-80,144-160) and their autograd backward.
 #include "common.cuh"

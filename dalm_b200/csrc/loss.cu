@@ -370,7 +370,7 @@ extern "C" int dalm_b200_inbatch_loss_fwd_bwd(const float* Q, const float* P, in
     DALM_CUDA(cudaFuncSetAttribute(inbatch_loss_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     attr_set = true;
   }
-  const int grid = B < kNumSMs ? B : kNumSMs;     // co-resident by construction (<= 1 CTA per SM)
+  const int grid = B < num_sms() ? B : num_sms();     // co-resident by construction (<= 1 CTA per SM)
   void* args[] = {&p};
   DALM_CUDA(cudaLaunchCooperativeKernel((void*)inbatch_loss_kernel, dim3(grid), dim3(256), args, smem,
                                         (cudaStream_t)stream));

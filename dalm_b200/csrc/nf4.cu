@@ -5,7 +5,7 @@
 // bnb_4bit_compute_dtype=bfloat16): weights are cast to fp16, split into blocks of 64 consecutive elements, each block
 // stores absmax (fp32) and sixteen-level codes of x / absmax; every forward dequantises code * absmax back to fp16 and runs
 // the matmul in bf16. The values the GEMM sees are therefore a pure function of the checkpoint — this kernel computes them
-// once at load time, and the product keeps them resident as bf16 (a B200 has the HBM; the reference quantises to fit 7B
+// once at load time, and the product keeps them resident as bf16 (an H100 has the HBM for 7B; the reference quantises to fit 7B
 // models on smaller parts). Same numerics as bnb's forward, none of its per-step dequantisation.
 #include "common.cuh"
 #include <cuda_fp16.h>
@@ -83,7 +83,7 @@ __global__ void nf4_quantize_kernel(const float* __restrict__ w, long long n, un
 
 // bf16 out[r, c] = bf16(fp16(code * absmax))  (the value the dequantised-resident mode keeps). grid (ceil((cols/16 + 1)/256), rows):
 // a thread expands 16 codes (8 bytes in, 32 bytes out); the sixteen levels sit in shared memory (divergent indices into
-// __constant__ memory serialise: the first version of this kernel ran at 0.95 TB/s); the last thread of a row copies the row's
+// __constant__ memory serialise); the last thread of a row copies the row's
 // `tail_cols` extra columns (the LoRA block of a K-augmented weight) from `tail`
 __global__ void __launch_bounds__(256) nf4_dequant_bf16_kernel(const unsigned char* __restrict__ packed, const float* __restrict__ absmax,
                                                                long long rows, int cols, __nv_bfloat16* __restrict__ out, long long ldo,

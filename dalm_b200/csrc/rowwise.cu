@@ -1,7 +1,7 @@
 // dalm_b200 — HBM-bound row-wise kernels of the encoder/decoder blocks (everything that is not a tensor-core tile):
 // LayerNorm / RMSNorm forward+backward, embedding gathers, RoPE, SwiGLU, GELU, masked mean-pool + L2 normalise,
 // LoRA weight-gradients, fused Adam. All use 16-byte vector accesses, warp-shuffle reductions and one CTA per row
-// (rows = tokens; 3204..26700 per launch => several waves over 148 SMs).
+// (rows = tokens; 3204..26700 per launch => several waves over 132 SMs).
 //
 // Reference semantics: HF BertModel / LlamaForCausalLM blocks reached via dalm/models/rag_e2e_base_model.py:93,105;
 // mean_pooling + F.normalize: rag_e2e_base_model.py:96-97,108-111; torch.optim.Adam: train_rage2e.py:336.
@@ -323,7 +323,7 @@ __global__ void rope_kernel(__nv_bfloat16* __restrict__ buf, long long ld, int c
 // ------------------------------------------------------------------------------------------------------------
 // gate / up column of feature i inside a [M, 2F] gate|up buffer: il == 0: [gate 0..F | up 0..F] (HF order); il > 0: blocks of il
 // features interleaved [gate blk | up blk | gate blk+1 | ...] - the layout that puts a feature's gate AND up accumulator in the
-// same 128 x 256 GEMM tile (gemm_tcgen05.cu: SwiGLU epilogue)
+// same 128 x 256 GEMM tile (gemm_wgmma.cu: SwiGLU epilogue)
 __device__ __forceinline__ int gate_col(int i, int F, int il, int& up_off) {
   if (il == 0) { up_off = F; return i; }
   up_off = il;
@@ -368,7 +368,7 @@ __global__ void swiglu_bwd_kernel(__nv_bfloat16* __restrict__ gu, long long ldgu
 
 // GELU(erf) forward on a pre-activation buffer, and backward in place on the incoming gradient
 // GELU forward / backward: each thread walks GELU_ROWS rows of one 8-column group with all of its 16-byte loads issued before
-// the first use (one row per thread left HBM at 0.45 / 0.56 of the measured peak: profiles/r02_hbm_kernels_ncu.txt)
+// the first use (one row per thread leaves most of the HBM bandwidth unused)
 constexpr int GELU_ROWS = 4;
 __global__ void gelu_fwd_kernel(const __nv_bfloat16* __restrict__ pre, long long ldp, __nv_bfloat16* __restrict__ act,
                                 long long lda, int M, int F) {
@@ -415,8 +415,7 @@ __global__ void gelu_bwd_kernel(const __nv_bfloat16* __restrict__ pre, long long
 
 // ------------------------------------------------------------------------------------------------------------
 // LayerNorm, one WARP per row (H = 256 NV8, NV8 <= 8: bge-large's 1024). The CTA-per-row kernels above give a 1024-wide row to
-// 256 threads - one float4 each - and spend their time in two block-wide reductions: 0.39 (fwd) / 0.62 (bwd) of the measured
-// HBM peak at cfg-2 (profiles/r02_hbm_kernels_ncu.txt), 14 % of that step. Here a lane keeps its 8 NV8 elements in registers
+// 256 threads - one float4 each - and spend their time in two block-wide reductions, far from the HBM bandwidth. Here a lane keeps its 8 NV8 elements in registers
 // (8 consecutive floats per 256-wide chunk: one Philox group per chunk when dropout is on), statistics by warp shuffles, no
 // shared memory, 8 rows per CTA.
 // ------------------------------------------------------------------------------------------------------------
@@ -592,7 +591,7 @@ __global__ void __launch_bounds__(256) pool_norm_fwd_kernel(const float* __restr
   for (int i = threadIdx.x; i < H; i += blockDim.x) emb[(size_t)b * H + i] = pooled[(size_t)b * H + i] * s;
 }
 // The same forward for H % 128 == 0, spread over the machine: the one-CTA-per-sample kernel above walks the L rows serially
-// (B CTAs, 168 us for 9.4 MB = 56 GB/s at cfg-3). Here CTA (chunk, b) owns 128 columns of sample b: each of its 8 warps
+// (B CTAs: a small fraction of the machine). Here CTA (chunk, b) owns 128 columns of sample b: each of its 8 warps
 // streams the rows l = warp, warp + 8, ... (one coalesced 512-byte float4 row piece per warp-load, masked rows skipped), the
 // warps' partial sums meet in shared memory. B x H/128 CTAs (144 at cfg-3, 1200 at cfg-2). A second tiny launch normalises.
 __global__ void __launch_bounds__(256) pool_sum_kernel(const float* __restrict__ hidden, const int64_t* __restrict__ mask,
@@ -720,7 +719,7 @@ __global__ void __launch_bounds__(256) lora_dx_kernel(__nv_bfloat16* __restrict_
   const unsigned long long dstream = drop_stream(drop);
   const int nrows = min(ROWS, M - m0);
   // four rows per step with their loads issued together: the read-modify-write of dh otherwise serialises one 16-byte
-  // load per thread per iteration (measured 47 us for 76 MB = a quarter of HBM speed)
+  // load per thread per iteration
   for (int mm = 0; mm < nrows; mm += 4) {
     bf16x8 raw[4];
 #pragma unroll
@@ -976,8 +975,8 @@ extern "C" int dalm_b200_lora_dx(void* dh, long long lddh, const void* G, long l
                                  const void* offset, void* stream) {
   DALM_REQUIRE((R == 8 || R == 16 || R == 24) && (K % 8) == 0 && (lddh % 8) == 0 && (lda % 8) == 0, "lora_dx: bad shape R=%d K=%d", R, K);
   DALM_REQUIRE(p >= 0.f && p < 1.f, "lora_dx: p must be in [0,1)");
-  // one thread per 8 columns: a CTA no wider than the row (bge-large, K = 1024: 128 threads - a 256-thread CTA kept half of its
-  // warps resident but idle, 107 us for 109 MB at cfg-2)
+  // one thread per 8 columns: a CTA no wider than the row (bge-large, K = 1024: 128 threads - a 256-thread CTA keeps half of its
+  // warps resident but idle)
   const int cols8 = K / 8;
   const int threads = cols8 >= 256 ? 256 : ((cols8 + 31) / 32) * 32;
   dim3 grid((cols8 + threads - 1) / threads, (M + 15) / 16);

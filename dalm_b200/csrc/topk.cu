@@ -2,8 +2,8 @@
 //
 // Replaces the approximate hnswlib index of the reference's evaluation path (dalm/eval/utils.py:18-66: space "ip",
 // M=100, ef_construction=200, ef=100; `knn_query` returns labels sorted by distance = 1 - <q,p>) with an exact sweep:
-// for 200k x 1024 fp32 passages one query batch reads 819 MB — 125 us at HBM speed — so there is no reason to
-// approximate on a B200. HBM-bound: algorithmic bytes = N*D*4 (the passage matrix, read once per query tile of <= 8).
+// for 200k x 1024 fp32 passages one query batch reads 819 MB — about 0.25 ms at the H100's 3.35 TB/s — so there is no reason to
+// approximate on an H100. HBM-bound: algorithmic bytes = N*D*4 (the passage matrix, read once per query tile of <= 8).
 //
 // Stage 1 (topk_scan_kernel): the grid walks the passage rows; each warp takes two rows at a time (lanes read consecutive
 //   float4: 512 contiguous bytes per request), accumulates the dot products with the <= 8 queries of the tile held in
@@ -88,8 +88,11 @@ __device__ __forceinline__ void reduce_and_insert(const float2 (&acc2)[2][QT], f
 }
 
 __device__ __forceinline__ float2 fma2(const float4& p, const float4& x, float2 acc) {
-  acc = __ffma2_rn(make_float2(p.x, p.y), make_float2(x.x, x.y), acc);        // Blackwell packed fp32 FMA: 2 per instruction
-  return __ffma2_rn(make_float2(p.z, p.w), make_float2(x.z, x.w), acc);
+  acc.x = fmaf(p.x, x.x, acc.x);                               // two independent fp32 FMA chains per pair of lanes
+  acc.y = fmaf(p.y, x.y, acc.y);
+  acc.x = fmaf(p.z, x.z, acc.x);
+  acc.y = fmaf(p.w, x.w, acc.y);
+  return acc;
 }
 
 template <int QT>
@@ -167,10 +170,9 @@ __global__ void __launch_bounds__(256, 2) topk_scan_kernel(const float* __restri
 // Pipelined variant (D <= kTopkPipeMaxD): every warp owns a 2-slot shared-memory ring of R = 2 passage rows; lanes stream
 // the NEXT 2 rows in with 16-byte cp.async while the warp computes on the current 2 from shared memory (no CTA-wide
 // barrier: a warp only waits for its own copies). ncu of the register-load version above showed 16 warps/SM stalled on
-// their own global loads ("long scoreboard" 6.8 of 13 issue cycles, 27 % of HBM peak): the loads of a warp were only in
+// their own global loads: the loads of a warp were only in
 // flight while it was not computing. Here 8 warps x 8 KB stay in flight per SM for the whole sweep (160 KB of shared
-// memory at D = 1024: one CTA per SM). Measured 3.1-3.5 TB/s (0.48-0.54 of the HBM copy peak) at 200k x 1024; a variant with
-// 4 rows per query read and 6 warps (224 KB) was slower (2.6 TB/s): fewer warps cost more than the saved LDS traffic.
+// memory at D = 1024: one CTA per SM).
 constexpr int kTopkPipeMaxD = 1024;
 constexpr int kTopkR = 2;
 constexpr int kTopkPipeWarps = 8;   // 8 warps x 2 slots x 2 rows x 4 KB + the 32 KB query tile = 160 KB at D = 1024
@@ -284,7 +286,7 @@ __global__ void __launch_bounds__(256) topk_merge_kernel(const float* __restrict
 using namespace dalm;
 
 // workspace the caller must provide: dalm_b200_topk_ip_workspace(nq, K) bytes
-static int topk_grid_x() { return 2 * kNumSMs; }
+static int topk_grid_x() { return 2 * num_sms(); }
 extern "C" long long dalm_b200_topk_ip_workspace(int nq, int K) {
   return (long long)topk_grid_x() * nq * K * (long long)(sizeof(float) + sizeof(int));
 }
@@ -312,7 +314,7 @@ extern "C" int dalm_b200_topk_ip(const float* Q, const float* P, long long ldp, 
   const size_t smem_pipe = (size_t)(kTopkQT + kTopkPipeWarps * 2 * kTopkR) * D * sizeof(float);
   if (D <= kTopkPipeMaxD && smem_pipe >= smem_m) {
     // pipelined sweep: one CTA per SM (its rings take most of the shared memory), 2 rows per warp step
-    gx = smem_pipe * 2 <= 200 * 1024 ? 2 * kNumSMs : kNumSMs;   // small D: two CTAs per SM keep enough bytes in flight
+    gx = smem_pipe * 2 <= 200 * 1024 ? 2 * num_sms() : num_sms();   // small D: two CTAs per SM keep enough bytes in flight
     const int max_gx = (N + kTopkR * kTopkPipeWarps - 1) / (kTopkR * kTopkPipeWarps);
     if (gx > max_gx) gx = max_gx;
     const size_t smem = smem_pipe;

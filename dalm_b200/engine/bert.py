@@ -7,7 +7,7 @@ FFN(GELU erf) + residual -> LN], eps 1e-12, token_type_ids = 0 (the reference ca
 
 HBM layout (per layer, bf16 unless noted):
   Wqkv_aug [3H, H+Ra]   rows q|k|v of the fused projection; the last Ra=3r columns hold (alpha/r)*B_j so that LoRA's
-                        up-projection is part of the same tcgen05 GEMM (A operand = [x | x A^T])
+                        up-projection is part of the same wgmma GEMM (A operand = [x | x A^T])
   WqkvT_aug [H, 3H+Ra]  resident transpose for dgrad; last Ra columns hold A_j^T
   A_stack [64, H]       LoRA down-projection operand (rows j*r..), zero padded to one 64-row TMA box
   Bblk [64, 3H]         block-diagonal (alpha/r)*B_j^T: g = dQKV . Bblk^T gives all LoRA mid-gradients in one GEMM

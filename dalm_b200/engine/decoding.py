@@ -126,10 +126,9 @@ def greedy_generate(dec, input_ids: Optional[torch.Tensor] = None, attention_mas
             ops.greedy_step_(lg, dec.V, eos_t, pad, unfinished, tokens, kmask, cur_row, next_ids, pos, alive)
 
         graph, replays, eager = None, 0, 0
-        # Measured (profiles/r01_decode_bench.jsonl): a `torch.cuda.graph` capture costs 50-300 ms per call (its entry runs
-        # gc.collect + empty_cache, the private pool is allocated afresh) and a replayed step is only ~0.5-1 ms faster than
-        # the Python launch sequence while the step is GPU-bound (decode attention), so by default only long generations
-        # are captured. DALM_B200_DECODE_GRAPH=1 / 0 forces it.
+        # A `torch.cuda.graph` capture is expensive per call (its entry runs gc.collect + empty_cache, the private pool is
+        # allocated afresh) and a replayed step saves only launch overhead while the step is GPU-bound (decode attention), so
+        # by default only long generations are captured. DALM_B200_DECODE_GRAPH=1 / 0 forces it.
         mode = os.environ.get("DALM_B200_DECODE_GRAPH", "auto")
         lean_capture = mode == "2"                                                # candidate, see _capture_lean
         use_graph = dev.type == "cuda" and ((mode in ("1", "2") and total - col >= 4) or (mode == "auto" and total - col >= GRAPH_MIN_STEPS))

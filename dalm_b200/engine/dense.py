@@ -7,7 +7,7 @@ element offsets:
 
   p32  fp32 master weights  (what Adam updates; biases / norm gains are read by the kernels straight from here)
   g32  fp32 gradients       (weight gradients are written by the wgrad GEMM epilogue, the rest accumulated by atomics)
-  p16  bf16 shadow          (what the tcgen05 GEMMs / embedding gathers read; refreshed by the Adam kernel itself)
+  p16  bf16 shadow          (what the wgmma GEMMs / embedding gathers read; refreshed by the Adam kernel itself)
 
 so the optimizer is one launch and the data-parallel all-reduce one contiguous range per model. Entries of kind "acc"
 (bias, norm and embedding gradients: accumulated with atomics, so they must start from zero) are laid out first; entries of

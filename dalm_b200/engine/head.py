@@ -4,16 +4,15 @@ The reference materialises fp32 logits [B,L,V] and three more copies of them (tr
 per-sample `cat`, the `stack`) — 590 MB each at cfg-3, 9.6 GB each at cfg-5. Here the token rows are processed in
 chunks of whole 128-row GEMM tiles:
 
-    logits_chunk = hf[r0:r1] @ W_head^T          tcgen05 GEMM into a scratch sized for the 126 MB L2
+    logits_chunk = hf[r0:r1] @ W_head^T          wgmma GEMM into a scratch sized for the L2
     ce_rows(logits_chunk)                        log-softmax + gather + mask weights; d(logits) written IN PLACE
     dhf[r0:r1]   = dlogits_chunk @ W_head        head dgrad straight from the same scratch
     dW_head     += dlogits_chunk^T @ hf[r0:r1]   (full fine-tuning only)
 
 so forward, loss and the head's backward are one sweep over the rows; what survives it is tok_lp [B,L] (fp32) and
-dhf [M,H] (bf16). The scratch is re-used by every chunk and, in PEFT mode, sized (74 MB at cfg-3) to fit the 126 MB L2 between
-the three launches that touch it; whatever part of a chunk is evicted anyway costs one extra 74 MB pass, not the reference's
-four [B,L,V] tensors. Measured at cfg-3 the step time is unchanged (131.8 vs 131.4 samples/s, profiles/r02b_bench_ab.jsonl): the
-gain is the memory (0.3 GB at cfg-3, 4.5 GB at cfg-5) and the absence of a V-sized tensor, not time.
+dhf [M,H] (bf16). The scratch is re-used by every chunk and, in PEFT mode, sized to fit the H100's 50 MB L2 between the three
+launches that touch it; whatever part of a chunk is evicted anyway costs one extra pass over the scratch, not the reference's
+four [B,L,V] tensors. The gain is the memory and the absence of a V-sized tensor.
 """
 from __future__ import annotations
 
@@ -26,9 +25,10 @@ from .. import ops
 
 bf16, f32 = torch.bfloat16, torch.float32
 
-# scratch budgets (bytes of bf16 logits per chunk): frozen head -> sized to sit in L2 next to the streaming weight panels;
-# trainable head -> larger chunks, because every chunk's wgrad re-reads and re-writes the fp32 [V,H] gradient
-L2_BUDGET = int(os.environ.get("DALM_B200_HEAD_CHUNK_MB", "80")) << 20
+# scratch budgets (bytes of bf16 logits per chunk): frozen head -> sized to sit in L2 next to the streaming weight panels
+# (24 MB: about half of the H100's 50 MB L2; an estimate, not a measured optimum); trainable head -> larger chunks, because
+# every chunk's wgrad re-reads and re-writes the fp32 [V,H] gradient
+L2_BUDGET = int(os.environ.get("DALM_B200_HEAD_CHUNK_MB", "24")) << 20
 FULL_BUDGET = int(os.environ.get("DALM_B200_HEAD_CHUNK_FULL_MB", "512")) << 20
 
 

@@ -417,7 +417,7 @@ class LlamaDecoder(torch.nn.Module):
                 ops.rope_pos_(a.qkv, 0, self.nh + self.nkv, self.hd, cos_t, sin_t, pos)
             if kv_sink is not None:
                 kv_sink(li, a.qkv)
-            a.att, a.lse = ops.attention_auto_fwd(a.qkv[:, :self.Nq], a.qkv[:, self.Nq:self.Nq + self.Nkv],   # tcgen05/TMEM (head_dim 64 / 128)
+            a.att, a.lse = ops.attention_auto_fwd(a.qkv[:, :self.Nq], a.qkv[:, self.Nq:self.Nq + self.Nkv],
                                                   a.qkv[:, self.Nq + self.Nkv:], ctx.mask, B, L, self.nh, self.nkv, self.hd, causal=True)
             a.x_mid = ops.gemm(a.att, W["Wo"], out_dtype=f32, resid=x)
             a.h2, a.rstd2 = ops.rmsnorm_fwd(a.x_mid, W["g2"], self.eps)
@@ -514,7 +514,7 @@ class LlamaDecoder(torch.nn.Module):
             if bank is not None:
                 ops.wgrad_(dx16, a.act, G(l, "Wd"), acc)
             if bank is None and self.nf4 is None and self.gu_il == 128 and F >= 256 and ops.FUSE_SWIGLU_BWD:
-                ops.gemm_swiglu_bwd_(dx16, W["WdT"], a.gu)                         # d(act) stays in TMEM; gu <- [dgate | dup] in the epilogue
+                ops.gemm_swiglu_bwd_(dx16, W["WdT"], a.gu)                         # d(act) stays on chip; gu <- [dgate | dup] in the epilogue
             else:
                 dact = self._dgrad(dx16, W, "Wd")                                  # [M,F]
                 ops.swiglu_bwd_(a.gu, dact, F, interleave=self.gu_il)              # gu <- [dgate | dup] (same layout as gu)

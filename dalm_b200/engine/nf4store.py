@@ -2,7 +2,7 @@
 
 The reference's `use_bnb` (rag_e2e_base_model.py:136-142) keeps every nn.Linear weight of the sub-model as NF4 codes and
 dequantises it inside each forward (`bnb.matmul_4bit`: dequantize_4bit -> matmul). The default here expands the codes once at
-load time and keeps bf16 copies resident (a B200 has the HBM). This module is the other choice: the base weights stay packed
+load time and keeps bf16 copies resident (an H100 has the HBM for 7B). This module is the other choice: the base weights stay packed
 (0.5625 B per parameter; Llama-2-7B: 3.6 GB instead of 26.5 GB with the dgrad transposes) and one layer's worth of bf16
 scratch is shared by all layers - a weight is expanded right before the GEMM that reads it, forward and backward. The values
 the GEMMs see are bit-identical to the resident mode (csrc/nf4.cu). The backward reads W[out,in] itself as an MN-major operand

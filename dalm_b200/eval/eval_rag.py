@@ -75,7 +75,7 @@ def evaluate_rag(
     retriever_is_autoregressive: bool = False,
 ) -> EvalResults:
     if not str(device).startswith("cuda"):
-        raise RuntimeError("dalm_b200 evaluates on a CUDA (sm_100a) device only: there is no CPU path")
+        raise RuntimeError("dalm_b200 evaluates on a CUDA (sm_90a) device only: there is no CPU path")
     test_dataset = load_dataset(dataset_or_path)
     selected_torch_dtype: Final[torch.dtype] = torch.float16 if torch_dtype == "float16" else torch.bfloat16
     with inference_only():
@@ -148,7 +148,7 @@ _FLAGS = [
 
 def parse_args() -> Namespace:
     from ..training.utils.loop import build_parser
-    return build_parser("RAG evaluation: retrieval metrics + greedy generation / exact match (B200-native)", _FLAGS).parse_args()
+    return build_parser("RAG evaluation: retrieval metrics + greedy generation / exact match (H100-native)", _FLAGS).parse_args()
 
 
 def main() -> None:

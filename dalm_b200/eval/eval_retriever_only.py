@@ -38,7 +38,7 @@ _FLAGS = [
 
 def parse_args() -> Namespace:
     from ..training.utils.loop import build_parser
-    return build_parser("Retriever evaluation: exact top-k search over the passage embeddings (B200-native)", _FLAGS).parse_args()
+    return build_parser("Retriever evaluation: exact top-k search over the passage embeddings (H100-native)", _FLAGS).parse_args()
 
 
 def evaluate_retriever(
@@ -58,7 +58,7 @@ def evaluate_retriever(
     """reference :105-178. `device` must be a CUDA device (no CPU path); `torch_dtype` is accepted for signature parity —
     the forward always runs bf16 GEMMs with fp32 pooling."""
     if not str(device).startswith("cuda"):
-        raise RuntimeError("dalm_b200 evaluates on a CUDA (sm_100a) device only: there is no CPU path")
+        raise RuntimeError("dalm_b200 evaluates on a CUDA (sm_90a) device only: there is no CPU path")
     test_dataset = load_dataset(dataset_or_path)
     selected_torch_dtype: Final[torch.dtype] = torch.float16 if torch_dtype == "float16" else torch.bfloat16
     with inference_only():

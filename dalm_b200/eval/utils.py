@@ -3,7 +3,7 @@
 The one semantic change: the reference builds an APPROXIMATE hnswlib index (space "ip", M=100, ef_construction=200, ef=100,
 dalm/eval/utils.py:18-55) on the host; here `construct_search_index` keeps the passage embeddings resident in HBM and
 `get_nearest_neighbours` runs an EXACT inner-product top-k sweep over them (csrc/topk.cu: one pass over 200k x 1024 fp32 is
-819 MB, ~125 us at HBM speed). Exact search is the limit hnswlib approximates, so recall / precision / hit-rate computed
+819 MB, about 0.25 ms at the H100's 3.35 TB/s data-sheet bandwidth). Exact search is the limit hnswlib approximates, so recall / precision / hit-rate computed
 from it are >= the reference's for the same embeddings.
 """
 from __future__ import annotations

@@ -1,6 +1,6 @@
-"""B200-native `AutoModelForRagE2E` — same constructor, attributes and methods as the reference wrapper
+"""H100-native `AutoModelForRagE2E` — same constructor, attributes and methods as the reference wrapper
 (dalm/models/rag_e2e_base_model.py:16-160), with the HF/PEFT modules behind it replaced by the dalm_b200 engine
-(hand-written sm_100a kernels through the C ABI). There is no CPU or eager-PyTorch fallback.
+(hand-written sm_90a kernels through the C ABI). There is no CPU or eager-PyTorch fallback.
 """
 from __future__ import annotations
 
@@ -52,7 +52,7 @@ def _want_full(lora: bool) -> bool:
 
 def _device() -> torch.device:
     if not torch.cuda.is_available():
-        raise RuntimeError("dalm_b200 needs a CUDA (sm_100a) device: there is no CPU path for the training step")
+        raise RuntimeError("dalm_b200 needs a CUDA (sm_90a) device: there is no CPU path for the training step")
     return torch.device("cuda", int(os.environ.get("LOCAL_RANK", torch.cuda.current_device())))
 
 

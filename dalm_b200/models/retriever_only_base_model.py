@@ -1,4 +1,4 @@
-"""B200-native `AutoModelForSentenceEmbedding` (reference dalm/models/retriever_only_base_model.py:10-110)."""
+"""H100-native `AutoModelForSentenceEmbedding` (reference dalm/models/retriever_only_base_model.py:10-110)."""
 from __future__ import annotations
 
 import logging

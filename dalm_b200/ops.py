@@ -130,10 +130,18 @@ def ce_marginal_rows_(chunk: torch.Tensor, ids: torch.Tensor, mask: torch.Tensor
               _p(mask), _p(nsum), _p(tok_lp), B, L, int(V), chunk.stride(0), float(grad_out), int(row0), chunk.shape[0], _stream())
 
 
-def head_chunk_rows(M: int, Vp: int, budget_bytes: int, tile_n: int = 256, sms: int = 148) -> int:
+def num_sms() -> int:
+    """SM count of the current CUDA device (what the persistent GEMM grids are sized to)"""
+    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+
+
+def head_chunk_rows(M: int, Vp: int, budget_bytes: int, tile_n: int = 256, sms: Optional[int] = None) -> int:
     """Row-chunk height of the chunked lm_head + CE pass: the largest split into equal, 128-row-aligned chunks whose bf16
     logits scratch [rows, Vp] stays within `budget_bytes`, choosing among the next few chunk counts the one whose GEMMs
-    waste the fewest tile waves on `sms` persistent CTAs (a chunk of m x n tiles costs ceil(m n / sms) waves)."""
+    waste the fewest tile waves on `sms` persistent CTAs (a chunk of m x n tiles costs ceil(m n / sms) waves; default: the
+    current device's SM count)."""
+    if sms is None:
+        sms = num_sms()
     m_tiles = (M + 127) // 128
     n_tiles = (Vp + tile_n - 1) // tile_n
     max_rows = max(128, budget_bytes // (2 * Vp) // 128 * 128)
@@ -261,17 +269,15 @@ class GemmTimer:
 GEMM_TIMER = None
 # Persistent-GEMM grid cap (0 = one CTA per SM). accel.GradientSync lowers it while collectives overlap the backward (full
 # fine-tuning on > 1 rank): the GEMM walks its tiles with a static stride of gridDim, so a CTA that cannot be scheduled because
-# NCCL's kernels hold its SM would run ALL of its tiles after the others finished - measured at N=2: GEMMs at 813 instead of
-# 1164 TFLOP/s, the overlap bought nothing (profiles/r02_bench_cfg3_fullft_n2.json). Leaving NCCL its SMs keeps the wave intact.
+# NCCL's kernels hold its SM would run ALL of its tiles after the others finished, and the overlap would buy nothing. Leaving
+# NCCL its SMs keeps the wave intact.
 GEMM_MAX_CTAS = 0
 
 
 # ----------------------------------------------------------------------------------------------------------------
 # attention
 # ----------------------------------------------------------------------------------------------------------------
-def attention_fwd(q, k, v, mask, B: int, L: int, Hq: int, Hkv: int, D: int, causal: bool, out=None,
-                  scale: Optional[float] = None, drop: Optional[Drop] = None):
-    """q/k/v: bf16 token-major 2-D views [B*L, H*D] (may be column slices of one qkv buffer). -> (out, lse)"""
+def _attention_fwd(sym, q, k, v, mask, B, L, Hq, Hkv, D, causal, out, scale, drop):
     for t, n in ((q, "q"), (k, "k"), (v, "v")):
         _chk(t, bf16, n)
     if out is None:
@@ -280,76 +286,60 @@ def attention_fwd(q, k, v, mask, B: int, L: int, Hq: int, Hkv: int, D: int, caus
     if mask is not None and mask.dtype != i64:
         raise _lib.DalmB200Error("attention: mask must be int64")
     scale = 1.0 / math.sqrt(D) if scale is None else scale
-    _lib.call("dalm_b200_attention_fwd", _p(q), _ld(q), _p(k), _ld(k), _p(v), _ld(v), _p(mask), _p(out), _ld(out),
+    _lib.call(sym, _p(q), _ld(q), _p(k), _ld(k), _p(v), _ld(v), _p(mask), _p(out), _ld(out),
               _p(lse), B, L, Hq, Hkv, D, float(scale), 1 if causal else 0, *_d(drop), _stream())
     return out, lse
 
 
-def attention_tc_fwd(q, k, v, mask, B: int, L: int, Hq: int, Hkv: int, D: int, causal: bool, out=None,
-                     scale: Optional[float] = None, drop: Optional[Drop] = None):
-    """tcgen05/TMEM attention forward (head_dim 128 or 64; probability dropout at 64). Same contract as attention_fwd."""
-    for t, n in ((q, "q"), (k, "k"), (v, "v")):
-        _chk(t, bf16, n)
-    if out is None:
-        out = torch.empty(B * L, Hq * D, dtype=bf16, device=q.device)
-    lse = torch.empty(B, Hq, L, dtype=f32, device=q.device)
-    if mask is not None and mask.dtype != i64:
-        raise _lib.DalmB200Error("attention: mask must be int64")
-    scale = 1.0 / math.sqrt(D) if scale is None else scale
-    _lib.call("dalm_b200_attention_tc_fwd", _p(q), _ld(q), q.shape[1], 0, _p(k), _ld(k), k.shape[1], 0, _p(v), _ld(v), v.shape[1], 0,
-              _p(mask), _p(out), _ld(out), _p(lse), B, L, Hq, Hkv, D, float(scale), 1 if causal else 0, *_d(drop), _stream())
-    return out, lse
-
-
-_ATTN_MODE_SET = False
-
-
-def attention_tc_bwd(q, k, v, mask, out, lse, d_out, B: int, L: int, Hq: int, Hkv: int, D: int, causal: bool,
-                     dq=None, dk=None, dv=None, scale: Optional[float] = None, drop: Optional[Drop] = None):
-    """tcgen05/TMEM attention backward (head_dim 128 or 64). Same contract as attention_bwd."""
-    global _ATTN_MODE_SET
-    if not _ATTN_MODE_SET:                                     # A/B switch: DALM_B200_ATTN_BWD_PIPE=0 -> the one-chain-per-CTA kernels
-        _ATTN_MODE_SET = True
-        if os.environ.get("DALM_B200_ATTN_BWD_PIPE", "1") == "0":
-            _lib.load().dalm_b200_attention_tc_set_mode(0)
-    dev = q.device
-    if dq is None: dq = torch.empty(B * L, Hq * D, dtype=bf16, device=dev)
-    if dk is None: dk = torch.empty(B * L, Hkv * D, dtype=bf16, device=dev)
-    if dv is None: dv = torch.empty(B * L, Hkv * D, dtype=bf16, device=dev)
-    delta = torch.empty(2, B, Hq, (L + 63) // 64 * 64, dtype=f32, device=dev)      # workspace: rowsum(dO*O) and -lse*log2e, rows padded to 64
-    scale = 1.0 / math.sqrt(D) if scale is None else scale
-    _lib.call("dalm_b200_attention_tc_bwd", _p(q), _ld(q), q.shape[1], _p(k), _ld(k), k.shape[1], _p(v), _ld(v), v.shape[1],
-              _p(mask), _p(out), _ld(out), _p(lse), _p(d_out), _ld(d_out), d_out.shape[1], _p(delta), _p(dq), _ld(dq),
-              _p(dk), _ld(dk), _p(dv), _ld(dv), B, L, Hq, Hkv, D, float(scale), 1 if causal else 0, *_d(drop), _stream())
-    return dq, dk, dv
-
-
-def attention_auto_fwd(q, k, v, mask, B, L, Hq, Hkv, D, causal, out=None, scale=None, drop=None):
-    """head_dim 64 / 128 -> tcgen05 kernels (csrc/attention_tc.cu); head_dim 32 (bge-small) -> mma.sync kernels.
-    DALM_B200_ATTN_TC=0 forces the mma.sync path (cross-checks)."""
-    if D in (64, 128) and os.environ.get("DALM_B200_ATTN_TC", "1") != "0":
-        return attention_tc_fwd(q, k, v, mask, B, L, Hq, Hkv, D, causal, out=out, scale=scale, drop=drop)
-    return attention_fwd(q, k, v, mask, B, L, Hq, Hkv, D, causal, out=out, scale=scale, drop=drop)
-
-
-def attention_auto_bwd(q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq=None, dk=None, dv=None, scale=None, drop=None):
-    if D in (64, 128) and os.environ.get("DALM_B200_ATTN_TC", "1") != "0":
-        return attention_tc_bwd(q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq=dq, dk=dk, dv=dv, scale=scale, drop=drop)
-    return attention_bwd(q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq=dq, dk=dk, dv=dv, scale=scale, drop=drop)
-
-
-def attention_bwd(q, k, v, mask, out, lse, d_out, B: int, L: int, Hq: int, Hkv: int, D: int, causal: bool,
-                  dq=None, dk=None, dv=None, scale: Optional[float] = None, drop: Optional[Drop] = None):
+def _attention_bwd(sym, q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq, dk, dv, scale, drop):
     dev = q.device
     if dq is None: dq = torch.empty(B * L, Hq * D, dtype=bf16, device=dev)
     if dk is None: dk = torch.empty(B * L, Hkv * D, dtype=bf16, device=dev)
     if dv is None: dv = torch.empty(B * L, Hkv * D, dtype=bf16, device=dev)
     delta = torch.empty(B, Hq, L, dtype=f32, device=dev)
     scale = 1.0 / math.sqrt(D) if scale is None else scale
-    _lib.call("dalm_b200_attention_bwd", _p(q), _ld(q), _p(k), _ld(k), _p(v), _ld(v), _p(mask), _p(out), _ld(out),
+    _lib.call(sym, _p(q), _ld(q), _p(k), _ld(k), _p(v), _ld(v), _p(mask), _p(out), _ld(out),
               _p(lse), _p(d_out), _ld(d_out), _p(delta), _p(dq), _ld(dq), _p(dk), _ld(dk), _p(dv), _ld(dv),
               B, L, Hq, Hkv, D, float(scale), 1 if causal else 0, *_d(drop), _stream())
     return dq, dk, dv
+
+
+def attention_fwd(q, k, v, mask, B: int, L: int, Hq: int, Hkv: int, D: int, causal: bool, out=None,
+                  scale: Optional[float] = None, drop: Optional[Drop] = None):
+    """mma.sync attention forward (head_dim 32/64/128). q/k/v: bf16 token-major 2-D views [B*L, H*D] (may be column slices
+    of one qkv buffer). -> (out, lse)"""
+    return _attention_fwd("dalm_b200_attention_fwd", q, k, v, mask, B, L, Hq, Hkv, D, causal, out, scale, drop)
+
+
+def attention_bwd(q, k, v, mask, out, lse, d_out, B: int, L: int, Hq: int, Hkv: int, D: int, causal: bool,
+                  dq=None, dk=None, dv=None, scale: Optional[float] = None, drop: Optional[Drop] = None):
+    """mma.sync attention backward. -> (dq, dk, dv)"""
+    return _attention_bwd("dalm_b200_attention_bwd", q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq, dk, dv, scale, drop)
+
+
+def attention_tc_fwd(q, k, v, mask, B: int, L: int, Hq: int, Hkv: int, D: int, causal: bool, out=None,
+                     scale: Optional[float] = None, drop: Optional[Drop] = None):
+    """wgmma/TMA attention forward (head_dim 128 or 64; probability dropout at 64). Same contract as attention_fwd."""
+    return _attention_fwd("dalm_b200_attention_tc_fwd", q, k, v, mask, B, L, Hq, Hkv, D, causal, out, scale, drop)
+
+
+def attention_tc_bwd(q, k, v, mask, out, lse, d_out, B: int, L: int, Hq: int, Hkv: int, D: int, causal: bool,
+                     dq=None, dk=None, dv=None, scale: Optional[float] = None, drop: Optional[Drop] = None):
+    """wgmma/TMA attention backward (head_dim 128 or 64). Same contract as attention_bwd."""
+    return _attention_bwd("dalm_b200_attention_tc_bwd", q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq, dk, dv, scale, drop)
+
+
+def attention_auto_fwd(q, k, v, mask, B, L, Hq, Hkv, D, causal, out=None, scale=None, drop=None):
+    """head_dim 64 / 128 -> wgmma kernels; head_dim 32 (bge-small) -> mma.sync kernels."""
+    if D in (64, 128):
+        return attention_tc_fwd(q, k, v, mask, B, L, Hq, Hkv, D, causal, out=out, scale=scale, drop=drop)
+    return attention_fwd(q, k, v, mask, B, L, Hq, Hkv, D, causal, out=out, scale=scale, drop=drop)
+
+
+def attention_auto_bwd(q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq=None, dk=None, dv=None, scale=None, drop=None):
+    if D in (64, 128):
+        return attention_tc_bwd(q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq=dq, dk=dk, dv=dv, scale=scale, drop=drop)
+    return attention_bwd(q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq=dq, dk=dk, dv=dv, scale=scale, drop=drop)
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -467,9 +457,8 @@ def gemm_swiglu(a: torch.Tensor, w_il: torch.Tensor, gu: Optional[torch.Tensor] 
 
 
 # GELU in the GEMM epilogues pays only when the tile's mainloop is long enough to hide the erf / exp work of the 256 epilogue
-# threads: measured at cfg-2 (bge-large, K = 1024: 16 k-blocks per tile) the fused launches cost 10.6 ms more GEMM time than the
-# 7.1 ms of stand-alone gelu kernels they remove (profiles/r02b_bench_ab.jsonl) - so the fusion is taken from K >= 2048 (Falcon's
-# 4544-wide MLP), and BERT keeps the separate kernels. DALM_B200_FUSE_GELU_MIN_K overrides (0 = always, huge = never).
+# threads, so the fusion is taken from K >= 2048 (Falcon's 4544-wide MLP) and BERT (K = 1024: 16 k-blocks per tile) keeps the
+# separate kernels. The threshold was chosen on the previous (Blackwell) kernels and has not been re-measured on H100. DALM_B200_FUSE_GELU_MIN_K overrides (0 = always, huge = never).
 FUSE_GELU_MIN_K = int(os.environ.get("DALM_B200_FUSE_GELU_MIN_K", "2048"))
 
 
@@ -477,8 +466,8 @@ def fuse_gelu(K: int) -> bool:
     return K >= FUSE_GELU_MIN_K
 
 
-# measured (profiles/r02b_fusion_probe.jsonl): fused 466 us vs 382 us for the dgrad GEMM + swiglu_bwd kernel at the Llama-2-7B shape - the
-# epilogue's per-thread row loads of gate / up (32 lines per warp instruction) cost more than the stand-alone pass. Opt-in only.
+# the epilogue's per-thread row loads of gate / up (32 lines per warp instruction) cost more than the stand-alone swiglu_bwd pass
+# on the previous (Blackwell) kernels; not re-measured on H100. Opt-in only.
 FUSE_SWIGLU_BWD = os.environ.get("DALM_B200_FUSE_SWIGLU_BWD", "0") == "1"
 
 
@@ -647,7 +636,7 @@ def cast_f32_bf16(src, dst=None):
 
 
 def wgrad_(dy, x, gw, accumulate: bool, K: Optional[int] = None) -> None:
-    """gw[out,in] (fp32) = (or +=) dy[T,out]^T @ x[T,in]: the weight gradient of y = x W^T as one tcgen05 GEMM contracting
+    """gw[out,in] (fp32) = (or +=) dy[T,out]^T @ x[T,in]: the weight gradient of y = x W^T as one wgmma GEMM contracting
     over the token rows (both operands read MN-major from their row-major buffers)"""
     gemm(dy, x, out=gw, layout=2, resid=gw if accumulate else None, K=K)
 
@@ -772,7 +761,7 @@ def decode_gemm(a: torch.Tensor, w: torch.Tensor, out: Optional[torch.Tensor] = 
 
 
 def gemm_rows(a: torch.Tensor, w: torch.Tensor, *, out_dtype=bf16, act: int = 0, resid: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """a[M,K] @ w[N,K]^T for a decode step: up to 16 rows go through the weight-streaming `decode_gemm` (the 128-row tcgen05
+    """a[M,K] @ w[N,K]^T for a decode step: up to 16 rows go through the weight-streaming `decode_gemm` (the 128-row wgmma
     tile would be 7/8 empty), larger batches through the training GEMM. DALM_B200_DECODE_GEMM=0 forces the latter."""
     if a.shape[0] <= 16 and os.environ.get("DALM_B200_DECODE_GEMM", "1") != "0":
         return decode_gemm(a, w, out_dtype=out_dtype, act=act, resid=resid)

@@ -53,7 +53,7 @@ _FLAGS = [
 
 
 def parse_args() -> Namespace:
-    return build_parser("RAG end-to-end training (B200-native)", _FLAGS).parse_args()
+    return build_parser("RAG end-to-end training (H100-native)", _FLAGS).parse_args()
 
 
 def _save_final(tokenizers):

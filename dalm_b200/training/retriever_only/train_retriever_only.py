@@ -44,7 +44,7 @@ _FLAGS = [
 
 
 def parse_args() -> Namespace:
-    return build_parser("contrastive retriever training (B200-native)", _FLAGS).parse_args()
+    return build_parser("contrastive retriever training (H100-native)", _FLAGS).parse_args()
 
 
 def train_retriever(

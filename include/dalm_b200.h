@@ -1,4 +1,4 @@
-/* dalm_b200 — C ABI of the B200-native RAG-e2e / retriever-only training-step kernels.
+/* dalm_b200 — C ABI of the H100-native (sm_90a) RAG-e2e / retriever-only training-step kernels.
  *
  * The reference (arcee-ai/DALM) has no FFI: its hot path is Python calling PyTorch/HF/PEFT library kernels. Each entry
  * point below cites the reference call site whose library work it replaces (paths relative to the reference root).
@@ -19,7 +19,7 @@ const char* dalm_b200_last_error(void);
 const char* dalm_b200_version(void);
 long long   dalm_b200_launch_count(void);          /* kernels launched by this library since the last reset */
 void        dalm_b200_reset_launch_count(void);
-int         dalm_b200_probe_device(void);          /* 0 iff the current device is sm_100 */
+int         dalm_b200_probe_device(void);          /* 0 iff the current device is sm_90 (H100) */
 
 /* ---- loss path ----
  * marginal_counts: c_b / N of marginalize_log_probs + the mask normaliser
@@ -69,7 +69,7 @@ int dalm_b200_lora_dx(void* dh, long long lddh, const void* G, long long ldg, co
                       int R, float p, unsigned long long seed, unsigned long long stream_id, const void* offset,
                       void* stream);
 
-/* ---- dense contractions (tcgen05 / TMEM / TMA) ----
+/* ---- dense contractions (wgmma / TMA) ----
  * out[M,N] = act(alpha * A[M,K] B[N,K]^T + bias) + resid. Replaces every nn.Linear forward / dgrad reached through
  * dalm/models/rag_e2e_base_model.py:93,105 and dalm/models/retriever_only_base_model.py:58 (HF modeling code -> cuBLAS). */
 int dalm_b200_gemm_bf16_tn(const void* A, long long lda, const void* B, long long ldb, void* out, long long ldo,
@@ -96,7 +96,7 @@ int dalm_b200_gemm_bf16_swiglu(const void* A, long long lda, const void* B, long
 int dalm_b200_gemm_bf16_rope(const void* A, long long lda, const void* B, long long ldb, void* out, long long ldo, int M, int N,
                              int K, const float* cos_t, const float* sin_t, int L, int rope_cols, void* stream);
 /* gemm_bf16_swiglu_bwd: LlamaMLP backward through down_proj and act_fn(gate) * up in one launch: d(act)[M,F] = dY[M,K] WdT[F,K]^T
- * stays in TMEM; gu [M,2F] (gate|up interleaved in 128-feature blocks, as gemm_bf16_swiglu left it) is overwritten in place with
+ * never reaches HBM; gu [M,2F] (gate|up interleaved in 128-feature blocks, as gemm_bf16_swiglu left it) is overwritten in place with
  * [d gate | d up]. Bit-identical to gemm_bf16 followed by swiglu_bwd (interleave 128). */
 int dalm_b200_gemm_bf16_swiglu_bwd(const void* dY, long long lddy, const void* WdT, long long ldw, void* gu, long long ldgu, int M,
                                    int F, int K, void* stream);
@@ -126,28 +126,17 @@ int dalm_b200_attention_bwd(const void* q, long long ldq, const void* k, long lo
                             long long lddv, int B, int L, int Hq, int Hkv, int D, float scale, int causal, float drop_p, unsigned long long drop_seed,
     unsigned long long drop_stream_id, const void* drop_offset, void* stream);
 
-/* tcgen05 / TMEM / TMA attention: head_dim 128 (Llama decoder) or 64 (bge-large encoder incl. attention-probability dropout;
- * Falcon MQA decoder). q/k/v are bf16 token-major matrices [B*L, *cols] with row stride ld*; head h starts at column
- * *col0 + h*D. Same outputs, mask semantics and dropout element indexing as dalm_b200_attention_fwd / _bwd (the mma.sync
- * kernels, kept for head_dim 32 and as a cross-check). */
-int dalm_b200_attention_tc_fwd(const void* q, long long ldq, long long qcols, int qcol0, const void* k, long long ldk,
-                               long long kcols, int kcol0, const void* v, long long ldv, long long vcols, int vcol0,
+/* wgmma / TMA attention (Hopper tensor cores): head_dim 128 (Llama decoder) or 64 (bge-large encoder incl.
+ * attention-probability dropout; Falcon MQA decoder). Same arguments, outputs, mask semantics and dropout element indexing
+ * as dalm_b200_attention_fwd / _bwd (the mma.sync kernels, kept for head_dim 32 and as a cross-check). */
+int dalm_b200_attention_tc_fwd(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv,
                                const int64_t* mask, void* out, long long ldo, float* lse, int B, int L, int Hq, int Hkv,
                                int D, float scale, int causal, float drop_p, unsigned long long drop_seed,
                                unsigned long long drop_stream_id, const void* drop_offset, void* stream);
-
-/* attention_tc_bwd's `delta` is a caller-provided fp32 WORKSPACE of 2 * B * Hq * Lp floats, Lp = L rounded up to a multiple
- * of 64 (rowsum(dO*O) and -lse*log2(e) per query, padded rows). */
-/* backward kernel selection (test / tuning hook): 1 = pipelined persistent dKdV / dQ kernels (default), 0 = the
- * one-chain-per-CTA kernels they replaced (kept as an independent cross-check) */
-void dalm_b200_attention_tc_set_mode(int pipelined_backward);
-/* tuning aid: a device buffer of 64 int64 receives clock64 phase timestamps of one forward CTA (NULL disables) */
-void dalm_b200_attention_tc_set_debug(void* dev_buffer_64xint64);
-int dalm_b200_attention_tc_bwd(const void* q, long long ldq, long long qcols, const void* k, long long ldk, long long kcols,
-                               const void* v, long long ldv, long long vcols, const int64_t* mask, const void* out,
-                               long long ldo, const float* lse, const void* d_out, long long lddo, long long docols,
-                               float* delta, void* dq, long long lddq, void* dk, long long lddk, void* dv, long long lddv,
-                               int B, int L, int Hq, int Hkv, int D, float scale, int causal, float drop_p,
+int dalm_b200_attention_tc_bwd(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv,
+                               const int64_t* mask, const void* out, long long ldo, const float* lse, const void* d_out,
+                               long long lddo, float* delta, void* dq, long long lddq, void* dk, long long lddk, void* dv,
+                               long long lddv, int B, int L, int Hq, int Hkv, int D, float scale, int causal, float drop_p,
                                unsigned long long drop_seed, unsigned long long drop_stream_id, const void* drop_offset,
                                void* stream);
 

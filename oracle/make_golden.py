@@ -144,6 +144,27 @@ def gen_eval_helpers(ref):
         json.dump(out, f)
 
 
+def gen_live_checks(ref):
+    """the reference's outputs for the fixed inputs of tests/test_oracle_golden.py::test_live_reference_if_present and
+    tests/test_eval_host.py::test_live_reference_helpers_if_present (inputs rebuilt from the same seed / literals there)"""
+    g = torch.Generator().manual_seed(123)
+    B, L, V, D = 6, 10, 31, 24
+    q = torch.nn.functional.normalize(torch.randn(B, D, generator=g), dim=1)
+    p = torch.nn.functional.normalize(torch.randn(B, D, generator=g), dim=1)
+    lg = torch.randn(B, L, V, generator=g); ids = torch.randint(0, V, (B, L), generator=g)
+    mask = torch.ones(B, L, dtype=torch.int64); mask[2, :4] = 0; mask[4, 7:] = 0
+    ql = torch.tensor([1, 2, 9, 10, 12, 5])
+    S = ref.train_utils.get_cosine_sim(q, p, 100)
+    loss = ref.train_utils.compute_marginalized_loss_from_logits(lg, ids, mask, S, ql)
+    eu = ref.eval_utils
+    pr = [list(eu.calculate_precision_recall(r, c)) for r, c in ((["a", "b"], ["b"]), (["k"] * 4, ["k"]), (["m", "n", "o"], ["z"]))]
+    res = eu.calc_eval_results(5, [0.1] * 5, [1, 0, 1, 1, 0], 3)
+    out = {"marginalized_loss": loss.double().tolist(), "marginalized_loss_hex": float(loss).hex(),
+           "precision_recall": pr, "calc_eval_results": res.model_dump() if hasattr(res, "model_dump") else res.dict()}
+    with open(os.path.join(GOLD, "live_reference.json"), "w") as f:
+        json.dump(out, f)
+
+
 def main():
     from oracle import ref_import
 
@@ -153,6 +174,7 @@ def main():
     gen_pooling(ref)
     gen_preprocess(ref)
     gen_eval_helpers(ref)
+    gen_live_checks(ref)
     print("golden fixtures written to", GOLD)
 
 

@@ -134,7 +134,7 @@ def retriever_step(bert: nn.Module, batch: Dict[str, torch.Tensor], logit_scale:
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# timing support for bench.py's baselines (cpu_baseline / --impl reference on host cores, gpu_eager_baseline on the B200):
+# timing support for bench.py's baselines (cpu_baseline / --impl reference on host cores, gpu_eager_baseline on the GPU):
 # the SAME modules as above, built without the minutes-long HF random initialisation of a 7 B model
 # ----------------------------------------------------------------------------------------------------------------
 def build_for_timing(kind: str, cfg: Dict, device="cpu", seed: int = 0) -> nn.Module:

@@ -29,14 +29,14 @@ def test_library_builds_and_exports_header_symbols():
         assert n in exported, f"{n} declared in the header but not exported"
         assert hasattr(lib, n)
     assert set(_lib.SIGNATURES) == set(names), set(_lib.SIGNATURES) ^ set(names)
-    assert "sm_100a" in _lib.version()
+    assert "sm_90a" in _lib.version()
 
 
-def test_sass_is_blackwell_native():
-    """tcgen05 / TMA must really be in the binary (UTCHMMA / UTMALDG / LDTM), not a recompiled legacy path"""
+def test_sass_is_hopper_native():
+    """wgmma / TMA must really be in the binary (HGMMA / UTMALDG / UTMASTG), not a recompiled legacy path"""
     from dalm_b200 import _lib
     sass = subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True).stdout
-    for mnemonic in ("UTCHMMA", "UTMALDG", "LDTM"):
+    for mnemonic in ("HGMMA", "UTMALDG", "UTMASTG"):
         assert mnemonic in sass, mnemonic
 
 

@@ -1,4 +1,4 @@
-"""-m gpu: tcgen05/TMEM attention (head_dim 128) against the fp64 torch reference and the mma.sync kernels."""
+"""-m gpu: wgmma/TMA attention (head_dim 128 and 64) against the fp64 torch reference and the mma.sync kernels."""
 import math
 
 import pytest
@@ -215,37 +215,3 @@ def test_attention_tc_head_dim_64_speed_report(cuda_dev, capsys):
                     "bwd_mma_us": t(lambda: ops.attention_bwd(q, k, v, mask, out, lse, do, B, L, Hq, Hkv, D, causal, dq=dq, dk=dk, dv=dv, drop=d))}
     with capsys.disabled():
         print("\nATTN_TC64_TIMING", res)
-
-
-@pytest.mark.parametrize("B,L,Hq,Hkv,D,causal,pad,p_drop", [
-    (3, 200, 4, 4, 128, True, "right", 0.0), (2, 96, 4, 4, 128, True, "left", 0.0), (2, 200, 2, 2, 64, False, "right", 0.1),
-    (5, 50, 16, 16, 64, False, "right", 0.1), (2, 300, 7, 1, 64, True, "left", 0.0), (1, 520, 4, 2, 64, True, "right", 0.0),
-])
-def test_attention_tc_backward_pipelined_vs_single_chain_kernels(cuda_dev, B, L, Hq, Hkv, D, causal, pad, p_drop):
-    """the pipelined persistent backward (default) and the one-chain-per-CTA kernels it replaced are two independent
-    implementations of the same tiles: identical masks and dropout bits, P / dS rounded to bf16 at the same point - they may
-    differ only by where the softmax scale is applied (before vs after the bf16 rounding of dS)"""
-    from dalm_b200 import _lib, ops
-    torch.manual_seed(L + D)
-    dev = cuda_dev
-    wide = (Hq + 2 * Hkv) * D
-    qkv = torch.randn(B * L, wide, device=dev).to(bf16)
-    q, k, v = qkv[:, :Hq * D], qkv[:, Hq * D:(Hq + Hkv) * D], qkv[:, (Hq + Hkv) * D:]
-    mask = torch.ones(B, L, dtype=torch.int64, device=dev)
-    if pad == "right":
-        for b in range(B): mask[b, L - 3 - (5 * b) % (L // 2):] = 0
-    else:
-        for b in range(B): mask[b, :4 + 3 * b] = 0
-    d = ops.Drop(p_drop, 9, 77, None) if p_drop > 0 else None
-    out, lse = ops.attention_tc_fwd(q, k, v, mask, B, L, Hq, Hkv, D, causal, drop=d)
-    d_out = torch.randn(B * L, Hq * D, device=dev).to(bf16)
-    lib = _lib.load()
-    res = {}
-    try:
-        for mode in (1, 0):
-            lib.dalm_b200_attention_tc_set_mode(mode)
-            res[mode] = [t.float() for t in ops.attention_tc_bwd(q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, drop=d)]
-    finally:
-        lib.dalm_b200_attention_tc_set_mode(1)
-    for a, b_ in zip(res[1], res[0]):
-        assert torch.isfinite(a).all() and _rel(a, b_) < 6e-3

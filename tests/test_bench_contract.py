@@ -1,6 +1,5 @@
 """CPU: the parts of bench.py's contract that do not need a GPU — rank-strided batches (accelerate order, the N>1 arm),
-the reference arm's JSON line (same metric / unit / workload as the B200 arm, rank 0 only), `roofline.traffic` read from the
-committed ncu capture."""
+the reference arm's JSON line (same metric / unit / workload as the GPU arm, rank 0 only)."""
 import json
 import os
 import sys
@@ -57,14 +56,4 @@ def test_reference_arm_line(monkeypatch, capsys, tmp_path):
     assert line["value"] == 0.25 and line["cpu_baseline"] == {"value": 0.25, "unit": "samples/s", "cores": 8, "kind": "port", "sample": "stubbed sample"}
     assert line["e2e"] == {"value": 0.25, "unit": "samples/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}
     args = bench.parse()
-    assert line["config"]["workload"] == bench.workload_name(args)   # the same workload name as the B200 arm prints
-
-
-def test_roofline_traffic_from_committed_capture():
-    import bench
-    traffic, detail = bench.ncu_traffic()
-    assert detail["source"].startswith("profiles/r0") and detail["source"].endswith("_ncu_full_raw.csv") and detail["launches"] == 4
-    assert os.path.exists(os.path.join(ROOT, detail["source"]))      # a committed capture, newest first (bench.ncu_traffic)
-    assert traffic == pytest.approx(sum(detail["dram_bytes_per_launch"]) / 4) and 2e8 < traffic < 7e8
-    for dram, algo in zip(detail["dram_bytes_per_launch"], detail["algorithmic_bytes_per_launch"]):
-        assert dram > 0.90 * algo        # DRAM bytes sit at or above the algorithmic minimum (a little of A may already be in L2)
+    assert line["config"]["workload"] == bench.workload_name(args)   # the same workload name as the GPU arm prints

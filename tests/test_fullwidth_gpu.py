@@ -62,8 +62,8 @@ def _rag_batch(B, Lq, Lp, Lg, vb, vl, seed):
 # cfg-3 / cfg-4: bge-large-en + Llama-2-7b-hf + PEFT(both), B 18, Lq 50 / Lp 128 / Lg 256 — the whole fused step
 # ----------------------------------------------------------------------------------------------------------------
 def test_cfg3_step_at_full_width(cuda_dev):
-    """2 encoder layers + 1 decoder layer at the real widths through `fused_rag_step` (tcgen05 GEMMs incl. the K-augmented
-    QKV projection and the 32000-wide lm_head, tcgen05 attention at (18, 256, 32 x 128), the 32000-wide CE, the fused
+    """2 encoder layers + 1 decoder layer at the real widths through `fused_rag_step` (wgmma GEMMs incl. the K-augmented
+    QKV projection and the 32000-wide lm_head, wgmma attention at (18, 256, 32 x 128), the 32000-wide CE, the fused
     in-batch loss) vs the oracle's loop body (reference train_rage2e.py:431-471)."""
     from dalm_b200 import ops, synthetic
     from dalm_b200.engine import params
@@ -221,7 +221,7 @@ def test_cfg5_falcon_full_finetune_grads_at_full_width(cuda_dev):
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# tcgen05 attention at the cfg-3 decoder shape against fp64 (not against the repo's own mma.sync kernel)
+# wgmma attention at the cfg-3 decoder shape against fp64 (not against the repo's own mma.sync kernel)
 # ----------------------------------------------------------------------------------------------------------------
 def _attn_ref64(q, k, v, mask, causal, B, L, Hq, Hkv, D, d_out=None):
     """fp64 attention, one sequence at a time (memory: Hq x L x L doubles per chunk); with d_out also (dq, dk, dv)"""

@@ -168,7 +168,7 @@ def test_decode_gemm(cuda_dev, M, N, K):
     assert _rel(ops.decode_gemm(a, w, out_dtype=bf16, resid=r16).float(), ref + r16.float()) < 4e-3
     gelu = torch.nn.functional.gelu(ref)
     assert _rel(ops.decode_gemm(a, w, out_dtype=f32, act=1), gelu) < 1e-4
-    # the same numbers as the tcgen05 GEMM the rest of the engine uses (bf16 outputs agree to rounding)
+    # the same numbers as the wgmma GEMM the rest of the engine uses (bf16 outputs agree to rounding)
     if M == 16:
         assert _rel(ops.gemm(a, w).float(), out.float()) < 4e-3
     wide = torch.zeros(M, N + 16, dtype=f32, device=cuda_dev)                  # output into a column slice

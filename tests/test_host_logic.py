@@ -188,15 +188,15 @@ def test_head_chunk_rows_plans_whole_tiles_within_budget():
     """row-chunk planner of the chunked lm_head + CE head (dalm_b200/ops.py): 128-row aligned, scratch within the budget,
     fewest wasted tile waves among the next few chunk counts"""
     from dalm_b200 import ops
-    # cfg-3: 4608 rows x 32000 logits, 80 MB budget -> 4 chunks of 9 m-tiles (1 152 rows, 74 MB): 32 waves vs 36 for 6 x 6
-    assert ops.head_chunk_rows(4608, 32000, 80 << 20) == 1152
+    # cfg-3: 4608 rows x 32000 logits, 80 MB budget, 148 SMs -> 4 chunks of 9 m-tiles (1 152 rows, 74 MB): 32 waves vs 36 for 6 x 6
+    assert ops.head_chunk_rows(4608, 32000, 80 << 20, sms=148) == 1152
     # cfg-5: 36 864 rows x 65 024 logits: L2-sized chunks for a frozen head, 512 MB chunks for a trainable one
-    r_l2, r_full = ops.head_chunk_rows(36864, 65024, 80 << 20), ops.head_chunk_rows(36864, 65024, 512 << 20)
+    r_l2, r_full = ops.head_chunk_rows(36864, 65024, 80 << 20, sms=132), ops.head_chunk_rows(36864, 65024, 512 << 20, sms=132)
     assert r_l2 % 128 == 0 and r_l2 * 65024 * 2 <= 80 << 20 and r_full % 128 == 0 and r_full * 65024 * 2 <= 512 << 20 and r_full > r_l2
     # tiny problems: one 128-row tile per chunk at least, never zero
-    assert ops.head_chunk_rows(5, 504, 1) == 128 and ops.head_chunk_rows(300, 1000, 128 * 1000 * 2) == 128
+    assert ops.head_chunk_rows(5, 504, 1, sms=132) == 128 and ops.head_chunk_rows(300, 1000, 128 * 1000 * 2, sms=132) == 128
     for M, Vp, budget in ((4608, 32000, 80 << 20), (200, 504, 128 * 504 * 2), (36864, 65024, 512 << 20), (1000, 30528, 64 << 20)):
-        rows = ops.head_chunk_rows(M, Vp, budget)
+        rows = ops.head_chunk_rows(M, Vp, budget, sms=132)
         assert rows >= 128 and rows % 128 == 0
         assert sum(min(rows, M - r0) for r0 in range(0, M, rows)) == M          # the chunks tile the rows exactly
 

@@ -16,7 +16,7 @@ def _rel(a, b):
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# GEMM (tcgen05)
+# GEMM (wgmma)
 # ----------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("M,N,K,bn", [
     (128, 64, 64, 64), (128, 128, 128, 128), (128, 256, 256, 256),       # single tile per config
@@ -39,7 +39,7 @@ def test_gemm_plain(cuda_dev, M, N, K, bn):
 
 
 def test_gemm_multi_tile_per_cta(cuda_dev):
-    """force few CTAs so each walks many tiles: exercises the smem ring wrap-around and both TMEM accumulator stages"""
+    """force few CTAs so each walks many tiles: exercises the smem ring wrap-around and the parked-accumulator hand-off between tiles"""
     from dalm_b200 import ops
     torch.manual_seed(0)
     M, N, K = 1024, 2048, 768
@@ -486,7 +486,7 @@ def test_gemm_l2_hints_and_raster_modes_do_not_change_results(cuda_dev):
 
 @pytest.mark.parametrize("M,F,K", [(300, 256, 192), (4608, 1408, 512), (1000, 11008, 264), (130, 384, 72)])
 def test_gemm_with_fused_swiglu_backward_epilogue(cuda_dev, M, F, K):
-    """down-projection dgrad + SwiGLU backward in one launch (d(act) never leaves TMEM, gate|up overwritten in place with
+    """down-projection dgrad + SwiGLU backward in one launch (d(act) never leaves the SM, gate|up overwritten in place with
     [d gate | d up]) == dgrad GEMM + swiglu_bwd kernel, bit for bit; and against torch autograd of silu(gate) * up"""
     from dalm_b200 import ops
     g = torch.Generator(device="cpu").manual_seed(M + F + K + 1)

@@ -152,9 +152,10 @@ def test_attention_fwd_bwd(cuda_dev, B, L, Hq, Hkv, D, causal, pad):
 # ----------------------------------------------------------------------------------------------------------------
 # row-wise kernels
 # ----------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("M,H", [(333, 1024), (26700, 1024), (77, 384), (130, 256), (9, 2048), (50, 4544)])
+@pytest.mark.parametrize("M,H", [(333, 1024), (26700, 1024), (77, 384), (130, 256), (9, 2048), (50, 4544), (257, 512), (131, 768)])
 def test_layernorm_fwd_bwd(cuda_dev, M, H):
-    """H in {256, 512, 1024, 2048} runs the warp-per-row kernels, other widths (bge-small 384, Falcon 4544) the CTA-per-row ones"""
+    """H in {256, 512, 1024, 2048} runs the warp-per-row kernels, other widths (bge-small 384, bge-base 768, Falcon 4544) the
+    CTA-per-row ones"""
     from dalm_b200 import ops
     torch.manual_seed(2)
     z = torch.randn(M, H, device=cuda_dev) * 2 + 0.3

@@ -8,6 +8,7 @@
 //                          appended to the cache by the same launch (no separate copy kernel)
 //   greedy_step_kernel   : argmax over the vocabulary row + HF's finished-sequence bookkeeping (pad after EOS), writes
 //                          the token, its attention-mask bit and its position id for the next step
+//   sample_step_kernel   : the same step with the token drawn from HF's temperature -> top-k -> top-p warpers
 //
 // All state a step needs (next token ids, position ids, finished flags, per-step alive counts, and — in device-column mode —
 // each row's current column) lives in device memory: a decode step is then the SAME launch sequence with the same
@@ -222,6 +223,27 @@ __global__ void __launch_bounds__(128) attn_decode_v2_kernel(const __nv_bfloat16
   }
 }
 
+// HF's per-token bookkeeping (transformers generation/utils.py _sample), run by one thread per row after the token is chosen:
+// finished rows emit pad, a row finishes when it emits an EOS id, the new column joins the attention mask, the position id
+// advances, alive[col] counts the rows still generating, and in device-column mode the row's column counter advances.
+__device__ __forceinline__ void finish_token(int b, int col, long long cand, const int64_t* __restrict__ eos_ids, int n_eos,
+                                             long long pad_id, int* __restrict__ unfinished, int64_t* __restrict__ tokens,
+                                             long long ldt, int64_t* __restrict__ mask, long long ldm, int* __restrict__ cur_dev,
+                                             int64_t* __restrict__ next_ids, int64_t* __restrict__ pos, int* __restrict__ alive) {
+  int unf = unfinished[b];
+  const long long tok = unf ? cand : pad_id;
+  tokens[(size_t)b * ldt + col] = tok;
+  mask[(size_t)b * ldm + col] = 1;               // HF appends ones to the attention mask for every generated column
+  next_ids[b] = tok;
+  pos[b] += 1;                                   // position id of the new token = cumsum(mask) - 1
+  if (unf)
+    for (int e = 0; e < n_eos; ++e)
+      if (tok == eos_ids[e]) unf = 0;
+  unfinished[b] = unf;
+  if (unf) atomicAdd(alive + col, 1);
+  if (cur_dev) cur_dev[b] = col;
+}
+
 // grid B, 256 threads. argmax over logits[b, 0..V) (ties -> lowest index, like torch.argmax), then HF's greedy bookkeeping
 // (transformers generation/utils.py _sample, do_sample=False): finished rows emit pad, a row finishes when it emits an EOS id.
 __global__ void __launch_bounds__(256) greedy_step_kernel(const __nv_bfloat16* __restrict__ logits, long long ld, int V,
@@ -259,19 +281,281 @@ __global__ void __launch_bounds__(256) greedy_step_kernel(const __nv_bfloat16* _
       const int oi = si[w];
       if (oi != INT_MAX && (bi == INT_MAX || ov > best || (ov == best && oi < bi))) { best = ov; bi = oi; }
     }
-    int unf = unfinished[b];
-    const long long tok = unf ? (long long)bi : pad_id;
-    tokens[(size_t)b * ldt + col] = tok;
-    mask[(size_t)b * ldm + col] = 1;             // HF appends ones to the attention mask for every generated column
-    next_ids[b] = tok;
-    pos[b] += 1;                                 // position id of the new token = cumsum(mask) - 1
-    if (unf)
-      for (int e = 0; e < n_eos; ++e)
-        if (tok == eos_ids[e]) unf = 0;
-    unfinished[b] = unf;
-    if (unf) atomicAdd(alive + col, 1);
-    if (cur_dev) cur_dev[b] = col;
+    finish_token(b, col, (long long)bi, eos_ids, n_eos, pad_id, unfinished, tokens, ldt, mask, ldm, cur_dev, next_ids, pos, alive);
   }
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// Sampling step: HF's _sample with do_sample=True and its warper stack, temperature -> top-k -> top-p, then one draw.
+// grid B, 1024 threads, one CTA per row; the row is re-read from L2 by every pass (V up to SAMPLE_MAX_V).
+//   keys      every pass works on the 16-bit order-preserving key of the bf16 logit (-0 folded onto +0). x = logit / T is
+//             strictly increasing over bf16 logits as long as it does not underflow, so ties and order of x are those of
+//             the keys
+//   top-k     radix select (two 8-bit digits) of the k-th largest key; survivors are the keys >= it (ties all kept)
+//   top-p     mass-weighted radix search over the survivors' keys, ascending: the first key at which the cumulative mass
+//             exceeds (1 - top_p) * Z. Masses are exp(x - max) in 2^-40 fixed point (64-bit integer sums are exact and
+//             order-independent; the quantisation moves a cumulative share by < 1e-7). Inside the tie group at the cut,
+//             tokens are removed in ascending index order, i.e. the order is (x, index): our deterministic rule where
+//             HF's unstable sort leaves it open. The largest (x, index) always stays (min_tokens_to_keep = 1)
+//   draw      u in [0, 1) from Philox keyed by the seed with counter (column, row): the same column gives the same draw
+//             whether the step is launched eagerly or replayed from a CUDA graph. The token is the first kept index,
+//             ascending, whose inclusive prefix sum of exp(x - max) exceeds u * Z; prefix sums and Z in fp64, in a fixed
+//             order (warp segments of consecutive indices)
+// ------------------------------------------------------------------------------------------------------------
+constexpr int SAMPLE_THREADS = 1024;
+constexpr int SAMPLE_MAX_V = 1 << 20;            // 2^20 * 2^40 fits the 64-bit mass sums; indices fit 3 radix digits
+
+__device__ __forceinline__ unsigned int bf16_key(unsigned short b) {
+  if (b == 0x8000u) b = 0;                       // -0 == +0
+  return (b & 0x8000u) ? (~b & 0xFFFFu) : (b | 0x8000u);
+}
+__device__ __forceinline__ float key_logit(unsigned int k) {
+  const unsigned int b = (k & 0x8000u) ? (k & 0x7FFFu) : (~k & 0xFFFFu);
+  return __uint_as_float(b << 16);
+}
+// exp(x - m) with the difference carried past fp32: d = x - m is exact in fp64; exp(hi + lo) ~ expf(hi) * (1 + lo)
+__device__ __forceinline__ double mass_of(float x, float m) {
+  const double d = (double)x - (double)m;
+  const float hi = (float)d;
+  return (double)expf(hi) * (1.0 + (d - (double)hi));
+}
+__device__ __forceinline__ double sample_uniform(unsigned long long seed, int col, int row) {
+  const uint4 r = philox4x32_7(make_uint2((unsigned int)seed, (unsigned int)(seed >> 32)),
+                               make_uint4((unsigned int)col, 0u, (unsigned int)row, 0u));
+  return (double)(((unsigned long long)r.x << 21) | (r.y >> 11)) * 0x1p-53;    // 53 random bits
+}
+
+// k-th largest (k >= 1) of key(i) over the i < V with pred(i, key), by `levels` 8-bit radix digits (most significant first).
+// cnt: 256 shared counters, bc: 2 shared words.
+template <class KeyF, class PredF>
+__device__ unsigned int radix_kth_largest(int V, int levels, KeyF key, PredF pred, unsigned int k, unsigned int* cnt,
+                                          unsigned int* bc) {
+  unsigned int prefix = 0, hmask = 0;
+  for (int lv = levels - 1; lv >= 0; --lv) {
+    const int shift = 8 * lv;
+    for (int j = threadIdx.x; j < 256; j += blockDim.x) cnt[j] = 0;
+    __syncthreads();
+    for (int i0 = threadIdx.x & ~31; i0 < V; i0 += blockDim.x) {          // warp-uniform trip count
+      const int i = i0 + (threadIdx.x & 31);
+      unsigned int kk = 0;
+      bool want = i < V;
+      if (want) { kk = key(i); want = (kk & hmask) == prefix && pred(i, kk); }
+      const unsigned int act = __ballot_sync(0xffffffffu, want);
+      if (want) {                                // one atomic per distinct bin of the warp: few bins hold most keys
+        const unsigned int d = (kk >> shift) & 255u;
+        const unsigned int peers = __match_any_sync(act, d);
+        if ((int)(threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(&cnt[d], (unsigned int)__popc(peers));
+      }
+    }
+    __syncthreads();
+    if (threadIdx.x < 32) {
+      const int lane = threadIdx.x;
+      unsigned int c[8], s = 0;
+#pragma unroll
+      for (int e = 0; e < 8; ++e) { c[e] = cnt[255 - 8 * lane - e]; s += c[e]; }      // lane 0 holds the top bins
+      unsigned int inc = s;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned int t = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += t;
+      }
+      unsigned int run = inc - s;
+      if (run < k && k <= inc) {
+        for (int e = 0; e < 8; ++e) {
+          if (run + c[e] >= k) { bc[0] = 255 - 8 * lane - e; bc[1] = k - run; break; }
+          run += c[e];
+        }
+      }
+    }
+    __syncthreads();
+    prefix |= bc[0] << shift;
+    hmask |= 255u << shift;
+    k = bc[1];
+  }
+  return prefix;
+}
+
+__global__ void __launch_bounds__(SAMPLE_THREADS) sample_step_kernel(
+    const __nv_bfloat16* __restrict__ logits, long long ld, int V, const int64_t* __restrict__ eos_ids, int n_eos,
+    long long pad_id, int* __restrict__ unfinished, int64_t* __restrict__ tokens, long long ldt, int64_t* __restrict__ mask,
+    long long ldm, int col_host, int* __restrict__ cur_dev, int T, int64_t* __restrict__ next_ids, int64_t* __restrict__ pos,
+    int* __restrict__ alive, float temperature, int top_k, float top_p, unsigned long long seed,
+    const double* __restrict__ u_in, float* __restrict__ scores_out) {
+  __shared__ unsigned int cnt[256];
+  __shared__ unsigned long long qmass[256];
+  __shared__ unsigned int bc[4];
+  __shared__ unsigned long long bcl[2];
+  __shared__ double wtot[32], bcd[2];
+  __shared__ int wlast[32], chosen;
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int col = cur_dev ? cur_dev[b] + 1 : col_host;
+  if (col >= T) return;                          // a replay past the end of the buffers is a no-op
+  if (unfinished[b]) {                           // finished rows emit pad: nothing to choose
+    const unsigned short* row = reinterpret_cast<const unsigned short*>(logits + (size_t)b * ld);
+    auto lkey = [&](int i) { return bf16_key(row[i]); };
+    auto xval = [&](int i) { return __fdiv_rn(__bfloat162float(__ushort_as_bfloat16(row[i])), temperature); };
+
+    // ---- max key (the largest x, the softmax shift) ----
+    unsigned int mk = 0;
+    for (int i = tid; i < V; i += SAMPLE_THREADS) mk = max(mk, lkey(i));
+    mk = __reduce_max_sync(0xffffffffu, mk);
+    if (lane == 0) cnt[warp] = mk;
+    __syncthreads();
+    if (warp == 0) {
+      const unsigned int v = __reduce_max_sync(0xffffffffu, cnt[lane]);
+      if (lane == 0) bc[2] = v;
+    }
+    __syncthreads();
+    mk = bc[2];
+    const float mx = __fdiv_rn(key_logit(mk), temperature);
+
+    // ---- top-k: survivors are the keys >= the k-th largest ----
+    unsigned int kthr = 0;
+    if (top_k > 0 && top_k < V)
+      kthr = radix_kth_largest(V, 2, lkey, [](int, unsigned int) { return true; }, (unsigned int)top_k, cnt, bc);
+
+    // ---- top-p: kept = (key, index) >= (kp, icut) ----
+    unsigned int kp = kthr, icut = 0;
+    if (top_p < 1.f) {
+      unsigned int prefix = 0, hmask = 0;
+      unsigned long long below = 0;              // fixed-point mass of the survivors below the current prefix
+      double c = 0.0;                            // (1 - top_p) * Z, warp 0 only
+      for (int lv = 1; lv >= 0; --lv) {
+        const int shift = 8 * lv;
+        for (int j = tid; j < 256; j += SAMPLE_THREADS) { cnt[j] = 0; qmass[j] = 0; }
+        __syncthreads();
+        for (int i0 = tid - lane; i0 < V; i0 += SAMPLE_THREADS) {          // warp-uniform trip count
+          const int i = i0 + lane;
+          unsigned int kk = 0;
+          bool want = i < V;
+          if (want) { kk = lkey(i); want = kk >= kthr && (kk & hmask) == prefix; }
+          const unsigned int act = __ballot_sync(0xffffffffu, want);
+          if (want) {                            // the warp's tokens of one bin are summed first: one atomic per bin
+            const unsigned int d = (kk >> shift) & 255u;
+            const unsigned long long q = __double2ull_rn(mass_of(xval(i), mx) * 0x1p40);
+            const unsigned int peers = __match_any_sync(act, d);
+            unsigned long long sum = 0;
+            for (unsigned int p = peers; p; p &= p - 1) sum += __shfl_sync(peers, q, __ffs(p) - 1);
+            if (lane == __ffs(peers) - 1) {
+              atomicAdd(&qmass[d], sum);
+              atomicAdd(&cnt[d], (unsigned int)__popc(peers));
+            }
+          }
+        }
+        __syncthreads();
+        if (warp == 0) {
+          unsigned long long m8[8], s = 0;
+          unsigned int any = 0;
+#pragma unroll
+          for (int e = 0; e < 8; ++e) { m8[e] = qmass[8 * lane + e]; s += m8[e]; any |= cnt[8 * lane + e]; }   // ascending bins
+          unsigned long long inc = s;
+#pragma unroll
+          for (int o = 1; o < 32; o <<= 1) {
+            const unsigned long long t = __shfl_up_sync(0xffffffffu, inc, o);
+            if (lane >= o) inc += t;
+          }
+          if (lv == 1) c = (1.0 - (double)top_p) * (double)__shfl_sync(0xffffffffu, inc, 31);
+          const unsigned int cross = __ballot_sync(0xffffffffu, (double)(below + inc) > c);
+          // no bin crosses only when rounding ate the last (1 - top_p) share: keep the largest key, as HF keeps one token
+          const int src = cross ? __ffs(cross) - 1 : 31 - __clz(__ballot_sync(0xffffffffu, any != 0));
+          if (lane == src) {
+            int e = 0;
+            if (cross)
+              while (e < 7 && !((double)(below + inc - s + m8[e]) > c)) s -= m8[e++];    // s: mass from bin e to the lane's end
+            else
+              for (int f = 7; f >= 0; --f)
+                if (cnt[8 * lane + f]) { e = f; break; }
+            unsigned long long run = below + inc - s;                                      // mass below bin e
+            if (!cross)
+              for (int f = 0; f < e; ++f) run += m8[f];
+            const int d = 8 * lane + e;
+            bc[0] = d; bc[1] = cnt[d]; bcl[0] = run; bcl[1] = qmass[d];
+            if (lv == 0) {
+              // tie group at the cut: n tokens of mass w each, cumulative run + (r + 1) w; the first r0 (by index) have
+              // a cumulative share <= 1 - top_p and go; at least one of the group stays
+              const unsigned int n = cnt[d];
+              const double w = (double)(qmass[d] / n);
+              double r0 = floor((c - (double)run) / w);
+              r0 = r0 < 0.0 ? 0.0 : (r0 > (double)(n - 1) ? (double)(n - 1) : r0);
+              bc[2] = (unsigned int)r0;
+            }
+          }
+        }
+        __syncthreads();
+        prefix |= bc[0] << shift;
+        hmask |= 255u << shift;
+        below = bcl[0];
+      }
+      kp = prefix;
+      const unsigned int nt = bc[1], r0 = bc[2];
+      if (r0 > 0)                                // the (nt - r0)-th largest index of the tie group is the first one kept
+        icut = radix_kth_largest(V, 3, [](int i) { return (unsigned int)i; },
+                                 [&](int i, unsigned int) { return lkey(i) == kp; }, nt - r0, cnt, bc);
+    }
+    auto kept = [&](int i, unsigned int kk) { return kk > kp || (kk == kp && (unsigned int)i >= icut); };
+
+    // ---- draw: per-warp segments of consecutive indices, fp64 sums in a fixed order ----
+    const double u = u_in ? u_in[b] : sample_uniform(seed, col, b);
+    const int seg = (((V + 31) / 32) + 31) & ~31;
+    const int s0 = warp * seg, s1 = min(V, s0 + seg);
+    double acc = 0.0;
+    int last = -1;
+    for (int i = s0 + lane; i < s1; i += 32) {
+      const unsigned int kk = lkey(i);
+      const float x = xval(i);
+      const bool k_ = kept(i, kk);
+      if (k_) {
+        const double w = mass_of(x, mx);
+        acc += w;
+        if (w > 0.0) last = i;
+      }
+      if (scores_out) scores_out[(size_t)b * ld + i] = k_ ? x : -INFINITY;
+    }
+    acc = warp_sum_d(acc);
+    last = __reduce_max_sync(0xffffffffu, last);
+    if (lane == 0) { wtot[warp] = acc; wlast[warp] = last; }
+    __syncthreads();
+    if (warp == 0) {
+      const double t = wtot[lane];
+      double inc = t;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const double v = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += v;
+      }
+      const double target = u * __shfl_sync(0xffffffffu, inc, 31);
+      const unsigned int cross = __ballot_sync(0xffffffffu, inc > target);
+      const int glast = __reduce_max_sync(0xffffffffu, wlast[lane]);
+      const int wc = cross ? __ffs(cross) - 1 : -1;
+      const double base = __shfl_sync(0xffffffffu, inc - t, wc < 0 ? 0 : wc);
+      if (lane == 0) { bc[3] = (unsigned int)wc; bcd[0] = base; bcd[1] = target; chosen = glast; }
+    }
+    __syncthreads();
+    if (warp == (int)bc[3]) {                    // the warp whose segment holds the crossing walks it 32 tokens at a time
+      double run = bcd[0];
+      const double target = bcd[1];
+      int pick = wlast[warp];                    // rounding fallback: the segment's last kept token
+      for (int j = s0; j < s1; j += 32) {
+        const int i = j + lane;
+        double w = 0.0;
+        if (i < s1 && kept(i, lkey(i))) w = mass_of(xval(i), mx);
+        double inc = w;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+          const double v = __shfl_up_sync(0xffffffffu, inc, o);
+          if (lane >= o) inc += v;
+        }
+        const unsigned int hit = __ballot_sync(0xffffffffu, w > 0.0 && run + inc > target);
+        if (hit) { pick = j + __ffs(hit) - 1; break; }
+        run += __shfl_sync(0xffffffffu, inc, 31);
+      }
+      if (lane == 0) chosen = pick;
+    }
+    __syncthreads();
+  }
+  if (tid == 0)
+    finish_token(b, col, (long long)chosen, eos_ids, n_eos, pad_id, unfinished, tokens, ldt, mask, ldm, cur_dev, next_ids, pos,
+                 alive);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -474,4 +758,25 @@ extern "C" int dalm_b200_greedy_step(const void* logits, long long ld, int B, in
                                                 ldt, mask, ldm, col, cur_dev, T, next_ids, pos, alive);
   count_launch();
   return check_launch("greedy_step_kernel");
+}
+
+extern "C" int dalm_b200_sample_step(const void* logits, long long ld, int B, int V, const int64_t* eos_ids, int n_eos,
+                                     long long pad_id, int* unfinished, int64_t* tokens, long long ldt, int64_t* mask,
+                                     long long ldm, int col, int* cur_dev, int T, int64_t* next_ids, int64_t* pos, int* alive,
+                                     float temperature, int top_k, float top_p, unsigned long long seed, const double* u,
+                                     float* scores_out, void* stream) {
+  DALM_REQUIRE(B > 0 && V > 0 && T > 0 && T <= ldt && T <= ldm && ld >= V, "sample_step: bad shape B=%d V=%d T=%d", B, V, T);
+  DALM_REQUIRE(V <= SAMPLE_MAX_V, "sample_step: vocabulary of %d exceeds the kernel's limit of %d", V, SAMPLE_MAX_V);
+  DALM_REQUIRE(cur_dev != nullptr || (col >= 0 && col < T), "sample_step: column %d outside the %d-token buffers", col, T);
+  DALM_REQUIRE(n_eos >= 0 && (n_eos == 0 || eos_ids != nullptr), "sample_step: eos list");
+  DALM_REQUIRE(unfinished && tokens && mask && next_ids && pos && alive, "sample_step: null state pointer");
+  DALM_REQUIRE(temperature > 0.f && isfinite(temperature), "sample_step: temperature must be positive and finite (got %g)",
+               (double)temperature);
+  DALM_REQUIRE(top_p > 0.f && top_p <= 1.f, "sample_step: top_p must be in (0, 1] (got %g)", (double)top_p);
+  DALM_REQUIRE(top_k >= 0, "sample_step: top_k must be >= 0 (0 or >= V: off), got %d", top_k);
+  sample_step_kernel<<<B, SAMPLE_THREADS, 0, ST(stream)>>>((const __nv_bfloat16*)logits, ld, V, eos_ids, n_eos, pad_id, unfinished,
+                                                           tokens, ldt, mask, ldm, col, cur_dev, T, next_ids, pos, alive,
+                                                           temperature, top_k, top_p, seed, u, scores_out);
+  count_launch();
+  return check_launch("sample_step_kernel");
 }

@@ -308,9 +308,10 @@ class FalconDecoder(torch.nn.Module):
         return ops.gemm_rows(hf, self.lm_head)
 
     def generate(self, input_ids: Optional[torch.Tensor] = None, attention_mask: Optional[torch.Tensor] = None, **kw) -> torch.Tensor:
-        """HF `generate` for the call the reference makes (greedy search); see engine/decoding.py"""
-        from .decoding import greedy_generate
-        return greedy_generate(self, input_ids, attention_mask, **kw)
+        """HF `generate`: greedy search or sampling, as the checkpoint's generation config and the call select; see
+        engine/decoding.py"""
+        from .decoding import generate
+        return generate(self, input_ids, attention_mask, **kw)
 
     def backward_logits(self, ctx, dlogits: torch.Tensor) -> None:
         """dlogits bf16 [B,L,V] -> gradients of every parameter (full mode); nothing to do for a frozen decoder"""

@@ -470,9 +470,10 @@ class LlamaDecoder(torch.nn.Module):
         return self.Nq, self.Nq + self.Nkv, self.Nkv
 
     def generate(self, input_ids: Optional[torch.Tensor] = None, attention_mask: Optional[torch.Tensor] = None, **kw) -> torch.Tensor:
-        """HF `generate` for the call the reference makes (greedy search); see engine/decoding.py"""
-        from .decoding import greedy_generate
-        return greedy_generate(self, input_ids, attention_mask, **kw)
+        """HF `generate`: greedy search or sampling, as the checkpoint's generation config and the call select; see
+        engine/decoding.py"""
+        from .decoding import generate
+        return generate(self, input_ids, attention_mask, **kw)
 
     # ------------------------------------------------------------------------------------------------------------
     def backward_logits(self, ctx: _Ctx, dlogits: torch.Tensor) -> None:

@@ -1,9 +1,9 @@
 """`dalm eval-rag` — reference dalm/eval/eval_rag.py:167-290. Retriever half: passage sweep, exact top-k, recall / precision /
 hit-rate through `rag_model.retrieval_forward`. Generator half (`run_generator_on_prompts` :126-140, `eval_generator_on_batch`
 :143-164, exact match :268-283): prompts `#query# q #passage# p #answer# ` are tokenised exactly as the reference does and
-decoded by `generator_model.generate` — greedy search with a KV cache over the C-ABI kernels (engine/decoding.py), HF
-`generate` semantics for the reference's call. A checkpoint whose generation_config asks for sampling (Llama-2's does) is
-decoded greedily here; that is stated in the log line, not hidden."""
+decoded by `generator_model.generate` with a KV cache over the C-ABI kernels (engine/decoding.py), HF `generate` semantics
+for the reference's call: greedy search, or sampling (temperature -> top-k -> top-p) when the checkpoint's generation_config
+asks for it, as Llama-2's does. The log line states which one runs."""
 from __future__ import annotations
 
 import logging
@@ -95,7 +95,8 @@ def evaluate_rag(
     model, tokenizer = rag_model.generator_model, rag_model.generator_tokenizer
     if evaluate_generator:
         tokenizer.pad_token = tokenizer.eos_token                                 # reference :240
-        logger.info("generator evaluation decodes greedily (do_sample=False); a sampling generation_config is not honoured")
+        from ..engine.decoding import decoding_mode
+        logger.info(f"generator evaluation decodes by {decoding_mode(model, max_length=max_length, early_stopping=True)}")
     loader = DataLoader(processed, batch_size=test_batch_size, shuffle=True, collate_fn=mixed_collate_fn)
     for batch in loader:
         p_, r_, h_, top_passages = evaluate_retriever_on_batch(batch, passage_column_name, rag_model.retrieval_forward, index,
@@ -148,7 +149,7 @@ _FLAGS = [
 
 def parse_args() -> Namespace:
     from ..training.utils.loop import build_parser
-    return build_parser("RAG evaluation: retrieval metrics + greedy generation / exact match (H100-native)", _FLAGS).parse_args()
+    return build_parser("RAG evaluation: retrieval metrics + generation / exact match (H100-native)", _FLAGS).parse_args()
 
 
 def main() -> None:

@@ -15,6 +15,7 @@ from .. import ops
 from ..engine import params
 from ..engine.bert import BertEncoder
 from ..engine.bridge import EncodeFn, GenerateFn, PoolFn
+from ..engine.decoding import load_generation_config
 from ..engine.falcon import FalconDecoder
 from ..engine.llama import LlamaDecoder
 
@@ -129,10 +130,13 @@ def build_decoder(name_or_path: str, lora: bool, device: torch.device, state_dic
     if not nf4:
         sd = _maybe_bnb(sd, bnb, full, device)
     if kind == "falcon":
-        return _named(FalconDecoder(cfg, sd, device=device, lora=lora, full=full), name_or_path)   # raises for lora=True, like peft would
-    if kind != "llama":
+        dec = FalconDecoder(cfg, sd, device=device, lora=lora, full=full)      # raises for lora=True, like peft would
+    elif kind != "llama":
         raise NotImplementedError(f"generator of kind {kind!r} is not a causal decoder")
-    return _named(LlamaDecoder(cfg, sd, device=device, lora=lora, full=full, nf4_storage=nf4), name_or_path)
+    else:
+        dec = LlamaDecoder(cfg, sd, device=device, lora=lora, full=full, nf4_storage=nf4)
+    dec.generation_config = load_generation_config(name_or_path)              # what `generate` starts from, like HF
+    return _named(dec, name_or_path)
 
 
 class AutoModelForRagE2E(torch.nn.Module):

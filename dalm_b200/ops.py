@@ -812,15 +812,42 @@ def greedy_step_(logits, V: int, eos_ids, pad_id: int, unfinished, tokens, mask,
     unfinished int32 [B]; tokens / mask int64 [B, T]; next_ids / pos int64 [B]; alive int32 [T] (zeroed by the caller).
     col: the column to write (int), or the int32 [B] device tensor holding each row's CURRENT column (the kernel writes
     column + 1 and advances it: CUDA-graph mode)."""
-    _chk(logits, bf16, "greedy logits"); _chk(tokens, i64, "tokens"); _chk(mask, i64, "mask")
+    _lib.call("dalm_b200_greedy_step", *_step_args("greedy_step", logits, V, eos_ids, pad_id, unfinished, tokens, mask, col,
+                                                   next_ids, pos, alive), _stream())
+
+
+def _step_args(what: str, logits, V: int, eos_ids, pad_id: int, unfinished, tokens, mask, col, next_ids, pos, alive) -> tuple:
+    """checks and C arguments shared by greedy_step_ and sample_step_ (everything up to `alive`)"""
+    _chk(logits, bf16, f"{what} logits"); _chk(tokens, i64, "tokens"); _chk(mask, i64, "mask")
     _chk(next_ids, i64, "next_ids"); _chk(pos, i64, "pos")
     T = tokens.shape[1]
     if unfinished.dtype != torch.int32 or alive.dtype != torch.int32 or alive.numel() < T or mask.shape[1] < T:
-        raise _lib.DalmB200Error("greedy_step: unfinished / alive must be int32, alive and mask as long as the token buffer")
+        raise _lib.DalmB200Error(f"{what}: unfinished / alive must be int32, alive and mask as long as the token buffer")
     if eos_ids is not None:
         _chk(eos_ids, i64, "eos_ids")
     B = logits.shape[0]
-    col_host, cur_dev = _cur_arg(col, B, "greedy_step")
-    _lib.call("dalm_b200_greedy_step", _p(logits), _ld(logits), B, int(V), _p(eos_ids), 0 if eos_ids is None else eos_ids.numel(),
-              int(pad_id), _p(unfinished), _p(tokens), tokens.stride(0), _p(mask), mask.stride(0), col_host, cur_dev, T,
-              _p(next_ids), _p(pos), _p(alive), _stream())
+    col_host, cur_dev = _cur_arg(col, B, what)
+    return (_p(logits), _ld(logits), B, int(V), _p(eos_ids), 0 if eos_ids is None else eos_ids.numel(), int(pad_id),
+            _p(unfinished), _p(tokens), tokens.stride(0), _p(mask), mask.stride(0), col_host, cur_dev, T, _p(next_ids), _p(pos),
+            _p(alive))
+
+
+def sample_step_(logits, V: int, eos_ids, pad_id: int, unfinished, tokens, mask, col, next_ids, pos, alive, *,
+                 temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0, seed: int = 0,
+                 u: Optional[torch.Tensor] = None, scores_out: Optional[torch.Tensor] = None) -> None:
+    """one sampling step on device state: greedy_step_'s arguments and bookkeeping, the token drawn from HF's warper stack
+    temperature -> top-k (0 = off) -> top-p (1 = off) with a Philox draw keyed by `seed` and (column, row); see
+    include/dalm_b200.h. Test hooks: u fp64 [B] replaces the draw; scores_out fp32 [B, >=V] with the logits' row stride
+    receives the warped scores (-inf where removed)."""
+    args = _step_args("sample_step", logits, V, eos_ids, pad_id, unfinished, tokens, mask, col, next_ids, pos, alive)
+    B = logits.shape[0]
+    if u is not None:
+        _chk(u, torch.float64, "sample_step u")
+        if u.numel() != B or not u.is_contiguous():
+            raise _lib.DalmB200Error(f"sample_step: u needs one contiguous fp64 value per row ({u.numel()} for {B} rows)")
+    if scores_out is not None:
+        _chk(scores_out, f32, "sample_step scores_out")
+        if scores_out.shape[0] != B or scores_out.shape[1] < V or _ld(scores_out) != _ld(logits):
+            raise _lib.DalmB200Error("sample_step: scores_out must be fp32 [B, >=V] with the logits' row stride")
+    _lib.call("dalm_b200_sample_step", *args, float(temperature), int(top_k), float(top_p), int(seed) & (2**64 - 1), _p(u),
+              _p(scores_out), _stream())

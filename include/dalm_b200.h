@@ -256,6 +256,23 @@ int dalm_b200_attention_decode(const void* qkv, long long ldq, int q_col, int k_
 int dalm_b200_greedy_step(const void* logits, long long ld, int B, int V, const int64_t* eos_ids, int n_eos,
                           long long pad_id, int* unfinished, int64_t* tokens, long long ldt, int64_t* mask, long long ldm,
                           int col, int* cur_dev, int T, int64_t* next_ids, int64_t* pos, int* alive, void* stream);
+/* sample_step: greedy_step with the token drawn instead of taken by argmax (HF _sample, do_sample=True), same arguments and
+ * the same bookkeeping after the choice. The warpers run in HF's order on fp32 scores x = float(logit) / temperature
+ * (IEEE division, so kept scores equal HF's bit for bit):
+ *   top-k (0 < top_k < V; 0 or >= V is off): remove x < the k-th largest x; ties at the k-th value are all kept;
+ *   top-p (top_p < 1): order the survivors ascending by (x, index) and remove while the cumulative softmax share is
+ *     <= 1 - top_p, always keeping the last one. HF sorts with an unstable sort; the (x, index) order is this library's
+ *     deterministic rule for a tie group that straddles the cut;
+ *   draw: u in [0, 1) from Philox keyed by seed with counter (column, row) -- the same token for an eager launch and a CUDA
+ *     graph replay; the token is the first kept index, ascending, whose inclusive prefix sum of exp(x - max) exceeds u * Z
+ *     (prefix sums and Z in fp64).
+ * Requires temperature > 0 and finite, 0 < top_p <= 1, top_k >= 0, V <= 2^20. Test hooks (NULL in production): u
+ * (fp64 [B]) replaces the Philox draw; scores_out (fp32, row stride ld) receives the warped scores of every unfinished row,
+ * -inf where a token was removed. Finished rows emit pad_id and are not scored. */
+int dalm_b200_sample_step(const void* logits, long long ld, int B, int V, const int64_t* eos_ids, int n_eos,
+                          long long pad_id, int* unfinished, int64_t* tokens, long long ldt, int64_t* mask, long long ldm,
+                          int col, int* cur_dev, int T, int64_t* next_ids, int64_t* pos, int* alive, float temperature,
+                          int top_k, float top_p, unsigned long long seed, const double* u, float* scores_out, void* stream);
 
 #ifdef __cplusplus
 }

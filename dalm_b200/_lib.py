@@ -55,7 +55,7 @@ SIGNATURES = {
     "dalm_b200_swiglu_fwd": [_P, _L, _P, _L, _I, _I, _I, _P],
     "dalm_b200_swiglu_bwd": [_P, _L, _P, _L, _I, _I, _I, _P],
     "dalm_b200_gemm_bf16_swiglu": [_P, _L, _P, _L, _P, _L, _P, _L, _I, _I, _I, _P],
-    "dalm_b200_gemm_bf16_rope": [_P, _L, _P, _L, _P, _L, _I, _I, _I, _P, _P, _I, _I, _P],
+    "dalm_b200_gemm_bf16_rope": [_P, _L, _P, _L, _P, _L, _I, _I, _I, _P, _P, _P, _I, _I, _P],
     "dalm_b200_gemm_bf16_swiglu_bwd": [_P, _L, _P, _L, _P, _L, _I, _I, _I, _P],
     "dalm_b200_gemm_bf16_gelu": [_P, _L, _P, _L, _P, _L, _P, _L, _I, _I, _I, _P, _P],
     "dalm_b200_gelu_fwd": [_P, _L, _P, _L, _I, _I, _P],
@@ -77,7 +77,7 @@ SIGNATURES = {
     "dalm_b200_nf4_roundtrip": [_P, _L, _P, _P, _P],
     "dalm_b200_nf4_quantize": [_P, _L, _P, _P, _P],
     "dalm_b200_nf4_dequant_bf16": [_P, _P, _L, _I, _P, _L, _P, _L, _I, _P],
-    "dalm_b200_decode_gemm": [_P, _L, _P, _L, _P, _L, _I, _P, _L, _I, _I, _I, _I, _I, _P],
+    "dalm_b200_decode_gemm": [_P, _L, _P, _L, _P, _L, _I, _P, _P, _L, _I, _I, _I, _I, _I, _P],
     "dalm_b200_rope_pos": [_P, _L, _I, _I, _I, _P, _P, _P, _I, _I, _P],
     "dalm_b200_attention_decode": [_P, _L, _I, _I, _I, _P, _P, _L, _L, _P, _L, _P, _L, _I, _I, _I, _I, _I, _P, _I, _F, _P],
     "dalm_b200_greedy_step": [_P, _L, _I, _I, _P, _I, _L, _P, _P, _L, _P, _L, _I, _P, _I, _P, _P, _P, _P],

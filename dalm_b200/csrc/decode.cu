@@ -559,7 +559,7 @@ __global__ void __launch_bounds__(SAMPLE_THREADS) sample_step_kernel(
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// Weight-streaming GEMM for the decode step: out[m, n] = act(sum_k A[m,k] W[n,k]) + resid[m,n] with M <= 16 token rows.
+// Weight-streaming GEMM for the decode step: out[m, n] = act(sum_k A[m,k] W[n,k] + bias[n]) + resid[m,n] with M <= 16 token rows.
 // HBM-bound: every weight is read exactly once (N*K*2 bytes), the activations (16 x K bf16) stay in L2. The 128-row wgmma
 // tile of the training GEMM wastes 7/8 of its A tile here and runs N = 4096 on 64 CTAs, so this path uses one `mma.sync.m16n8k16` row tile = the whole batch instead:
 //   CTA = 16 output columns (2 n-tiles) x all of K, 256 threads; the 8 warps interleave over 32-wide k-chunks (split-K inside
@@ -599,6 +599,7 @@ constexpr int DG_SMEM = DG_STAGES * 8 * DG_SLOTS * 32 * 16;     // 96 KB: [stage
 __global__ void __launch_bounds__(256) decode_gemm_kernel(const __nv_bfloat16* __restrict__ A, long long lda,
                                                           const __nv_bfloat16* __restrict__ W, long long ldw,
                                                           void* __restrict__ out, long long ldo, int out_f32,
+                                                          const float* __restrict__ bias,
                                                           const void* __restrict__ resid, long long ldr, int resid_f32, int act,
                                                           int M, int N, int K) {
   extern __shared__ __align__(16) unsigned char dg_smem[];
@@ -667,6 +668,7 @@ __global__ void __launch_bounds__(256) decode_gemm_kernel(const __nv_bfloat16* _
     float v = 0.f;
 #pragma unroll
     for (int w = 0; w < 8; ++w) v += part[w][m][nn];
+    if (bias) v += bias[n];
     if (act == 1) v = gelu_erf(v);
     if (resid) v += resid_f32 ? static_cast<const float*>(resid)[(size_t)m * ldr + n]
                               : __bfloat162float(static_cast<const __nv_bfloat16*>(resid)[(size_t)m * ldr + n]);
@@ -681,8 +683,8 @@ using namespace dalm;
 #define ST(s) ((cudaStream_t)(s))
 
 extern "C" int dalm_b200_decode_gemm(const void* A, long long lda, const void* W, long long ldw, void* out, long long ldo,
-                                     int out_f32, const void* resid, long long ldr, int resid_f32, int act, int M, int N, int K,
-                                     void* stream) {
+                                     int out_f32, const float* bias, const void* resid, long long ldr, int resid_f32, int act,
+                                     int M, int N, int K, void* stream) {
   DALM_REQUIRE(M > 0 && M <= 16 && N > 0 && K > 0, "decode_gemm: needs 1 <= M <= 16 token rows (got M=%d N=%d K=%d)", M, N, K);
   DALM_REQUIRE((K % 8) == 0 && (lda % 8) == 0 && (ldw % 8) == 0 && lda >= K && ldw >= K && ldo >= N,
                "decode_gemm: K and the operand row strides must be multiples of 8 elements");
@@ -692,7 +694,7 @@ extern "C" int dalm_b200_decode_gemm(const void* A, long long lda, const void* W
   static bool attr = false;
   if (!attr) { DALM_CUDA(cudaFuncSetAttribute(decode_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, DG_SMEM)); attr = true; }
   decode_gemm_kernel<<<(N + DG_NT * 8 - 1) / (DG_NT * 8), 256, DG_SMEM, ST(stream)>>>(
-      (const __nv_bfloat16*)A, lda, (const __nv_bfloat16*)W, ldw, out, ldo, out_f32, resid, ldr, resid_f32, act, M, N, K);
+      (const __nv_bfloat16*)A, lda, (const __nv_bfloat16*)W, ldw, out, ldo, out_f32, bias, resid, ldr, resid_f32, act, M, N, K);
   count_launch();
   return check_launch("decode_gemm_kernel");
 }

@@ -185,13 +185,15 @@ __device__ __forceinline__ void epilogue_drain_tile(const GemmEpilogue& ep, cons
 #pragma unroll
       for (int g = 0; g < 8; ++g)
         *reinterpret_cast<float4*>(st + ((g ^ sw) << 4)) = make_float4(f[g * 4], f[g * 4 + 1], f[g * 4 + 2], f[g * 4 + 3]);
-    } else if (ep.fuse == 2 && col0 < ep.rope_cols) {
+    } else if (BN == 256 && ep.fuse == 2 && col0 < ep.rope_cols) {   // gemm_bf16_rope launches 256-wide tiles only
       // RoPE in the QKV epilogue: this 64-column block is one rotate_half HALF of a head (x1 = columns 0..63, x2 = 64..127 of the
       // head; tiles are 256 columns = two whole heads); its partner half sits 64 columns away in the same accumulator.
       //   x1' = x1 cos - x2 sin ,  x2' = x2 cos + x1 sin        (cos / sin of the row's position, element j = column % 64)
-      // Replaces a separate in-place pass over the q|k columns of every layer's QKV output.
+      // Replaces a separate in-place pass over the q|k columns of every layer's QKV output. A q/k/v bias (Qwen2) is added to both
+      // halves in fp32 before the rotation, so the only rounding is the final bf16 store.
       const bool second = ((col0 >> 6) & 1) != 0;               // this block holds x2
       const int cp = second ? c - 64 : c + 64;
+      const int colp = tile_col0 + cp;
       const int pos = row_ok ? (row % ep.rope_L) : 0;
       const float* cs = ep.rope_cos + (size_t)pos * 64;
       const float* sn = ep.rope_sin + (size_t)pos * 64;
@@ -208,7 +210,11 @@ __device__ __forceinline__ void epilogue_drain_tile(const GemmEpilogue& ep, cons
         }
 #pragma unroll
         for (int i = 0; i < 32; ++i) {
-          const float own = __uint_as_float(vo[i]), oth = __uint_as_float(vq[i]);
+          float own = __uint_as_float(vo[i]), oth = __uint_as_float(vq[i]);
+          if (ep.bias) {
+            own += __ldg(ep.bias + col0 + h * 32 + i);
+            oth += __ldg(ep.bias + colp + h * 32 + i);
+          }
           f[i] = second ? fmaf(own, cc[i], oth * ss[i]) : fmaf(own, cc[i], -oth * ss[i]);
         }
 #pragma unroll
@@ -860,10 +866,12 @@ extern "C" int dalm_b200_gemm_bf16_gelu(const void* A, long long lda, const void
   return launch_gemm<64, 0, 3>(ta, tb, to, ep, 0, st, &to2);
 }
 
-// fused q|k|v projection + rotary embedding: out[M,N] = A[M,K] B[N,K]^T with HF's rotate_half RoPE (head_dim 128) applied to the
-// output columns [0, rope_cols) in the epilogue. cos / sin: fp32 [L, 64]; row m sits at position m % L (token-major [B*L] rows).
+// fused q|k|v projection + rotary embedding: out[M,N] = A[M,K] B[N,K]^T + bias with HF's rotate_half RoPE (head_dim 128) applied to
+// the output columns [0, rope_cols) in the epilogue. cos / sin: fp32 [L, 64]; row m sits at position m % L (token-major [B*L] rows).
+// bias: fp32 [N] or NULL, added before the rotation on every column.
 extern "C" int dalm_b200_gemm_bf16_rope(const void* A, long long lda, const void* B, long long ldb, void* out, long long ldo, int M,
-                                        int N, int K, const float* cos_t, const float* sin_t, int L, int rope_cols, void* stream) {
+                                        int N, int K, const float* bias, const float* cos_t, const float* sin_t, int L, int rope_cols,
+                                        void* stream) {
   DALM_REQUIRE(M > 0 && N > 0 && K > 0 && (N % 8) == 0 && (K % 8) == 0, "gemm_rope: bad shape M=%d N=%d K=%d", M, N, K);
   DALM_REQUIRE(rope_cols > 0 && rope_cols <= N && (rope_cols % 256) == 0, "gemm_rope: rope_cols=%d must be a multiple of 256 (whole 128-wide heads per tile)", rope_cols);
   DALM_REQUIRE(L > 0 && cos_t != nullptr && sin_t != nullptr && ((uintptr_t)cos_t & 15) == 0 && ((uintptr_t)sin_t & 15) == 0, "gemm_rope: cos / sin tables");
@@ -873,7 +881,7 @@ extern "C" int dalm_b200_gemm_bf16_rope(const void* A, long long lda, const void
   if (int e = get_tmap(B, N, K, ldb, 256, &tb)) return e;
   if (int e = get_tmap(out, M, N, ldo, 128, &to, 0)) return e;
   const int group_m = pick_group_m(M, N, K, 256, false);
-  GemmEpilogue ep{out, ldo, 0, nullptr, nullptr, 0, 0, 0, 1.f, M, N, K, make_drop(0.f, 0, 0, nullptr), group_m, 2, cos_t, sin_t, L, rope_cols,
+  GemmEpilogue ep{out, ldo, 0, bias, nullptr, 0, 0, 0, 1.f, M, N, K, make_drop(0.f, 0, 0, nullptr), group_m, 2, cos_t, sin_t, L, rope_cols,
                   pick_l2_hints(M, N, K, 256, group_m, false)};
   return launch_gemm<256>(ta, tb, to, ep, 0, (cudaStream_t)stream);
 }

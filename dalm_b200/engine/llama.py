@@ -1,4 +1,4 @@
-"""Llama decoder (Llama-2-7B shape and smaller) forward + backward as a launch sequence over the C-ABI kernels.
+"""Llama / Qwen2 decoder (Llama-2-7B / Qwen2.5-7B shape and smaller) forward + backward as a launch sequence over the C-ABI kernels.
 
 Mirrors `self.generator_model(input_ids=..., attention_mask=...).logits` of the reference
 (dalm/models/rag_e2e_base_model.py:104-106) through HF LlamaForCausalLM: embed -> N x [RMSNorm -> QKV(+LoRA on q,v)
@@ -9,7 +9,9 @@ HBM layout per layer (bf16 unless noted):
   WqkvT_aug [H, Nq+2Nkv+Ra] resident transpose for dgrad, last Ra columns = A_q^T | A_v^T
   A_stack [64,H], Bblk [64, Nq+2Nkv]   LoRA down / mid-gradient operands (see bert.py)
   Wo [H,Nq], WoT; Wgu [2F,H] (gate rows, then up rows), WguT [H,2F]; Wd [H,F], WdT [F,H]; RMSNorm gains fp32
+  bqkv [Nq+2Nkv], bo [H] fp32: attention biases (Qwen2: q|k|v only; Llama with attention_bias: both), added in the GEMM epilogues
 Residual stream and its gradient are fp32; every GEMM operand is bf16.
+Qwen2 is this architecture plus q/k/v biases (HF Qwen2ForCausalLM); configs are checked by params.check_llama_family.
 """
 from __future__ import annotations
 
@@ -21,6 +23,7 @@ import torch
 from .. import ops
 from .dense import DenseBank
 from .lora import LoraBank
+from .params import attention_biases, check_llama_family
 
 bf16, f32 = torch.bfloat16, torch.float32
 
@@ -55,7 +58,10 @@ class LlamaDecoder(torch.nn.Module):
         if nf4_storage:
             from .nf4store import Nf4Store
             self.nf4 = Nf4Store(device)
+        check_llama_family(cfg)
         self.cfg = cfg
+        self.kind = "qwen2" if cfg.get("model_type") == "qwen2" else "llama"
+        self.qkv_bias, self.o_bias = attention_biases(self.kind, cfg)
         self.H = H = cfg["hidden_size"]
         self.F = F = cfg["intermediate_size"]
         self.nl = cfg["num_hidden_layers"]
@@ -133,6 +139,10 @@ class LlamaDecoder(torch.nn.Module):
             m.append(("lm_head", "gemm", ["lm_head.weight"]))
         for l in range(self.nl):
             p = f"model.layers.{l}."
+            if self.qkv_bias:                                    # biases: "acc" entries (column sums accumulated by atomics)
+                m.append((f"L{l}.bqkv", "acc", [p + f"self_attn.{n}_proj.bias" for n in "qkv"]))
+            if self.o_bias:
+                m.append((f"L{l}.bo", "acc", [p + "self_attn.o_proj.bias"]))
             m += [(f"L{l}.Wqkv", "gemm", [p + f"self_attn.{n}_proj.weight" for n in "qkv"]),
                   (f"L{l}.Wo", "gemm", [p + "self_attn.o_proj.weight"]),
                   (f"L{l}.Wgu", "gemm", [p + "mlp.gate_proj.weight", p + "mlp.up_proj.weight"]),
@@ -170,7 +180,9 @@ class LlamaDecoder(torch.nn.Module):
         for l in range(self.nl):
             k = lambda n: f"L{l}.{n}"
             self.layers.append({"Wqkv_aug": bank.w16(k("Wqkv")), "Wo": bank.w16(k("Wo")), "Wgu": bank.w16(k("Wgu")),
-                                "Wd": bank.w16(k("Wd")), "g1": bank.w32(k("g1")), "g2": bank.w32(k("g2"))})
+                                "Wd": bank.w16(k("Wd")), "g1": bank.w32(k("g1")), "g2": bank.w32(k("g2")),
+                                "bqkv": bank.w32(k("bqkv")) if self.qkv_bias else None,
+                                "bo": bank.w32(k("bo")) if self.o_bias else None})
 
     def hf_state_dict(self) -> Dict[str, torch.Tensor]:
         """fp32 CPU tensors under HF LlamaForCausalLM names (save_pretrained of a fully fine-tuned decoder)"""
@@ -268,6 +280,7 @@ class LlamaDecoder(torch.nn.Module):
             W["WdT"] = W["Wd"].t().contiguous()
             W["g1"] = g(p + "input_layernorm.weight", f32)
             W["g2"] = g(p + "post_attention_layernorm.weight", f32)
+            self._frozen_biases(W, p, g)
             self.layers.append(W)
 
     def _init_layer_nf4(self, sd, l: int, g, lora: bool):
@@ -288,7 +301,14 @@ class LlamaDecoder(torch.nn.Module):
             W["Bblk"] = torch.zeros(64, self.Nqkv, dtype=bf16, device=self.dev)
         W["g1"] = g(p + "input_layernorm.weight", f32)
         W["g2"] = g(p + "post_attention_layernorm.weight", f32)
+        self._frozen_biases(W, p, g)
         return W
+
+    def _frozen_biases(self, W, p: str, g) -> None:
+        """frozen / LoRA modes: the attention biases are forward-only fp32 vectors (under use_bnb they take the fp16 cast of every
+        non-Linear-weight tensor, never the NF4 round trip)"""
+        W["bqkv"] = torch.cat([g(p + f"self_attn.{n}_proj.bias", f32) for n in "qkv"]) if self.qkv_bias else None
+        W["bo"] = g(p + "self_attn.o_proj.bias", f32) if self.o_bias else None
 
     def _drop(self, training: bool, call: int, layer: int):
         if not training or self.p_lora <= 0.0:
@@ -406,9 +426,10 @@ class LlamaDecoder(torch.nn.Module):
                                 dropx=self._drop(ctx.training, ctx.call, li))
             rope_cols = (self.nh + self.nkv) * self.hd
             if pos is None and self.fuse_rope and rope_cols % 256 == 0:
-                a.qkv = ops.gemm_rope(a.h1_aug, W["Wqkv_aug"], cos_t, sin_t, L, rope_cols)     # QKV (+LoRA) with RoPE in the epilogue
+                a.qkv = ops.gemm_rope(a.h1_aug, W["Wqkv_aug"], cos_t, sin_t, L, rope_cols,   # QKV (+LoRA, + bias) with RoPE in
+                                      bias=W["bqkv"])                                        # the epilogue
             else:
-                a.qkv = ops.gemm(a.h1_aug, W["Wqkv_aug"])                        # [M, Nq+2Nkv]
+                a.qkv = ops.gemm(a.h1_aug, W["Wqkv_aug"], bias=W["bqkv"])        # [M, Nq+2Nkv]
             if pos is None and not (self.fuse_rope and rope_cols % 256 == 0):
                 ops.rope_(a.qkv, 0, self.nh + self.nkv, self.hd, cos_t, sin_t, L)    # q heads then k heads are adjacent
             elif pos is None:
@@ -419,7 +440,7 @@ class LlamaDecoder(torch.nn.Module):
                 kv_sink(li, a.qkv)
             a.att, a.lse = ops.attention_auto_fwd(a.qkv[:, :self.Nq], a.qkv[:, self.Nq:self.Nq + self.Nkv],
                                                   a.qkv[:, self.Nq + self.Nkv:], ctx.mask, B, L, self.nh, self.nkv, self.hd, causal=True)
-            a.x_mid = ops.gemm(a.att, W["Wo"], out_dtype=f32, resid=x)
+            a.x_mid = ops.gemm(a.att, W["Wo"], out_dtype=f32, resid=x, bias=W["bo"])
             a.h2, a.rstd2 = ops.rmsnorm_fwd(a.x_mid, W["g2"], self.eps)
             if self.gu_il:
                 a.gu, a.act = ops.gemm_swiglu(a.h2, W["Wgu"])                     # [M,2F] (interleaved) + silu(gate)*up [M,F]: one launch
@@ -447,11 +468,11 @@ class LlamaDecoder(torch.nn.Module):
             ops.rmsnorm_fwd(x, W["g1"], self.eps, h=h1_aug[:, :H])
             if Ra:
                 ops.skinny_gemm(h1_aug[:, :H], W["A_stack"], h1_aug[:, H:], K=H, R=Ra)
-            qkv = ops.gemm_rows(h1_aug, W["Wqkv_aug"])                                # [B, Nq+2Nkv]
+            qkv = ops.gemm_rows(h1_aug, W["Wqkv_aug"], bias=W["bqkv"])                # [B, Nq+2Nkv]
             ops.rope_pos_(qkv, 0, self.nh + self.nkv, self.hd, cos_t, sin_t, pos)
             att = ops.attention_decode(qkv, 0, self.Nq, self.Nq + self.Nkv, caches[li][0], caches[li][1], kmask, cur,
                                        self.nh, self.nkv, self.hd)
-            x_mid = ops.gemm_rows(att, W["Wo"], out_dtype=f32, resid=x)
+            x_mid = ops.gemm_rows(att, W["Wo"], out_dtype=f32, resid=x, bias=W["bo"])
             h2, _ = ops.rmsnorm_fwd(x_mid, W["g2"], self.eps)
             act = ops.swiglu_fwd(ops.gemm_rows(h2, W["Wgu"]), F, interleave=self.gu_il)
             x = ops.gemm_rows(act, W["Wd"], out_dtype=f32, resid=x_mid)
@@ -527,6 +548,8 @@ class LlamaDecoder(torch.nn.Module):
             dmid32, dmid16 = ops.rmsnorm_bwd(a.x_mid, W["g2"], a.rstd2, dh2, dres_in=dx32)
             if bank is not None:
                 ops.wgrad_(dmid16, a.att, G(l, "Wo"), acc)
+                if self.o_bias:                                                    # d bo = column sums of d(o_proj output)
+                    ops.col_reduce_(dy_f32=dmid32, out_sum=G(l, "bo"))
             datt = self._dgrad(dmid16, W, "Wo")                                    # [M,Nq]
             dqkv = _aug_buf(M, self.Nqkv, Ra, self.dev)
             ops.attention_auto_bwd(a.qkv[:, :self.Nq], a.qkv[:, self.Nq:self.Nq + self.Nkv], a.qkv[:, self.Nq + self.Nkv:],
@@ -536,6 +559,8 @@ class LlamaDecoder(torch.nn.Module):
             ops.rope_(dqkv, 0, self.nh + self.nkv, self.hd, cos_t, sin_t, L, backward=True)
             if bank is not None:
                 ops.wgrad_(dqkv, a.h1_aug[:, :H], G(l, "Wqkv"), acc)
+                if self.qkv_bias:                                                  # d bqkv = column sums of d(pre-RoPE qkv)
+                    ops.col_reduce_(dy_bf16=dqkv, out_sum=G(l, "bqkv"))
                 dh1 = ops.gemm(dqkv, W["Wqkv_aug"], layout=1)
                 ops.col_reduce_(dy_bf16=dh1, z=a.x_in, rstd=a.rstd1, out_prod=G(l, "g1"))
                 dx32, dx16 = ops.rmsnorm_bwd(a.x_in, W["g1"], a.rstd1, dh1, dres_in=dmid32)

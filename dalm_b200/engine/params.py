@@ -3,7 +3,7 @@ from __future__ import annotations
 
 import json
 import os
-from typing import Dict
+from typing import Dict, Optional
 
 import torch
 
@@ -18,8 +18,11 @@ def _normal(gen: torch.Generator, shape, std: float, dtype, device) -> torch.Ten
     return t.to(device=device, dtype=dtype)
 
 
-def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, device="cpu") -> Dict[str, torch.Tensor]:
-    """HF parameter names for BertModel (no prefix) / LlamaForCausalLM, init N(0, initializer_range), LN = (1, 0)."""
+def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, device="cpu",
+                      bias_std: Optional[float] = None) -> Dict[str, torch.Tensor]:
+    """HF parameter names for BertModel (no prefix) / LlamaForCausalLM / Qwen2ForCausalLM / FalconForCausalLM, init
+    N(0, initializer_range), LN = (1, 0). Decoder attention biases (Qwen2's q/k/v, Llama's `attention_bias`) are drawn from
+    N(0, bias_std) (default: initializer_range) rather than HF's zeros, so that a dropped bias changes the outputs."""
     on_device = torch.device(device).type == "cuda" and cfg.get("_device_rng", False)
     gen = torch.Generator(device=device) if on_device else torch.Generator()
     gen.manual_seed(seed)
@@ -52,10 +55,12 @@ def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, 
             sd[p + "output.LayerNorm.bias"] = _normal(gen, (H,), std, dtype, device)
         sd["pooler.dense.weight"] = _normal(gen, (H, H), std, dtype, device)   # loaded by AutoModel, unused by the path
         sd["pooler.dense.bias"] = zeros(H)
-    elif kind == "llama":
+    elif kind in ("llama", "qwen2"):
         F, V = cfg["intermediate_size"], cfg["vocab_size"]
         nh, nkv = cfg["num_attention_heads"], cfg.get("num_key_value_heads", cfg["num_attention_heads"])
-        hd = cfg.get("head_dim", H // nh)
+        hd = cfg.get("head_dim") or H // nh
+        qkv_bias, o_bias = attention_biases(kind, cfg)
+        bstd = std if bias_std is None else float(bias_std)
         sd["model.embed_tokens.weight"] = _normal(gen, (V, H), std, dtype, device)
         for l in range(cfg["num_hidden_layers"]):
             p = f"model.layers.{l}."
@@ -63,13 +68,20 @@ def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, 
             sd[p + "self_attn.k_proj.weight"] = _normal(gen, (nkv * hd, H), std, dtype, device)
             sd[p + "self_attn.v_proj.weight"] = _normal(gen, (nkv * hd, H), std, dtype, device)
             sd[p + "self_attn.o_proj.weight"] = _normal(gen, (H, nh * hd), std, dtype, device)
+            if qkv_bias:
+                sd[p + "self_attn.q_proj.bias"] = _normal(gen, (nh * hd,), bstd, dtype, device)
+                sd[p + "self_attn.k_proj.bias"] = _normal(gen, (nkv * hd,), bstd, dtype, device)
+                sd[p + "self_attn.v_proj.bias"] = _normal(gen, (nkv * hd,), bstd, dtype, device)
+            if o_bias:
+                sd[p + "self_attn.o_proj.bias"] = _normal(gen, (H,), bstd, dtype, device)
             sd[p + "mlp.gate_proj.weight"] = _normal(gen, (F, H), std, dtype, device)
             sd[p + "mlp.up_proj.weight"] = _normal(gen, (F, H), std, dtype, device)
             sd[p + "mlp.down_proj.weight"] = _normal(gen, (H, F), std, dtype, device)
             sd[p + "input_layernorm.weight"] = ones(H) + _normal(gen, (H,), std, dtype, device)
             sd[p + "post_attention_layernorm.weight"] = ones(H) + _normal(gen, (H,), std, dtype, device)
         sd["model.norm.weight"] = ones(H) + _normal(gen, (H,), std, dtype, device)
-        sd["lm_head.weight"] = _normal(gen, (V, H), std, dtype, device)
+        if not cfg.get("tie_word_embeddings", False):             # tied checkpoints store no lm_head (Qwen2 0.5B-3B)
+            sd["lm_head.weight"] = _normal(gen, (V, H), std, dtype, device)
     elif kind == "falcon":
         V = cfg["vocab_size"]
         nh = cfg["num_attention_heads"]
@@ -129,15 +141,49 @@ def load_state_dict(path: str) -> Dict[str, torch.Tensor]:
 
 
 def model_kind(cfg: Dict) -> str:
+    """the engine family of an HF config; raises for model types, and for variants of the built ones, that are not built"""
     mt = cfg.get("model_type", "")
     if mt == "bert":
         return "bert"
-    if mt == "llama":
-        return "llama"
+    if mt in ("llama", "qwen2"):
+        check_llama_family(cfg)
+        return mt
     if mt == "falcon":
         return "falcon"
     raise NotImplementedError(
-        f"model_type {mt!r} is not built in dalm_b200 (supported: bert encoders; llama and falcon decoders); see DESIGN.md")
+        f"model_type {mt!r} is not built in dalm_b200 (supported: bert encoders; llama, qwen2 and falcon decoders)")
+
+
+def _rope_type(cfg: Dict) -> str:
+    for key in ("rope_scaling", "rope_parameters"):
+        rp = cfg.get(key)
+        if isinstance(rp, dict):
+            t = rp.get("rope_type", rp.get("type"))
+            if t not in (None, "default"):
+                return str(t)
+    return "default"
+
+
+def check_llama_family(cfg: Dict) -> None:
+    """refuses the settings of a llama / qwen2 config that LlamaDecoder would otherwise silently compute wrong"""
+    mt = cfg.get("model_type", "")
+    if cfg.get("mlp_bias", False):
+        raise NotImplementedError(f"{mt}: mlp_bias=true is not built (the fused SwiGLU MLP has no bias)")
+    if mt == "qwen2":
+        if cfg.get("use_sliding_window", False) or "sliding_attention" in (cfg.get("layer_types") or ()):
+            raise NotImplementedError("qwen2: sliding-window attention (use_sliding_window=true) is not built")
+        rt = _rope_type(cfg)
+        if rt != "default":
+            raise NotImplementedError(f"qwen2: RoPE type {rt!r} (rope_scaling / rope_parameters) is not built; only 'default'")
+
+
+def attention_biases(kind: str, cfg: Dict):
+    """(q/k/v projections carry a bias, o_proj carries a bias) for a llama-family config: Qwen2 has q/k/v biases only, Llama
+    has all four when `attention_bias` is set"""
+    if kind == "qwen2":
+        return True, False
+    ab = bool(cfg.get("attention_bias", False))
+    return ab, ab
 
 
 def is_bnb_linear_weight(name: str) -> bool:

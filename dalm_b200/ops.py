@@ -510,22 +510,31 @@ def gemm_gelu(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = N
     return pre, act
 
 
+def _chk_bias(bias: Optional[torch.Tensor], N: int, what: str) -> None:
+    if bias is not None:
+        _chk(bias, f32, what)
+        if bias.dim() != 1 or bias.shape[0] < N or not bias.is_contiguous():
+            raise _lib.DalmB200Error(f"{what}: need a contiguous fp32 vector of at least {N} elements, got {tuple(bias.shape)}")
+
+
 def gemm_rope(a: torch.Tensor, w: torch.Tensor, cos_t: torch.Tensor, sin_t: torch.Tensor, L: int, rope_cols: int,
-              out: Optional[torch.Tensor] = None) -> torch.Tensor:
+              out: Optional[torch.Tensor] = None, bias: Optional[torch.Tensor] = None) -> torch.Tensor:
     """q|k|v projection with RoPE (head_dim 128) on the first `rope_cols` output columns fused into the GEMM epilogue.
-    a [M,K], w [N,K] bf16; cos_t / sin_t fp32 [L, 64]; rows are token-major (position = row % L)."""
+    a [M,K], w [N,K] bf16; cos_t / sin_t fp32 [L, 64]; rows are token-major (position = row % L). bias: fp32 [N], added in fp32
+    before the rotation (Qwen2's q/k/v biases)."""
     _chk(a, bf16, "gemm_rope a"); _chk(w, bf16, "gemm_rope w"); _chk(cos_t, f32, "gemm_rope cos"); _chk(sin_t, f32, "gemm_rope sin")
     M, K = a.shape
     N = w.shape[0]
+    _chk_bias(bias, N, "gemm_rope bias")
     if cos_t.shape != (L, 64) or sin_t.shape != (L, 64) or not cos_t.is_contiguous() or not sin_t.is_contiguous():
         raise _lib.DalmB200Error("gemm_rope: cos / sin must be contiguous fp32 [L, 64] (head_dim 128)")
     if out is None:
         out = torch.empty(M, N, dtype=bf16, device=a.device)
     timer = GEMM_TIMER
     if timer is not None:
-        timer.begin(2.0 * M * N * K, (M, N, K, 0, "bfloat16", "rope", "-"))
-    _lib.call("dalm_b200_gemm_bf16_rope", _p(a), _ld(a), _p(w), _ld(w), _p(out), _ld(out), M, N, K, _p(cos_t), _p(sin_t), int(L),
-              int(rope_cols), _stream())
+        timer.begin(2.0 * M * N * K, (M, N, K, 0, "bfloat16", "rope", "bias" if bias is not None else "-"))
+    _lib.call("dalm_b200_gemm_bf16_rope", _p(a), _ld(a), _p(w), _ld(w), _p(out), _ld(out), M, N, K, _p(bias), _p(cos_t), _p(sin_t),
+              int(L), int(rope_cols), _stream())
     if timer is not None:
         timer.end()
     return out
@@ -742,30 +751,32 @@ def nf4_roundtrip_(w: torch.Tensor, want_codes: bool = False):
 # greedy decoding (evaluation: reference dalm/eval/eval_rag.py:126-140)
 # ----------------------------------------------------------------------------------------------------------------
 def decode_gemm(a: torch.Tensor, w: torch.Tensor, out: Optional[torch.Tensor] = None, *, out_dtype=bf16, act: int = 0,
-                resid: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """out[M,N] = act(a[M,K] @ w[N,K]^T) + resid for the M <= 16 token rows of a decode step: weight-streaming kernel, every
-    weight read once. a, w bf16 with contiguous rows (row strides multiples of 8); resid / out bf16 or fp32."""
+                resid: Optional[torch.Tensor] = None, bias: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out[M,N] = act(a[M,K] @ w[N,K]^T + bias) + resid for the M <= 16 token rows of a decode step: weight-streaming kernel,
+    every weight read once. a, w bf16 with contiguous rows (row strides multiples of 8); bias fp32 [N]; resid / out bf16 or fp32."""
     _chk(a, bf16, "decode_gemm a"); _chk(w, bf16, "decode_gemm w")
     M, K = a.shape
     N = w.shape[0]
     if w.shape[1] != K:
         raise _lib.DalmB200Error(f"decode_gemm: a is [{M},{K}] but w is {tuple(w.shape)}")
+    _chk_bias(bias, N, "decode_gemm bias")
     if out is None:
         out = torch.empty(M, N, dtype=out_dtype, device=a.device)
     if out.dtype not in (bf16, f32) or (resid is not None and resid.dtype not in (bf16, f32)):
         raise _lib.DalmB200Error("decode_gemm: out / resid must be bf16 or fp32")
-    _lib.call("dalm_b200_decode_gemm", _p(a), _ld(a), _p(w), _ld(w), _p(out), _ld(out), 1 if out.dtype == f32 else 0, _p(resid),
+    _lib.call("dalm_b200_decode_gemm", _p(a), _ld(a), _p(w), _ld(w), _p(out), _ld(out), 1 if out.dtype == f32 else 0, _p(bias), _p(resid),
               _ld(resid) if resid is not None else 0, 1 if (resid is not None and resid.dtype == f32) else 0, int(act), M, N, K,
               _stream())
     return out
 
 
-def gemm_rows(a: torch.Tensor, w: torch.Tensor, *, out_dtype=bf16, act: int = 0, resid: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """a[M,K] @ w[N,K]^T for a decode step: up to 16 rows go through the weight-streaming `decode_gemm` (the 128-row wgmma
-    tile would be 7/8 empty), larger batches through the training GEMM. DALM_B200_DECODE_GEMM=0 forces the latter."""
+def gemm_rows(a: torch.Tensor, w: torch.Tensor, *, out_dtype=bf16, act: int = 0, resid: Optional[torch.Tensor] = None,
+              bias: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """act(a[M,K] @ w[N,K]^T + bias) + resid for a decode step: up to 16 rows go through the weight-streaming `decode_gemm` (the
+    128-row wgmma tile would be 7/8 empty), larger batches through the training GEMM. DALM_B200_DECODE_GEMM=0 forces the latter."""
     if a.shape[0] <= 16 and os.environ.get("DALM_B200_DECODE_GEMM", "1") != "0":
-        return decode_gemm(a, w, out_dtype=out_dtype, act=act, resid=resid)
-    return gemm(a, w, out_dtype=out_dtype, act=act, resid=resid)
+        return decode_gemm(a, w, out_dtype=out_dtype, act=act, resid=resid, bias=bias)
+    return gemm(a, w, out_dtype=out_dtype, act=act, resid=resid, bias=bias)
 
 
 def rope_pos_(buf, col0: int, nheads: int, D: int, cos_t, sin_t, pos):

@@ -34,6 +34,16 @@ LLAMA_SHAPES: Dict[str, Dict] = {
 }
 
 
+QWEN2_SHAPES: Dict[str, Dict] = {
+    "qwen2-tiny": dict(hidden_size=896, num_hidden_layers=2, num_attention_heads=14, num_key_value_heads=2,
+                       intermediate_size=1152, tie_word_embeddings=True),                  # head_dim 64: un-fused RoPE
+    "qwen2-hd128": dict(hidden_size=1536, num_hidden_layers=2, num_attention_heads=12, num_key_value_heads=2,
+                        intermediate_size=2048, tie_word_embeddings=False),                # head_dim 128: RoPE in the QKV epilogue
+    "qwen2.5-7b": dict(hidden_size=3584, num_hidden_layers=28, num_attention_heads=28, num_key_value_heads=4,
+                       intermediate_size=18944, tie_word_embeddings=False),
+}
+
+
 FALCON_SHAPES: Dict[str, Dict] = {
     "falcon-tiny": dict(hidden_size=128, num_hidden_layers=2, num_attention_heads=2),
     "falcon-mini": dict(hidden_size=448, num_hidden_layers=2, num_attention_heads=7),          # 7 q heads x 64, one KV head
@@ -67,6 +77,17 @@ def llama_config(name: str, vocab_size: int = 32000) -> Dict:
         hidden_act="silu", rms_norm_eps=1e-5, rope_theta=10000.0, initializer_range=0.02, bos_token_id=1, eos_token_id=2,
         tie_word_embeddings=False, attention_bias=False, mlp_bias=False, attention_dropout=0.0,
         head_dim=s["hidden_size"] // s["num_attention_heads"], **s,
+    )
+
+
+def qwen2_config(name: str, vocab_size: int = 152064) -> Dict:
+    """Qwen2 / Qwen2.5 (HF Qwen2ForCausalLM): Llama plus q/k/v biases, rope_theta 1e6, rms_norm_eps 1e-6; full attention on
+    every layer (use_sliding_window false, as in the published checkpoints)"""
+    s = QWEN2_SHAPES[name]
+    return dict(
+        architectures=["Qwen2ForCausalLM"], model_type="qwen2", vocab_size=vocab_size, max_position_embeddings=32768,
+        hidden_act="silu", rms_norm_eps=1e-6, rope_theta=1000000.0, initializer_range=0.02, bos_token_id=0, eos_token_id=0,
+        use_sliding_window=False, sliding_window=None, max_window_layers=s["num_hidden_layers"], attention_dropout=0.0, **s,
     )
 
 
@@ -177,13 +198,51 @@ def build_llama_tokenizer(out_dir: str, vocab_size: int = 32000) -> str:
     return out_dir
 
 
+QWEN2_SPECIAL = ["<|endoftext|>", "<|im_start|>", "<|im_end|>"]
+
+
+def build_qwen2_tokenizer(out_dir: str, vocab_size: int = 152064) -> str:
+    """Qwen2-style byte-level BPE (GPT-2 byte alphabet, no BOS) trained on the synthetic corpus and wrapped in transformers'
+    Qwen2Tokenizer; the ChatML specials <|endoftext|> / <|im_start|> / <|im_end|> are ids 0-2, <|endoftext|> is pad and eos"""
+    from tokenizers import Tokenizer, models, pre_tokenizers, trainers
+    from transformers import Qwen2Tokenizer
+
+    tok = Tokenizer(models.BPE())
+    tok.pre_tokenizer = pre_tokenizers.ByteLevel(add_prefix_space=False)
+    trainer = trainers.BpeTrainer(vocab_size=min(vocab_size, 6000), special_tokens=QWEN2_SPECIAL, show_progress=False,
+                                  initial_alphabet=pre_tokenizers.ByteLevel.alphabet())
+    tok.train_from_iterator(_corpus(), trainer)
+    vocab = tok.get_vocab()
+    model_json = json.loads(tok.to_str())["model"]
+    merges = [tuple(m) if isinstance(m, list) else tuple(m.split(" ")) for m in model_json["merges"]]
+    nxt = len(vocab)
+    while nxt < vocab_size:
+        vocab[f"<|extra_{nxt}|>"] = nxt
+        nxt += 1
+    qt = Qwen2Tokenizer(vocab=vocab, merges=merges, unk_token=None, eos_token="<|endoftext|>", pad_token="<|endoftext|>",
+                        additional_special_tokens=["<|im_start|>", "<|im_end|>"], model_max_length=32768)
+    os.makedirs(out_dir, exist_ok=True)
+    qt.save_pretrained(out_dir)
+    return out_dir
+
+
+# base Qwen2.5 checkpoints decode greedily; the Instruct ones sample with a repetition penalty (their generation_config.json)
+QWEN2_GENERATION = {
+    "base": dict(bos_token_id=0, eos_token_id=0, do_sample=False, max_new_tokens=2048),
+    "instruct": dict(bos_token_id=0, eos_token_id=[2, 0], pad_token_id=0, do_sample=True, repetition_penalty=1.05,
+                     temperature=0.7, top_p=0.8, top_k=20),
+}
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # model directories
 # ---------------------------------------------------------------------------------------------------------------
 def write_model_dir(out_dir: str, kind: str, name: str, vocab_size: Optional[int] = None, with_weights: bool = True,
-                    seed: int = 0) -> str:
-    """kind: 'bert' | 'llama'. Writes config.json, tokenizer files and (optionally) seeded random-init safetensors in HF
-    parameter naming so both transformers (oracle) and dalm_b200 (product) can load the same directory."""
+                    seed: int = 0, generation_config: Optional[Dict] = None, bias_std: Optional[float] = None) -> str:
+    """kind: 'bert' | 'llama' | 'qwen2' | 'falcon'. Writes config.json, tokenizer files and (optionally) seeded random-init
+    safetensors in HF parameter naming so both transformers (oracle) and dalm_b200 (product) can load the same directory.
+    generation_config: written as generation_config.json when given (e.g. QWEN2_GENERATION["base"]). bias_std: std of the
+    random attention biases (engine/params.random_state_dict)."""
     os.makedirs(out_dir, exist_ok=True)
     if kind == "bert":
         cfg = bert_config(name, vocab_size or 30522)
@@ -191,6 +250,9 @@ def write_model_dir(out_dir: str, kind: str, name: str, vocab_size: Optional[int
     elif kind == "llama":
         cfg = llama_config(name, vocab_size or 32000)
         build_llama_tokenizer(out_dir, cfg["vocab_size"])
+    elif kind == "qwen2":
+        cfg = qwen2_config(name, vocab_size or 152064)
+        build_qwen2_tokenizer(out_dir, cfg["vocab_size"])
     elif kind == "falcon":
         cfg = falcon_config(name, vocab_size or 65024)
         build_llama_tokenizer(out_dir, cfg["vocab_size"])       # any causal-LM tokenizer works for the synthetic fixture
@@ -198,6 +260,9 @@ def write_model_dir(out_dir: str, kind: str, name: str, vocab_size: Optional[int
         raise ValueError(kind)
     with open(os.path.join(out_dir, "config.json"), "w") as f:
         json.dump(cfg, f, indent=1)
+    if generation_config is not None:
+        with open(os.path.join(out_dir, "generation_config.json"), "w") as f:
+            json.dump(generation_config, f, indent=1)
     if not with_weights:
         with open(os.path.join(out_dir, "dalm_b200_random_init.json"), "w") as f:      # engine/params.py: random init at load time
             json.dump({"seed": seed}, f)
@@ -207,6 +272,6 @@ def write_model_dir(out_dir: str, kind: str, name: str, vocab_size: Optional[int
 
         from .engine.params import random_state_dict
 
-        sd = random_state_dict(kind, cfg, seed=seed, dtype=torch.float32, device="cpu")
+        sd = random_state_dict(kind, cfg, seed=seed, dtype=torch.float32, device="cpu", bias_std=bias_std)
         save_file({k: v.contiguous() for k, v in sd.items()}, os.path.join(out_dir, "model.safetensors"))
     return out_dir

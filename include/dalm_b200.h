@@ -92,9 +92,11 @@ int dalm_b200_gemm_bf16(int layout, const void* A, long long lda, const void* B,
 int dalm_b200_gemm_bf16_swiglu(const void* A, long long lda, const void* B, long long ldb, void* gu, long long ldgu, void* act,
                                long long ldact, int M, int N, int K, void* stream);
 /* fused q|k|v projection + rotary position embedding (HF rotate_half, head_dim 128) on output columns [0, rope_cols); cos / sin
- * fp32 [L, 64]; output row m is at position m % L. Replaces q_proj / k_proj / v_proj + apply_rotary_pos_emb of HF LlamaAttention. */
+ * fp32 [L, 64]; output row m is at position m % L. Replaces q_proj / k_proj / v_proj + apply_rotary_pos_emb of HF LlamaAttention.
+ * bias: fp32 [N] or NULL (Qwen2's q/k/v biases): added to the fp32 accumulator before the rotation and the single bf16 rounding,
+ * on every column; NULL leaves the results bit-identical to a bias-free projection. */
 int dalm_b200_gemm_bf16_rope(const void* A, long long lda, const void* B, long long ldb, void* out, long long ldo, int M, int N,
-                             int K, const float* cos_t, const float* sin_t, int L, int rope_cols, void* stream);
+                             int K, const float* bias, const float* cos_t, const float* sin_t, int L, int rope_cols, void* stream);
 /* gemm_bf16_swiglu_bwd: LlamaMLP backward through down_proj and act_fn(gate) * up in one launch: d(act)[M,F] = dY[M,K] WdT[F,K]^T
  * never reaches HBM; gu [M,2F] (gate|up interleaved in 128-feature blocks, as gemm_bf16_swiglu left it) is overwritten in place with
  * [d gate | d up]. Bit-identical to gemm_bf16 followed by swiglu_bwd (interleave 128). */
@@ -242,11 +244,12 @@ int dalm_b200_nf4_dequant_bf16(const void* packed, const float* absmax, long lon
  * Device-column mode (cur_dev != NULL, int32 [B]): attention_decode takes cur = cur_dev[b], greedy_step writes column
  *   cur_dev[b] + 1 and advances cur_dev[b]; the host `cur` / `col` arguments are ignored, so the launch sequence of a
  *   decode step has identical arguments for every token and can be captured once in a CUDA graph and replayed. */
-/* decode_gemm: out[M,N] = act(A[M,K] W[N,K]^T) + resid for the M <= 16 token rows of a decode step (every nn.Linear of the
- *   generator once per generated token): weight-streaming mma.sync kernel, each weight read once. act 0 none / 1 gelu;
- *   out / resid bf16 or fp32 (resid may be NULL). */
+/* decode_gemm: out[M,N] = act(A[M,K] W[N,K]^T + bias) + resid for the M <= 16 token rows of a decode step (every nn.Linear of
+ *   the generator once per generated token): weight-streaming mma.sync kernel, each weight read once. act 0 none / 1 gelu;
+ *   bias fp32 [N] or NULL; out / resid bf16 or fp32 (resid may be NULL). Same order of operations as gemm_bf16. */
 int dalm_b200_decode_gemm(const void* A, long long lda, const void* W, long long ldw, void* out, long long ldo, int out_f32,
-                          const void* resid, long long ldr, int resid_f32, int act, int M, int N, int K, void* stream);
+                          const float* bias, const void* resid, long long ldr, int resid_f32, int act, int M, int N, int K,
+                          void* stream);
 int dalm_b200_rope_pos(void* buf, long long ld, int col0, int nheads, int D, const float* cos_t, const float* sin_t,
                        const int64_t* pos, int M, int T, void* stream);
 int dalm_b200_attention_decode(const void* qkv, long long ldq, int q_col, int k_col, int v_col, void* cache_k, void* cache_v,

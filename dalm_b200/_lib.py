@@ -33,7 +33,6 @@ SIGNATURES = {
     "dalm_b200_dropout_scale": [_P, _L, _F, _U, _U, _P, _P],
     "dalm_b200_lora_dx": [_P, _L, _P, _L, _P, _L, _I, _I, _I, _F, _U, _U, _P, _P],
     "dalm_b200_small_matmul_f32": [_P, _P, _P, _I, _I, _I, _I, _I, _F, _P],
-    "dalm_b200_gemm_bf16_tn": [_P, _L, _P, _L, _P, _L, _I, _I, _I, _I, _F, _P, _I, _P, _L, _I, _I, _I, *_DROP, _P],
     "dalm_b200_gemm_bf16": [_I, _P, _L, _P, _L, _P, _L, _I, _I, _I, _I, _F, _P, _I, _P, _L, _I, _I, _I, *_DROP, _P],
     "dalm_b200_gemm_clear_cache": [],
     "dalm_b200_gemm_set_raster": [_I],
@@ -56,7 +55,6 @@ SIGNATURES = {
     "dalm_b200_swiglu_bwd": [_P, _L, _P, _L, _I, _I, _I, _P],
     "dalm_b200_gemm_bf16_swiglu": [_P, _L, _P, _L, _P, _L, _P, _L, _I, _I, _I, _P],
     "dalm_b200_gemm_bf16_rope": [_P, _L, _P, _L, _P, _L, _I, _I, _I, _P, _P, _P, _I, _I, _P],
-    "dalm_b200_gemm_bf16_swiglu_bwd": [_P, _L, _P, _L, _P, _L, _I, _I, _I, _P],
     "dalm_b200_gemm_bf16_gelu": [_P, _L, _P, _L, _P, _L, _P, _L, _I, _I, _I, _P, _P],
     "dalm_b200_gelu_fwd": [_P, _L, _P, _L, _I, _I, _P],
     "dalm_b200_gelu_bwd": [_P, _L, _P, _L, _I, _I, _P],

@@ -14,8 +14,6 @@
 // each row's current column) lives in device memory: a decode step is then the SAME launch sequence with the same
 // arguments for every token and can be captured once as a CUDA graph and replayed (292 launches per token at Llama-2-7B).
 // The host reads back one "is anyone still generating" counter every few steps.
-// A decode step's cost grows with the cached tokens through attn_decode_kernel's PV pass (pass 3 below walks the keys serially
-// per thread, one dependent 2-byte load each); attn_decode_par_kernel below parallelises that pass and is the default.
 #include "common.cuh"
 #include <limits.h>
 #include <stdlib.h>
@@ -41,10 +39,22 @@ __global__ void rope_pos_kernel(__nv_bfloat16* __restrict__ buf, long long ld, i
   }
 }
 
-// grid (Hq, B), 128 threads. Shared memory: q[D] | p[cur+1] | red[32] | part[128] floats.
+// one explicit 16-byte read-only load -> 8 floats (struct-typed bf16x8 loads are split into 32-bit loads by the compiler)
+__device__ __forceinline__ void load8_nc(const __nv_bfloat16* p, float* f) {
+  const uint4 u = __ldg(reinterpret_cast<const uint4*>(p));
+  const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float2 t = __bfloat1622float2(h[i]);
+    f[2 * i] = t.x; f[2 * i + 1] = t.y;
+  }
+}
+
+// grid (Hq, B), 128 threads. Shared memory: q[D] | p[sp_cap] | red[32] | part[1024] floats.
 //   pass 1: thread-per-key scores (each thread reads whole K rows with 16-byte loads, q broadcast from smem)
 //   pass 2: block max / exp / sum
-//   pass 3: thread-per-output-column PV (128 / D thread groups split the keys, combined through smem)
+//   pass 3: PV with 128 threads = KG key groups x D/8 lanes; every lane loads 16 bytes of V unconditionally (masked keys
+//           carry p = 0; their cache rows are initialised memory) and the KG partial rows meet in shared memory
 template <int D>
 __global__ void __launch_bounds__(128) attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, long long ldq, int q_col,
                                                           int k_col, int v_col, __nv_bfloat16* __restrict__ cache_k,
@@ -58,6 +68,7 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const __nv_bfloat16* _
   float* sp = sm + D;
   float* red = sp + sp_cap;                      // sp_cap >= cur + 1, a multiple of 4 (host-side: the cache length in
   float* part = red + 32;                        // device-column mode, so one captured launch serves every step)
+                                                 // part = [KG][D] = 1024 floats for every supported D
   const int h = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
   const int cur = cur_dev ? min(cur_dev[b], sp_cap - 1) : cur_host;
   const int group = Hq / Hkv, kvh = h / group;
@@ -80,100 +91,6 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const __nv_bfloat16* _
     // column `cur` is the token being decoded: always visible, read from the qkv row (its cache slot is written above
     // by ANOTHER CTA of this launch, so nobody reads it back here)
     const bool valid = (t == cur) || mask[(size_t)b * ldm + t] != 0;
-    float s = -INFINITY;
-    if (valid) {
-      const __nv_bfloat16* kp = (t == cur) ? krow : ck + (size_t)t * cache_st;
-      s = 0.f;
-#pragma unroll
-      for (int j = 0; j < D; j += 8) {
-        float f[8];
-        unpack8(*reinterpret_cast<const bf16x8*>(kp + j), f);
-#pragma unroll
-        for (int e = 0; e < 8; ++e) s += sq[j + e] * f[e];
-      }
-    }
-    sp[t] = s;
-    lmax = fmaxf(lmax, s);
-  }
-  const float m = block_max(lmax, red);         // finite: column `cur` is always valid
-  float lsum = 0.f;
-  for (int t = tid; t <= cur; t += 128) {
-    const float s = sp[t];
-    const float p = (s == -INFINITY) ? 0.f : __expf(s - m);
-    sp[t] = p;
-    lsum += p;
-  }
-  const float sum = block_sum(lsum, red);
-  __syncthreads();
-
-  constexpr int G = 128 / D;                    // thread groups splitting the keys: 1 (D=128), 2 (64), 4 (32)
-  const int d = tid % D, g = tid / D;
-  float acc = 0.f;
-  for (int t = g; t <= cur; t += G) {
-    const float p = sp[t];
-    if (p != 0.f) {
-      const __nv_bfloat16* vp = (t == cur) ? vrow : cv + (size_t)t * cache_st;
-      acc += p * __bfloat162float(vp[d]);
-    }
-  }
-  if (G > 1) {
-    part[tid] = acc;
-    __syncthreads();
-    if (g == 0)
-      for (int gg = 1; gg < G; ++gg) acc += part[gg * D + d];
-  }
-  if (g == 0) out[(size_t)b * ldo + h * D + d] = __float2bfloat16(acc / sum);
-}
-
-// DEFAULT decode attention: the kernel above with a parallel PV pass (the first kernel's pass 3 walks the keys serially per
-// thread with the V load behind `if (p != 0)`). Here 128 threads = KG key groups x D/8 lanes, every lane loads 16 bytes of V unconditionally
-// (masked keys carry p = 0; their cache rows are initialised memory) and the KG partial rows meet in shared memory.
-// DALM_B200_DECODE_ATTN=1 selects the first
-// kernel (kept as the cross-check of tests/test_generate_gpu.py).
-// one explicit 16-byte read-only load -> 8 floats (the struct-typed loads above are split into 32-bit loads by the compiler)
-__device__ __forceinline__ void load8_nc(const __nv_bfloat16* p, float* f) {
-  const uint4 u = __ldg(reinterpret_cast<const uint4*>(p));
-  const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const float2 t = __bfloat1622float2(h[i]);
-    f[2 * i] = t.x; f[2 * i + 1] = t.y;
-  }
-}
-
-template <int D>
-__global__ void __launch_bounds__(128) attn_decode_v2_kernel(const __nv_bfloat16* __restrict__ qkv, long long ldq, int q_col,
-                                                             int k_col, int v_col, __nv_bfloat16* __restrict__ cache_k,
-                                                             __nv_bfloat16* __restrict__ cache_v, long long cache_sb,
-                                                             long long cache_st, const int64_t* __restrict__ mask,
-                                                             long long ldm, __nv_bfloat16* __restrict__ out, long long ldo,
-                                                             int Hq, int Hkv, int cur_host, const int* __restrict__ cur_dev,
-                                                             int sp_cap, float scale) {
-  extern __shared__ float sm[];
-  float* sq = sm;
-  float* sp = sm + D;
-  float* red = sp + sp_cap;
-  float* part = red + 32;                        // [KG][D] = 1024 floats for every supported D
-  const int h = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
-  const int cur = cur_dev ? min(cur_dev[b], sp_cap - 1) : cur_host;
-  const int group = Hq / Hkv, kvh = h / group;
-  const __nv_bfloat16* qrow = qkv + (size_t)b * ldq + q_col + h * D;
-  const __nv_bfloat16* krow = qkv + (size_t)b * ldq + k_col + kvh * D;
-  const __nv_bfloat16* vrow = qkv + (size_t)b * ldq + v_col + kvh * D;
-  __nv_bfloat16* ck = cache_k + (size_t)b * cache_sb + kvh * D;
-  __nv_bfloat16* cv = cache_v + (size_t)b * cache_sb + kvh * D;
-  if (tid < D) {
-    sq[tid] = __bfloat162float(qrow[tid]) * scale;
-    if (h % group == 0) {
-      ck[(size_t)cur * cache_st + tid] = krow[tid];
-      cv[(size_t)cur * cache_st + tid] = vrow[tid];
-    }
-  }
-  __syncthreads();
-
-  float lmax = -INFINITY;
-  for (int t = tid; t <= cur; t += 128) {
-    const bool valid = (t == cur) || mask[(size_t)b * ldm + t] != 0;
     const __nv_bfloat16* kp = (t == cur) ? krow : ck + (size_t)t * cache_st;
     float s = 0.f;
 #pragma unroll
@@ -187,7 +104,7 @@ __global__ void __launch_bounds__(128) attn_decode_v2_kernel(const __nv_bfloat16
     sp[t] = s;
     lmax = fmaxf(lmax, s);
   }
-  const float m = block_max(lmax, red);
+  const float m = block_max(lmax, red);         // finite: column `cur` is always valid
   float lsum = 0.f;
   for (int t = tid; t <= cur; t += 128) {
     const float s = sp[t];
@@ -722,21 +639,8 @@ extern "C" int dalm_b200_attention_decode(const void* qkv, long long ldq, int q_
                "attention_decode: pointers must be 16-byte aligned");
   DALM_REQUIRE(mask != nullptr && cache_st >= (long long)Hkv * D && cache_sb >= cache_st * T, "attention_decode: cache layout");
   const int sp_cap = ((cur_dev ? T : cur + 1) + 3) & ~3;
-  const char* variant = getenv("DALM_B200_DECODE_ATTN");
-  const bool v2 = !(variant != nullptr && variant[0] == '1');       // default: parallel-PV kernel; 1 = the first (serial-PV) kernel
-  const size_t smem = (size_t)(D + sp_cap + 32 + (v2 ? 1024 : 128)) * sizeof(float);
+  const size_t smem = (size_t)(D + sp_cap + 32 + 1024) * sizeof(float);
   dim3 grid(Hq, B);
-  if (v2) {
-#define DALM_DECODE2(DD)                                                                                                 \
-  attn_decode_v2_kernel<DD><<<grid, 128, smem, ST(stream)>>>((const __nv_bfloat16*)qkv, ldq, q_col, k_col, v_col,        \
-                                                             (__nv_bfloat16*)cache_k, (__nv_bfloat16*)cache_v, cache_sb, \
-                                                             cache_st, mask, ldm, (__nv_bfloat16*)out, ldo, Hq, Hkv, cur, \
-                                                             cur_dev, sp_cap, scale)
-    if (D == 128) DALM_DECODE2(128); else if (D == 64) DALM_DECODE2(64); else DALM_DECODE2(32);
-#undef DALM_DECODE2
-    count_launch();
-    return check_launch("attn_decode_v2_kernel");
-  }
 #define DALM_DECODE(DD)                                                                                                  \
   attn_decode_kernel<DD><<<grid, 128, smem, ST(stream)>>>((const __nv_bfloat16*)qkv, ldq, q_col, k_col, v_col,           \
                                                           (__nv_bfloat16*)cache_k, (__nv_bfloat16*)cache_v, cache_sb,    \

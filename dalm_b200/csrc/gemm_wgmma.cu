@@ -16,6 +16,17 @@
 namespace dalm {
 using namespace ptx;
 
+// Epilogue kind, a template parameter of the kernel: each fused entry point launches its own instance, and the plain
+// instances carry no fused code.
+enum class Epi {
+  Plain,     // out = act(alpha * acc + bias) (+ dropout) + resid                                        (gemm_bf16)
+  SwiGLU,    // tile columns [0,128) = gate, [128,256) = up of the same 128 features (weight rows interleaved); besides
+             // `out` (gate|up, the backward's input) the tile's silu(gate) * up goes to tmap_out2        (gemm_bf16_swiglu)
+  RoPE,      // rotary position embedding (head_dim 128, HF rotate_half) on output columns < rope_cols    (gemm_bf16_rope)
+  GeluPair,  // `out` = pre-activation (bf16, what the backward needs), tmap_out2 = gelu(pre) (bf16, the next GEMM's
+             // operand): one launch instead of GEMM + a 2-pass kernel                                     (gemm_bf16_gelu)
+};
+
 struct GemmEpilogue {
   void* out;            // [M, ldo]
   long long ldo;
@@ -30,15 +41,7 @@ struct GemmEpilogue {
   int M, N, K;
   DropCfg drop;         // dropout on act(alpha*acc+bias) BEFORE the residual add (BertSelfOutput / BertOutput); p = 0 => off
   int group_m;          // tile rasterisation: bands of group_m m-tiles, n-tiles walked serpentine inside a band (0 = m-fastest)
-  int fuse;             // 0: none; 1: SwiGLU forward - tile columns [0,128) = gate, [128,256) = up of the same 128 features (weight
-                        // rows interleaved); besides `out` (gate|up, the backward's input) the tile's silu(gate)*up goes to tmap_out2
-                        // 2: rotary position embedding (head_dim 128, HF rotate_half) on output columns < rope_cols
-                        // 4: SwiGLU backward in the down-projection's dgrad: the accumulator is d(act) [M,F]; with gate / up read from
-                        //    `resid` (= the interleaved gate|up buffer [M,2F], which is also `out`) the tile leaves as
-                        //    d gate = d act * up * s(g)(1 + g(1 - s(g))) and d up = d act * silu(g), written in place over gate / up
-                        // 3: GELU forward with both tensors kept - `out` = pre-activation (bf16, what the backward needs),
-                        //    tmap_out2 = gelu(pre) (bf16, the next GEMM's operand): one launch instead of GEMM + a 2-pass kernel
-  const float* rope_cos; const float* rope_sin;   // fuse == 2: fp32 [rope_L, 64]; the position of output row m is m % rope_L
+  const float* rope_cos; const float* rope_sin;   // Epi::RoPE: fp32 [rope_L, 64]; the position of output row m is m % rope_L
   int rope_L, rope_cols;
   int l2_hints;         // TMA L2 eviction priorities: bit 0 = A loads evict_last (the panel the resident CTAs share across waves),
                         // bit 1 = B loads evict_first (streamed once per band), bit 2 = output stores evict_first
@@ -140,22 +143,24 @@ __device__ __forceinline__ void acc_ld32(const float* p, uint32_t* v) {
 constexpr int kStageTileBytes = 128 * 128;
 constexpr int kEpiGroups = 2;                                   // two groups of 4 epilogue warps split a tile's store blocks
 constexpr int kGemmThreads = 128 + kEpiGroups * 128;            // warpgroup 0: TMA producer ; warpgroups 1-2: wgmma + epilogue
-template <int BN, int SPECIAL = 0>        // SPECIAL 3: the GELU two-output epilogue (fuse == 3) is compiled into its own kernel
+template <int BN, Epi EPI>
 __device__ __forceinline__ void epilogue_drain_tile(const GemmEpilogue& ep, const CUtensorMap* tmap_out, const CUtensorMap* tmap_out2,
                                                     unsigned char* staging, int grp, const float* arow, int row_in_tile, int tile_row0,
                                                     int tile_col0) {
+  static_assert(BN == 256 || EPI == Epi::Plain || EPI == Epi::GeluPair, "the SwiGLU and RoPE epilogues need 256-wide tiles");
   const int N = ep.N;
   const int row = tile_row0 + row_in_tile;
   const bool row_ok = row < ep.M;
-  const int sb_cols = ep.out_f32 ? 32 : 64;                    // 128 bytes of output per row per store block
+  constexpr bool F32_OUT = EPI == Epi::Plain;                   // the fused epilogues write bf16 only
+  const int sb_cols = (F32_OUT && ep.out_f32) ? 32 : 64;       // 128 bytes of output per row per store block
   const bool issuer = (threadIdx.x == 128 + grp * 128);        // first thread of this epilogue group
   unsigned char* tile = staging + grp * kStageTileBytes;       // one staging tile per group
   unsigned char* st = tile + row_in_tile * 128;
   const int sw = row_in_tile & 7;
   // fp32 residual (o_proj / down-projection: x_out = x + y): this thread's 128 bytes of the NEXT store block are fetched
-  // while the current block is processed, so the HBM latency of the residual no longer sits in the block's serial chain
-  // (accumulator ld -> residual ld -> math -> st.shared -> TMA store)
-  const bool rpf = ep.out_f32 && ep.resid != nullptr && ep.resid_f32;
+  // as soon as the current block's math has consumed its own, so the HBM latency of the residual no longer sits in the
+  // block's serial chain (accumulator ld -> residual ld -> math -> st.shared -> TMA store)
+  const bool rpf = F32_OUT && ep.out_f32 && ep.resid != nullptr && ep.resid_f32;
   float4 rnext[8];
   auto fetch_resid = [&](int cc) {
     const int cg0 = tile_col0 + cc;
@@ -171,21 +176,19 @@ __device__ __forceinline__ void epilogue_drain_tile(const GemmEpilogue& ep, cons
     if (col0 >= N) break;                                       // uniform across the group's 4 warps
     if (issuer) bulk_wait_read<0>();                            // the previous store has finished reading the staging tile
     named_bar_sync(1 + grp, 128);
-    if (ep.out_f32) {
+    if (F32_OUT && ep.out_f32) {
       uint32_t v[32]; float f[32];
       acc_ld32(arow + c, v);
-      float4 rcur[8];
-      if (rpf) {
-#pragma unroll
-        for (int g = 0; g < 8; ++g) rcur[g] = rnext[g];
+      if (rpf) {                                                // one block of residual in registers at a time
+        epilogue_math<true>(ep, v, f, row, col0, row_ok, rnext);
         fetch_resid(c + kEpiGroups * sb_cols);
+      } else {
+        epilogue_math<false>(ep, v, f, row, col0, row_ok);
       }
-      if (rpf) epilogue_math<true>(ep, v, f, row, col0, row_ok, rcur);
-      else     epilogue_math<false>(ep, v, f, row, col0, row_ok);
 #pragma unroll
       for (int g = 0; g < 8; ++g)
         *reinterpret_cast<float4*>(st + ((g ^ sw) << 4)) = make_float4(f[g * 4], f[g * 4 + 1], f[g * 4 + 2], f[g * 4 + 3]);
-    } else if (BN == 256 && ep.fuse == 2 && col0 < ep.rope_cols) {   // gemm_bf16_rope launches 256-wide tiles only
+    } else if (EPI == Epi::RoPE && col0 < ep.rope_cols) {
       // RoPE in the QKV epilogue: this 64-column block is one rotate_half HALF of a head (x1 = columns 0..63, x2 = 64..127 of the
       // head; tiles are 256 columns = two whole heads); its partner half sits 64 columns away in the same accumulator.
       //   x1' = x1 cos - x2 sin ,  x2' = x2 cos + x1 sin        (cos / sin of the row's position, element j = column % 64)
@@ -221,58 +224,7 @@ __device__ __forceinline__ void epilogue_drain_tile(const GemmEpilogue& ep, cons
         for (int g = 0; g < 4; ++g)
           *reinterpret_cast<bf16x8*>(st + (((h * 4 + g) ^ sw) << 4)) = pack8(f + g * 8);
       }
-    } else if (SPECIAL == 4) {
-      // SwiGLU backward (see GemmEpilogue::fuse): this block = 64 features f0.. of d(act); their gate columns sit at
-      // 256*(f0/128) + f0%128 of the interleaved buffer, the up columns 128 further. Same arithmetic and roundings as
-      // swiglu_bwd_kernel on a bf16 d(act), so the fused launch is bit-identical to the dgrad GEMM + that kernel.
-      const int gcol = ((col0 >> 7) << 8) + (col0 & 127);
-      const __nv_bfloat16* gp = reinterpret_cast<const __nv_bfloat16*>(ep.resid) + (size_t)row * ep.ldr + gcol;
-      bf16x8 pu[8];                                            // d gate goes straight to the staging tile, d up waits in registers
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        bf16x8 gq[4], uq[4];
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          gq[g] = row_ok ? *reinterpret_cast<const bf16x8*>(gp + h * 32 + g * 8) : bf16x8{};
-          uq[g] = row_ok ? *reinterpret_cast<const bf16x8*>(gp + 128 + h * 32 + g * 8) : bf16x8{};
-        }
-        uint32_t v[32];
-        acc_ld32(arow + (c + h * 32), v);
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          float gg[8], uu[8], dg[8], du[8];
-          unpack8(gq[g], gg);
-          unpack8(uq[g], uu);
-#pragma unroll
-          for (int k = 0; k < 8; ++k) {
-            const float d = __bfloat162float(__float2bfloat16_rn(__uint_as_float(v[g * 8 + k]) * ep.alpha));
-            const float sg = 1.f / (1.f + __expf(-gg[k]));
-            const float silu = gg[k] * sg;
-            dg[k] = d * uu[k] * sg * (1.f + gg[k] * (1.f - sg));
-            du[k] = d * silu;
-          }
-          *reinterpret_cast<bf16x8*>(st + (((h * 4 + g) ^ sw) << 4)) = pack8(dg);
-          pu[h * 4 + g] = pack8(du);
-        }
-      }
-      fence_proxy_async();
-      named_bar_sync(1 + grp, 128);
-      if (issuer) {
-        tma_store_2d(tmap_out, tile, gcol, tile_row0);
-        bulk_commit();
-        bulk_wait_read<0>();
-      }
-      named_bar_sync(1 + grp, 128);
-#pragma unroll
-      for (int g = 0; g < 8; ++g) *reinterpret_cast<bf16x8*>(st + ((g ^ sw) << 4)) = pu[g];
-      fence_proxy_async();
-      named_bar_sync(1 + grp, 128);
-      if (issuer) {
-        tma_store_2d(tmap_out, tile, gcol + 128, tile_row0);
-        bulk_commit();
-      }
-      continue;
-    } else if (SPECIAL == 3) {
+    } else if (EPI == Epi::GeluPair) {
       // GELU forward, both tensors: the 64-column block goes out twice through the same staging tile - first the bf16
       // pre-activation, then gelu() of those ROUNDED values (exactly what gelu_fwd_kernel would read back from HBM).
       bf16x8 pk[8];
@@ -338,35 +290,33 @@ __device__ __forceinline__ void epilogue_drain_tile(const GemmEpilogue& ep, cons
       bulk_commit();
     }
   }
-  if constexpr (BN == 256) {
-    if (ep.fuse == 1) {
-      // SwiGLU forward: act[:, 128 n_blk + 64 j + ...] = silu(gate) * up from the fp32 accumulators (gate columns 64j.., up columns
-      // 128 + 64j..): two more 128-byte-wide store blocks per tile, one per epilogue group. Replaces a separate pass that re-read
-      // the 203 MB gate|up buffer.
-      const int j = grp;
-      const int acol0 = (tile_col0 >> 1) + j * 64;              // column of the [M, N/2] activation matrix
-      if (issuer) bulk_wait_read<0>();
-      named_bar_sync(1 + grp, 128);
+  if constexpr (EPI == Epi::SwiGLU) {
+    // SwiGLU forward: act[:, 128 n_blk + 64 j + ...] = silu(gate) * up from the fp32 accumulators (gate columns 64j.., up columns
+    // 128 + 64j..): two more 128-byte-wide store blocks per tile, one per epilogue group. Replaces a separate pass that re-read
+    // the 203 MB gate|up buffer.
+    const int j = grp;
+    const int acol0 = (tile_col0 >> 1) + j * 64;                // column of the [M, N/2] activation matrix
+    if (issuer) bulk_wait_read<0>();
+    named_bar_sync(1 + grp, 128);
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        uint32_t vg[32], vu[32]; float f[32];
-        acc_ld32(arow + (j * 64 + h * 32), vg);
-        acc_ld32(arow + (128 + j * 64 + h * 32), vu);
+    for (int h = 0; h < 2; ++h) {
+      uint32_t vg[32], vu[32]; float f[32];
+      acc_ld32(arow + (j * 64 + h * 32), vg);
+      acc_ld32(arow + (128 + j * 64 + h * 32), vu);
 #pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const float g = __uint_as_float(vg[i]);
-          f[i] = g / (1.f + __expf(-g)) * __uint_as_float(vu[i]);
-        }
-#pragma unroll
-        for (int g4 = 0; g4 < 4; ++g4) *reinterpret_cast<bf16x8*>(st + (((h * 4 + g4) ^ sw) << 4)) = pack8(f + g4 * 8);
+      for (int i = 0; i < 32; ++i) {
+        const float g = __uint_as_float(vg[i]);
+        f[i] = g / (1.f + __expf(-g)) * __uint_as_float(vu[i]);
       }
-      fence_proxy_async();
-      named_bar_sync(1 + grp, 128);
-      if (issuer) {
-        if (ep.l2_hints & 4) tma_store_2d_hint(tmap_out2, tile, acol0, tile_row0, l2_policy_evict_first());
-        else                 tma_store_2d(tmap_out2, tile, acol0, tile_row0);
-        bulk_commit();
-      }
+#pragma unroll
+      for (int g4 = 0; g4 < 4; ++g4) *reinterpret_cast<bf16x8*>(st + (((h * 4 + g4) ^ sw) << 4)) = pack8(f + g4 * 8);
+    }
+    fence_proxy_async();
+    named_bar_sync(1 + grp, 128);
+    if (issuer) {
+      if (ep.l2_hints & 4) tma_store_2d_hint(tmap_out2, tile, acol0, tile_row0, l2_policy_evict_first());
+      else                 tma_store_2d(tmap_out2, tile, acol0, tile_row0);
+      bulk_commit();
     }
   }
 }
@@ -406,13 +356,13 @@ __device__ __forceinline__ void wgmma_tile(float* d, uint64_t da, uint64_t db, i
 // The producer starts the next tile's loads once both epilogue groups have left the parked accumulator.
 // CL = 2: a cluster of two CTAs computes a 256 x BN tile (128 rows each); each CTA loads half of the shared B tile and
 // multicasts it to both, so every B panel is read from L2 once per two CTAs (block_n 2128 / 2256).
-template <int BN, int LAYOUT, int SPECIAL, int CL>
+template <int BN, int LAYOUT, Epi EPI, int CL>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                     const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_out2, const GemmEpilogue ep) {
   using Cfg = GemmCfg<BN>;
   constexpr int BM = Cfg::BM, BK = Cfg::BK, STAGES = Cfg::STAGES;
-  static_assert(CL == 1 || (LAYOUT == 0 && SPECIAL == 0), "the cluster kernel takes the plain TN layout");
+  static_assert(CL == 1 || (LAYOUT == 0 && EPI == Epi::Plain), "the cluster kernel takes the plain TN layout");
   extern __shared__ unsigned char smem_raw[];
   // 128B swizzle atoms need 1024-byte aligned tile bases
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -435,7 +385,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
     prefetch_tmap(&tmap_a);
     prefetch_tmap(&tmap_b);
     prefetch_tmap(&tmap_out);
-    if (ep.fuse == 1 || ep.fuse == 3) prefetch_tmap(&tmap_out2);
+    if constexpr (EPI == Epi::SwiGLU || EPI == Epi::GeluPair) prefetch_tmap(&tmap_out2);
   }
   if (threadIdx.x == 32) {
     // consumer releases: one arrive per consumer warp, of every CTA whose producer writes into this stage
@@ -544,8 +494,8 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
       }
       named_bar_sync(3, 256);
       const int row_in_tile = q * 32 + lane;
-      epilogue_drain_tile<BN, SPECIAL>(ep, &tmap_out, &tmap_out2, staging, grp, acc_smem + (size_t)row_in_tile * Cfg::ACC_LD,
-                                       row_in_tile, (m_blk * CL + (int)rank) * BM, n_blk * BN);
+      epilogue_drain_tile<BN, EPI>(ep, &tmap_out, &tmap_out2, staging, grp, acc_smem + (size_t)row_in_tile * Cfg::ACC_LD,
+                                   row_in_tile, (m_blk * CL + (int)rank) * BM, n_blk * BN);
       // the next tile's TMA loads (async proxy) may overwrite what this warp has read
       fence_proxy_async();
       __syncwarp();
@@ -624,28 +574,37 @@ int get_tmap(const void* ptr, long long rows, long long cols, long long ld, int 
   return 0;
 }
 
-template <int BN, int LAYOUT = 0, int SPECIAL = 0>
+template <int BN, int LAYOUT, Epi EPI>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const GemmEpilogue& ep,
-                       int max_ctas, cudaStream_t stream, const CUtensorMap* to2 = nullptr) {
+                       int max_ctas, cudaStream_t stream, const CUtensorMap* to2) {
   using Cfg = GemmCfg<BN>;
   static bool attr_set = false;
   if (!attr_set) {
-    DALM_CUDA(cudaFuncSetAttribute(gemm_bf16_tn_kernel<BN, LAYOUT, SPECIAL, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    DALM_CUDA(cudaFuncSetAttribute(gemm_bf16_tn_kernel<BN, LAYOUT, EPI, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     attr_set = true;
   }
   const int num_tiles = ((ep.M + 127) / 128) * ((ep.N + BN - 1) / BN);
   int grid = num_tiles < num_sms() ? num_tiles : num_sms();
   if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
-  gemm_bf16_tn_kernel<BN, LAYOUT, SPECIAL, 1><<<grid, kGemmThreads, Cfg::SMEM_BYTES, stream>>>(ta, tb, to, to2 ? *to2 : to, ep);
+  gemm_bf16_tn_kernel<BN, LAYOUT, EPI, 1><<<grid, kGemmThreads, Cfg::SMEM_BYTES, stream>>>(ta, tb, to, to2 ? *to2 : to, ep);
   count_launch();
   return check_launch("gemm_bf16_tn_kernel");
+}
+
+// block_n (64 / 128 / 256) -> the single-CTA kernel of that tile width
+template <int LAYOUT, Epi EPI>
+static int launch_gemm_bn(int bn, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const GemmEpilogue& ep,
+                          int max_ctas, cudaStream_t stream, const CUtensorMap* to2 = nullptr) {
+  if (bn == 256) return launch_gemm<256, LAYOUT, EPI>(ta, tb, to, ep, max_ctas, stream, to2);
+  if (bn == 128) return launch_gemm<128, LAYOUT, EPI>(ta, tb, to, ep, max_ctas, stream, to2);
+  return launch_gemm<64, LAYOUT, EPI>(ta, tb, to, ep, max_ctas, stream, to2);
 }
 
 template <int BN>
 static int launch_gemm_cluster(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const GemmEpilogue& ep,
                                int max_ctas, cudaStream_t stream) {
   using Cfg = GemmCfg<BN>;
-  auto kern = gemm_bf16_tn_kernel<BN, 0, 0, 2>;
+  auto kern = gemm_bf16_tn_kernel<BN, 0, Epi::Plain, 2>;
   static bool attr_set = false;
   if (!attr_set) {
     DALM_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -671,12 +630,6 @@ static int launch_gemm_cluster(const CUtensorMap& ta, const CUtensorMap& tb, con
 }  // namespace dalm
 
 using namespace dalm;
-
-extern "C" int dalm_b200_gemm_bf16(int layout, const void* A, long long lda, const void* B, long long ldb, void* out,
-                                   long long ldo, int out_f32, int M, int N, int K, float alpha, const float* bias,
-                                   int act, const void* resid, long long ldr, int resid_f32, int block_n,
-                                   int max_ctas, float drop_p, unsigned long long drop_seed,
-                                   unsigned long long drop_stream_id, const void* drop_offset, void* stream);
 
 // tile rasterisation override: -1 = m-fastest order everywhere, 0 = automatic (default: pick_group_m below), -2 = bands
 // (bands for every multi-wave problem), > 0 = that many m-tiles per band. Initial value: env DALM_B200_GEMM_RASTER.
@@ -742,19 +695,27 @@ static int pick_group_m(int M, int N, int K, int tile_n, bool stream_out) {
   return group_m;
 }
 
-// D[M,N] = act(alpha * A[M,K] B[N,K]^T + bias) + resid
-//   A: bf16 [M,K] row stride lda;  B: bf16 [N,K] row stride ldb;  out: bf16|fp32 [M,N] row stride ldo
-//   block_n: 0 = auto, or one of 64/128/256.   max_ctas: 0 = all SMs (used by tests to force multi-tile-per-CTA paths)
-extern "C" int dalm_b200_gemm_bf16_tn(const void* A, long long lda, const void* B, long long ldb, void* out,
-                                      long long ldo, int out_f32, int M, int N, int K, float alpha, const float* bias,
-                                      int act, const void* resid, long long ldr, int resid_f32, int block_n,
-                                      int max_ctas, float drop_p, unsigned long long drop_seed,
-                                      unsigned long long drop_stream_id, const void* drop_offset, void* stream) {
-  return dalm_b200_gemm_bf16(0, A, lda, B, ldb, out, ldo, out_f32, M, N, K, alpha, bias, act, resid, ldr, resid_f32, block_n,
-                             max_ctas, drop_p, drop_seed, drop_stream_id, drop_offset, stream);
+// The epilogue of one launch over an M x N x K problem in tiles tile_n wide, writing `out`, with the plain epilogue's
+// defaults (alpha 1, no bias, activation, dropout or residual): callers set what their entry point adds. The raster and
+// the L2 hints are chosen here for every entry point; an fp32 output or a residual read counts as streamed output.
+static GemmEpilogue gemm_epilogue(int M, int N, int K, int tile_n, void* out, long long ldo, int out_f32 = 0,
+                                  const void* resid = nullptr, long long ldr = 0, int resid_f32 = 0) {
+  GemmEpilogue ep{};
+  ep.out = out; ep.ldo = ldo; ep.out_f32 = out_f32;
+  ep.resid = resid; ep.ldr = ldr; ep.resid_f32 = resid_f32;
+  ep.alpha = 1.f;
+  ep.M = M; ep.N = N; ep.K = K;
+  ep.drop = make_drop(0.f, 0, 0, nullptr);
+  const bool stream_out = out_f32 != 0 || resid != nullptr;
+  ep.group_m = pick_group_m(M, N, K, tile_n, stream_out);
+  ep.l2_hints = pick_l2_hints(M, N, K, tile_n, ep.group_m, stream_out);
+  return ep;
 }
 
+// D[M,N] = act(alpha * A[M,K] B[N,K]^T + bias) + resid, out: bf16|fp32 [M,N] row stride ldo
 // layout 0: A[M,K] B[N,K] (TN)   1: A[M,K] B[K,N] (NN, dgrad from W[out,in])   2: A[K,M] B[K,N] (wgrad, contraction over rows)
+// block_n: 0 = auto, 64/128/256, or 2128/2256 (cluster of two CTAs).   max_ctas: 0 = all SMs (used by tests to force
+// multi-tile-per-CTA paths)
 extern "C" int dalm_b200_gemm_bf16(int layout, const void* A, long long lda, const void* B, long long ldb, void* out,
                                    long long ldo, int out_f32, int M, int N, int K, float alpha, const float* bias,
                                    int act, const void* resid, long long ldr, int resid_f32, int block_n,
@@ -789,26 +750,15 @@ extern "C" int dalm_b200_gemm_bf16(int layout, const void* A, long long lda, con
   else             { if (int e = get_tmap(B, N, K, ldb, pair ? tile_n / 2 : tile_n, &tb)) return e; }
   if (int e = get_tmap(out, M, N, ldo, 128, &to, out_f32)) return e;
   DALM_REQUIRE(drop_p >= 0.f && drop_p < 1.f, "gemm: dropout p must be in [0,1)");
-  const int group_m = pick_group_m(M, N, K, tile_n, out_f32 != 0 || resid != nullptr);
-  GemmEpilogue ep{out, ldo, out_f32, bias, resid, ldr, resid_f32, act, alpha, M, N, K,
-                  make_drop(drop_p, drop_seed, drop_stream_id, drop_offset), group_m, 0, nullptr, nullptr, 0, 0,
-                  pick_l2_hints(M, N, K, tile_n, group_m, out_f32 != 0 || resid != nullptr)};
+  GemmEpilogue ep = gemm_epilogue(M, N, K, tile_n, out, ldo, out_f32, resid, ldr, resid_f32);
+  ep.bias = bias; ep.act = act; ep.alpha = alpha;
+  ep.drop = make_drop(drop_p, drop_seed, drop_stream_id, drop_offset);
   cudaStream_t st = (cudaStream_t)stream;
   if (bn == 2256) return launch_gemm_cluster<256>(ta, tb, to, ep, max_ctas, st);
   if (bn == 2128) return launch_gemm_cluster<128>(ta, tb, to, ep, max_ctas, st);
-  if (layout == 1) {
-    if (bn == 256) return launch_gemm<256, 1>(ta, tb, to, ep, max_ctas, st);
-    if (bn == 128) return launch_gemm<128, 1>(ta, tb, to, ep, max_ctas, st);
-    return launch_gemm<64, 1>(ta, tb, to, ep, max_ctas, st);
-  }
-  if (layout == 2) {
-    if (bn == 256) return launch_gemm<256, 2>(ta, tb, to, ep, max_ctas, st);
-    if (bn == 128) return launch_gemm<128, 2>(ta, tb, to, ep, max_ctas, st);
-    return launch_gemm<64, 2>(ta, tb, to, ep, max_ctas, st);
-  }
-  if (bn == 256) return launch_gemm<256>(ta, tb, to, ep, max_ctas, st);
-  if (bn == 128) return launch_gemm<128>(ta, tb, to, ep, max_ctas, st);
-  return launch_gemm<64>(ta, tb, to, ep, max_ctas, st);
+  if (layout == 1) return launch_gemm_bn<1, Epi::Plain>(bn, ta, tb, to, ep, max_ctas, st);
+  if (layout == 2) return launch_gemm_bn<2, Epi::Plain>(bn, ta, tb, to, ep, max_ctas, st);
+  return launch_gemm_bn<0, Epi::Plain>(bn, ta, tb, to, ep, max_ctas, st);
 }
 
 // gate|up projection of LlamaMLP with SiLU(gate) * up fused into the epilogue (see include/dalm_b200.h)
@@ -822,26 +772,8 @@ extern "C" int dalm_b200_gemm_bf16_swiglu(const void* A, long long lda, const vo
   if (int e = get_tmap(B, N, K, ldb, 256, &tb)) return e;
   if (int e = get_tmap(gu, M, N, ldgu, 128, &to, 0)) return e;
   if (int e = get_tmap(act, M, N / 2, ldact, 128, &to2, 0)) return e;
-  const int group_m = pick_group_m(M, N, K, 256, false);
-  GemmEpilogue ep{gu, ldgu, 0, nullptr, nullptr, 0, 0, 0, 1.f, M, N, K, make_drop(0.f, 0, 0, nullptr), group_m, 1, nullptr, nullptr, 0, 0,
-                  pick_l2_hints(M, N, K, 256, group_m, false)};
-  return launch_gemm<256>(ta, tb, to, ep, 0, (cudaStream_t)stream, &to2);
-}
-
-// down-projection dgrad of LlamaMLP with the SwiGLU backward in its epilogue: d(act) = dY WdT^T never reaches HBM; the interleaved
-// gate|up buffer of the forward (gemm_bf16_swiglu) is overwritten in place with [d gate | d up] (what swiglu_bwd produced).
-extern "C" int dalm_b200_gemm_bf16_swiglu_bwd(const void* dY, long long lddy, const void* WdT, long long ldw, void* gu, long long ldgu,
-                                              int M, int F, int K, void* stream) {
-  DALM_REQUIRE(M > 0 && K > 0 && F >= 256 && (F % 128) == 0, "gemm_swiglu_bwd: F=%d must be >= 256 and a multiple of 128 (interleave block)", F);
-  DALM_REQUIRE((K % 8) == 0 && lddy >= K && ldw >= K && ldgu >= 2LL * F && (ldgu % 8) == 0 && ((uintptr_t)gu & 15) == 0,
-               "gemm_swiglu_bwd: bad K / leading dimensions / alignment");
-  CUtensorMap ta, tb, to;
-  if (int e = get_tmap(dY, M, K, lddy, 128, &ta)) return e;
-  if (int e = get_tmap(WdT, F, K, ldw, 256, &tb)) return e;
-  if (int e = get_tmap(gu, M, 2LL * F, ldgu, 128, &to, 0)) return e;
-  const int group_m = pick_group_m(M, F, K, 256, false);
-  GemmEpilogue ep{gu, ldgu, 0, nullptr, gu, ldgu, 0, 0, 1.f, M, F, K, make_drop(0.f, 0, 0, nullptr), group_m, 4, nullptr, nullptr, 0, 0, 0};   // in-place output: no hints
-  return launch_gemm<256, 0, 4>(ta, tb, to, ep, 0, (cudaStream_t)stream);
+  const GemmEpilogue ep = gemm_epilogue(M, N, K, 256, gu, ldgu);
+  return launch_gemm<256, 0, Epi::SwiGLU>(ta, tb, to, ep, 0, (cudaStream_t)stream, &to2);
 }
 
 // intermediate projection of a GELU MLP (BertIntermediate, Falcon dense_h_to_4h) with the activation fused into the epilogue and
@@ -857,13 +789,9 @@ extern "C" int dalm_b200_gemm_bf16_gelu(const void* A, long long lda, const void
   if (int e = get_tmap(B, N, K, ldb, bn, &tb)) return e;
   if (int e = get_tmap(pre, M, N, ldpre, 128, &to, 0)) return e;
   if (int e = get_tmap(act, M, N, ldact, 128, &to2, 0)) return e;
-  const int group_m = pick_group_m(M, N, K, bn, false);
-  GemmEpilogue ep{pre, ldpre, 0, bias, nullptr, 0, 0, 0, 1.f, M, N, K, make_drop(0.f, 0, 0, nullptr), group_m, 3, nullptr, nullptr, 0, 0,
-                  pick_l2_hints(M, N, K, bn, group_m, false)};
-  cudaStream_t st = (cudaStream_t)stream;
-  if (bn == 256) return launch_gemm<256, 0, 3>(ta, tb, to, ep, 0, st, &to2);
-  if (bn == 128) return launch_gemm<128, 0, 3>(ta, tb, to, ep, 0, st, &to2);
-  return launch_gemm<64, 0, 3>(ta, tb, to, ep, 0, st, &to2);
+  GemmEpilogue ep = gemm_epilogue(M, N, K, bn, pre, ldpre);
+  ep.bias = bias;
+  return launch_gemm_bn<0, Epi::GeluPair>(bn, ta, tb, to, ep, 0, (cudaStream_t)stream, &to2);
 }
 
 // fused q|k|v projection + rotary embedding: out[M,N] = A[M,K] B[N,K]^T + bias with HF's rotate_half RoPE (head_dim 128) applied to
@@ -880,10 +808,10 @@ extern "C" int dalm_b200_gemm_bf16_rope(const void* A, long long lda, const void
   if (int e = get_tmap(A, M, K, lda, 128, &ta)) return e;
   if (int e = get_tmap(B, N, K, ldb, 256, &tb)) return e;
   if (int e = get_tmap(out, M, N, ldo, 128, &to, 0)) return e;
-  const int group_m = pick_group_m(M, N, K, 256, false);
-  GemmEpilogue ep{out, ldo, 0, bias, nullptr, 0, 0, 0, 1.f, M, N, K, make_drop(0.f, 0, 0, nullptr), group_m, 2, cos_t, sin_t, L, rope_cols,
-                  pick_l2_hints(M, N, K, 256, group_m, false)};
-  return launch_gemm<256>(ta, tb, to, ep, 0, (cudaStream_t)stream);
+  GemmEpilogue ep = gemm_epilogue(M, N, K, 256, out, ldo);
+  ep.bias = bias;
+  ep.rope_cos = cos_t; ep.rope_sin = sin_t; ep.rope_L = L; ep.rope_cols = rope_cols;
+  return launch_gemm<256, 0, Epi::RoPE>(ta, tb, to, ep, 0, (cudaStream_t)stream, nullptr);
 }
 
 // drop cached tensor maps (call when operand buffers are freed / re-allocated at the same address with other shapes)

@@ -41,28 +41,6 @@ MAX_CACHE_TOKENS = 8192                                     # dalm_b200_attentio
 GRAPH_MIN_STEPS = 192                                       # remaining tokens from which capturing the step pays for itself
 
 
-_LEAN_POOL = None
-
-
-def _capture_lean(graph: "torch.cuda.CUDAGraph", step) -> None:
-    """CANDIDATE (DALM_B200_DECODE_GRAPH=2, not a default): capture without `torch.cuda.graph`'s entry work (gc.collect +
-    empty_cache, measured at 50-300 ms per call) and into ONE memory pool shared by every capture of the process, so that
-    later `generate` calls find their decode-step buffers already cached. Written after the round's GPU minutes were spent:
-    its check (tests/test_generate_gpu.py, DALM_B200_EXPERIMENTAL=1) has not run yet."""
-    global _LEAN_POOL
-    if _LEAN_POOL is None:
-        _LEAN_POOL = torch.cuda.graph_pool_handle()
-    torch.cuda.synchronize()
-    side = torch.cuda.Stream()
-    with torch.cuda.stream(side):
-        graph.capture_begin(pool=_LEAN_POOL)
-        try:
-            step()
-        finally:
-            graph.capture_end()
-    torch.cuda.current_stream().wait_stream(side)
-
-
 # ----------------------------------------------------------------------------------------------------------------
 # generation config: what HF `generate` would do for the same checkpoint and call
 # ----------------------------------------------------------------------------------------------------------------
@@ -239,19 +217,15 @@ def _decode(dec, token_step, input_ids, attention_mask, max_length, max_new_toke
         # allocated afresh) and a replayed step saves only launch overhead while the step is GPU-bound (decode attention), so
         # by default only long generations are captured. DALM_B200_DECODE_GRAPH=1 / 0 forces it.
         mode = os.environ.get("DALM_B200_DECODE_GRAPH", "auto")
-        lean_capture = mode == "2"                                                # candidate, see _capture_lean
-        use_graph = dev.type == "cuda" and ((mode in ("1", "2") and total - col >= 4) or (mode == "auto" and total - col >= GRAPH_MIN_STEPS))
+        use_graph = dev.type == "cuda" and ((mode == "1" and total - col >= 4) or (mode == "auto" and total - col >= GRAPH_MIN_STEPS))
         while col < total:
             if eos_list and (col - L0) % 8 == 0 and int(alive[col - 1].item()) == 0:    # one host read every 8 tokens
                 break
             if use_graph and graph is None and col > L0 + 1:                     # one eager step first (lazy attributes, tensor maps)
                 try:
                     graph = torch.cuda.CUDAGraph()
-                    if lean_capture:
-                        _capture_lean(graph, step)
-                    else:
-                        with torch.cuda.graph(graph):
-                            step()
+                    with torch.cuda.graph(graph):
+                        step()
                 except Exception as e:                                            # capture is an optimisation, never a requirement
                     logger.warning(f"CUDA-graph capture of the decode step failed ({type(e).__name__}: {e}); launching eagerly")
                     graph, use_graph = None, False

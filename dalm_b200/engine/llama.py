@@ -15,7 +15,6 @@ Qwen2 is this architecture plus q/k/v biases (HF Qwen2ForCausalLM); configs are 
 """
 from __future__ import annotations
 
-import os
 from typing import Dict, List, Optional
 
 import torch
@@ -89,8 +88,8 @@ class LlamaDecoder(torch.nn.Module):
         self.layers: List[Dict[str, torch.Tensor]] = []
         # frozen-base modes keep the fused gate|up weight in the interleaved layout of the SwiGLU-epilogue GEMM (F % 128 == 0);
         # a fully fine-tuned model keeps HF's [gate; up] order inside its parameter bank (un-fused activation kernel)
-        self.fuse_rope = self.hd == 128 and os.environ.get("DALM_B200_FUSE_ROPE", "1") != "0"
-        self.gu_il = 128 if (not full and F % 128 == 0 and os.environ.get("DALM_B200_FUSE_SWIGLU", "1") != "0") else 0
+        self.fuse_rope = self.hd == 128
+        self.gu_il = 128 if (not full and F % 128 == 0) else 0
         if full:
             self._init_full(sd)
         else:
@@ -430,12 +429,10 @@ class LlamaDecoder(torch.nn.Module):
                                       bias=W["bqkv"])                                        # the epilogue
             else:
                 a.qkv = ops.gemm(a.h1_aug, W["Wqkv_aug"], bias=W["bqkv"])        # [M, Nq+2Nkv]
-            if pos is None and not (self.fuse_rope and rope_cols % 256 == 0):
-                ops.rope_(a.qkv, 0, self.nh + self.nkv, self.hd, cos_t, sin_t, L)    # q heads then k heads are adjacent
-            elif pos is None:
-                pass
-            else:
-                ops.rope_pos_(a.qkv, 0, self.nh + self.nkv, self.hd, cos_t, sin_t, pos)
+                if pos is None:
+                    ops.rope_(a.qkv, 0, self.nh + self.nkv, self.hd, cos_t, sin_t, L)    # q heads then k heads are adjacent
+                else:
+                    ops.rope_pos_(a.qkv, 0, self.nh + self.nkv, self.hd, cos_t, sin_t, pos)
             if kv_sink is not None:
                 kv_sink(li, a.qkv)
             a.att, a.lse = ops.attention_auto_fwd(a.qkv[:, :self.Nq], a.qkv[:, self.Nq:self.Nq + self.Nkv],
@@ -535,11 +532,8 @@ class LlamaDecoder(torch.nn.Module):
             W, a = self.layers[l], ctx.layers[l]
             if bank is not None:
                 ops.wgrad_(dx16, a.act, G(l, "Wd"), acc)
-            if bank is None and self.nf4 is None and self.gu_il == 128 and F >= 256 and ops.FUSE_SWIGLU_BWD:
-                ops.gemm_swiglu_bwd_(dx16, W["WdT"], a.gu)                         # d(act) stays on chip; gu <- [dgate | dup] in the epilogue
-            else:
-                dact = self._dgrad(dx16, W, "Wd")                                  # [M,F]
-                ops.swiglu_bwd_(a.gu, dact, F, interleave=self.gu_il)              # gu <- [dgate | dup] (same layout as gu)
+            dact = self._dgrad(dx16, W, "Wd")                                      # [M,F]
+            ops.swiglu_bwd_(a.gu, dact, F, interleave=self.gu_il)                  # gu <- [dgate | dup] (same layout as gu)
             if bank is not None:
                 ops.wgrad_(a.gu, a.h2, G(l, "Wgu"), acc)
             dh2 = self._dgrad(a.gu, W, "Wgu")                                      # [M,H]

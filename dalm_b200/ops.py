@@ -458,34 +458,9 @@ def gemm_swiglu(a: torch.Tensor, w_il: torch.Tensor, gu: Optional[torch.Tensor] 
 
 # GELU in the GEMM epilogues pays only when the tile's mainloop is long enough to hide the erf / exp work of the 256 epilogue
 # threads, so the fusion is taken from K >= 2048 (Falcon's 4544-wide MLP) and BERT (K = 1024: 16 k-blocks per tile) keeps the
-# separate kernels. The threshold was chosen on the previous (Blackwell) kernels and has not been re-measured on H100. DALM_B200_FUSE_GELU_MIN_K overrides (0 = always, huge = never).
-FUSE_GELU_MIN_K = int(os.environ.get("DALM_B200_FUSE_GELU_MIN_K", "2048"))
-
-
+# separate kernels. The threshold was chosen on the previous (Blackwell) kernels and has not been re-measured on H100.
 def fuse_gelu(K: int) -> bool:
-    return K >= FUSE_GELU_MIN_K
-
-
-# the epilogue's per-thread row loads of gate / up (32 lines per warp instruction) cost more than the stand-alone swiglu_bwd pass
-# on the previous (Blackwell) kernels; not re-measured on H100. Opt-in only.
-FUSE_SWIGLU_BWD = os.environ.get("DALM_B200_FUSE_SWIGLU_BWD", "0") == "1"
-
-
-def gemm_swiglu_bwd_(dy: torch.Tensor, wdT: torch.Tensor, gu: torch.Tensor) -> torch.Tensor:
-    """LlamaMLP backward through down_proj and SiLU(gate) * up in one launch: dy [M,H] (gradient of the MLP output), wdT [F,H]
-    (down_proj weight transposed), gu [M,2F] = gate|up interleaved in 128-feature blocks -> overwritten with [d gate | d up]."""
-    _chk(dy, bf16, "gemm_swiglu_bwd dy"); _chk(wdT, bf16, "gemm_swiglu_bwd w"); _chk(gu, bf16, "gemm_swiglu_bwd gu")
-    M, K = dy.shape
-    F = wdT.shape[0]
-    if gu.shape != (M, 2 * F):
-        raise _lib.DalmB200Error(f"gemm_swiglu_bwd: gu {tuple(gu.shape)} is not [{M}, {2 * F}]")
-    timer = GEMM_TIMER
-    if timer is not None:
-        timer.begin(2.0 * M * F * K, (M, F, K, 0, "bfloat16", "swiglu_bwd", "-"))
-    _lib.call("dalm_b200_gemm_bf16_swiglu_bwd", _p(dy), _ld(dy), _p(wdT), _ld(wdT), _p(gu), _ld(gu), M, F, K, _stream())
-    if timer is not None:
-        timer.end()
-    return gu
+    return K >= 2048
 
 
 def gemm_gelu(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, pre: Optional[torch.Tensor] = None,

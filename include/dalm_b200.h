@@ -71,13 +71,9 @@ int dalm_b200_lora_dx(void* dh, long long lddh, const void* G, long long ldg, co
 
 /* ---- dense contractions (wgmma / TMA) ----
  * out[M,N] = act(alpha * A[M,K] B[N,K]^T + bias) + resid. Replaces every nn.Linear forward / dgrad reached through
- * dalm/models/rag_e2e_base_model.py:93,105 and dalm/models/retriever_only_base_model.py:58 (HF modeling code -> cuBLAS). */
-int dalm_b200_gemm_bf16_tn(const void* A, long long lda, const void* B, long long ldb, void* out, long long ldo,
-                           int out_f32, int M, int N, int K, float alpha, const float* bias, int act, const void* resid,
-                           long long ldr, int resid_f32, int block_n, int max_ctas, float drop_p, unsigned long long drop_seed,
-    unsigned long long drop_stream_id, const void* drop_offset, void* stream);
-/* the same kernel reading either operand MN-major straight from its row-major buffer (nothing is transposed in HBM):
- *   layout 0: A[M,K], B[N,K]  (== dalm_b200_gemm_bf16_tn)
+ * dalm/models/rag_e2e_base_model.py:93,105 and dalm/models/retriever_only_base_model.py:58 (HF modeling code -> cuBLAS).
+ * Either operand is read K-major or MN-major straight from its row-major buffer (nothing is transposed in HBM):
+ *   layout 0: A[M,K], B[N,K]  "TN", both K-contiguous: forward y = x W^T, and dgrad against resident W^T copies
  *   layout 1: A[M,K], B[K,N]  dgrad dx = dy W against W[out,in] itself — full fine-tuning (reference default use_peft=None,
  *                             dalm/training/rag_e2e/train_rage2e.py:229-260,336) where weights change every step
  *   layout 2: A[K,M], B[K,N]  wgrad dW[out,in] = dy^T x, contraction over token rows (autograd of nn.Linear.weight) */
@@ -97,11 +93,6 @@ int dalm_b200_gemm_bf16_swiglu(const void* A, long long lda, const void* B, long
  * on every column; NULL leaves the results bit-identical to a bias-free projection. */
 int dalm_b200_gemm_bf16_rope(const void* A, long long lda, const void* B, long long ldb, void* out, long long ldo, int M, int N,
                              int K, const float* bias, const float* cos_t, const float* sin_t, int L, int rope_cols, void* stream);
-/* gemm_bf16_swiglu_bwd: LlamaMLP backward through down_proj and act_fn(gate) * up in one launch: d(act)[M,F] = dY[M,K] WdT[F,K]^T
- * never reaches HBM; gu [M,2F] (gate|up interleaved in 128-feature blocks, as gemm_bf16_swiglu left it) is overwritten in place with
- * [d gate | d up]. Bit-identical to gemm_bf16 followed by swiglu_bwd (interleave 128). */
-int dalm_b200_gemm_bf16_swiglu_bwd(const void* dY, long long lddy, const void* WdT, long long ldw, void* gu, long long ldgu, int M,
-                                   int F, int K, void* stream);
 /* gemm_bf16_gelu: pre[M,N] = A B^T + bias (bf16) AND act[M,N] = gelu_erf(pre) (bf16) from one launch: BertIntermediate
  * (dense + GELU, HF modeling_bert) / Falcon's dense_h_to_4h + act; the backward multiplies by gelu'(pre) inside the next dgrad
  * GEMM (gemm_bf16 with act = 2 and resid = pre), so neither direction runs a separate activation kernel. */

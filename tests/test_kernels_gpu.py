@@ -483,24 +483,3 @@ def test_gemm_l2_hints_and_raster_modes_do_not_change_results(cuda_dev):
                     assert torch.equal(x, y)
     finally:
         lib.dalm_b200_gemm_set_raster(0); lib.dalm_b200_gemm_set_l2_hints(-1)
-
-
-@pytest.mark.parametrize("M,F,K", [(300, 256, 192), (4608, 1408, 512), (1000, 11008, 264), (130, 384, 72)])
-def test_gemm_with_fused_swiglu_backward_epilogue(cuda_dev, M, F, K):
-    """down-projection dgrad + SwiGLU backward in one launch (d(act) never leaves the SM, gate|up overwritten in place with
-    [d gate | d up]) == dgrad GEMM + swiglu_bwd kernel, bit for bit; and against torch autograd of silu(gate) * up"""
-    from dalm_b200 import ops
-    g = torch.Generator(device="cpu").manual_seed(M + F + K + 1)
-    dy = torch.randn(M, K + 8, generator=g).to(cuda_dev, torch.bfloat16)[:, :K]        # strided view
-    wdT = (torch.randn(F, K, generator=g) * 0.2).to(cuda_dev, torch.bfloat16)           # down_proj weight [K, F] transposed
-    gate = torch.randn(M, F, generator=g).to(cuda_dev, torch.bfloat16)
-    up = torch.randn(M, F, generator=g).to(cuda_dev, torch.bfloat16)
-    gu = torch.stack([gate.view(M, F // 128, 128), up.view(M, F // 128, 128)], 2).reshape(M, 2 * F).contiguous()
-    two = ops.swiglu_bwd_(gu.clone(), ops.gemm(dy, wdT), F, interleave=128)
-    one = ops.gemm_swiglu_bwd_(dy, wdT, gu.clone())
-    assert torch.equal(one, two)
-    gf, uf = gate.float().requires_grad_(True), up.float().requires_grad_(True)
-    (torch.nn.functional.silu(gf) * uf).backward(dy.float() @ wdT.float().t())
-    blk = one.float().view(M, F // 128, 2, 128)
-    assert ((blk[:, :, 0].reshape(M, F) - gf.grad).norm() / gf.grad.norm()).item() < 8e-3
-    assert ((blk[:, :, 1].reshape(M, F) - uf.grad).norm() / uf.grad.norm()).item() < 8e-3

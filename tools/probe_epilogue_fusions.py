@@ -1,5 +1,5 @@
 """Fused-epilogue GEMMs against the launch pairs they replace (CUDA events, rotating operand sets): GELU forward / backward at the
-BERT (K = 1024) and Falcon (K = 4544) MLP shapes, SwiGLU backward at the Llama-2-7B shape. One JSON line per case.
+BERT (K = 1024) and Falcon (K = 4544) MLP shapes. One JSON line per case.
     python tools/probe_epilogue_fusions.py"""
 import json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -46,24 +46,7 @@ def gelu_case(name, M, H, F, nbuf=3):
                       "fused_us": round(t_one, 1)}), flush=True)
 
 
-def swiglu_bwd_case(M=4608, H=4096, F=11008, nbuf=3):
-    dys = [rnd(M, H) for _ in range(nbuf)]
-    wdT = rnd(F, H)
-    gu = rnd(M, 2 * F, s=1.0)
-    dact = torch.empty(M, F, device=dev, dtype=bf16)
-    i = [0]
-    def nxt():
-        i[0] += 1
-        return dys[i[0] % nbuf]
-    t_two = timeit(lambda: ops.swiglu_bwd_(gu, ops.gemm(nxt(), wdT, out=dact), F, interleave=128))
-    t_one = timeit(lambda: ops.gemm_swiglu_bwd_(nxt(), wdT, gu))
-    t_gemm = timeit(lambda: ops.gemm(nxt(), wdT, out=dact))
-    print(json.dumps({"case": "llama down-proj dgrad + swiglu_bwd", "M": M, "N": F, "K": H, "gemm_us": round(t_gemm, 1),
-                      "gemm+swiglu_bwd_us": round(t_two, 1), "fused_us": round(t_one, 1)}), flush=True)
-
-
 if __name__ == "__main__":
-    swiglu_bwd_case()
     gelu_case("bge-large cfg-2 (26700 rows)", 26700, 1024, 4096)
     gelu_case("bge-large cfg-3 (3204 rows)", 3204, 1024, 4096)
     gelu_case("falcon-7b (4096 rows)", 4096, 4544, 18176)

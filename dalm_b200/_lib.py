@@ -54,7 +54,7 @@ SIGNATURES = {
     "dalm_b200_swiglu_fwd": [_P, _L, _P, _L, _I, _I, _I, _P],
     "dalm_b200_swiglu_bwd": [_P, _L, _P, _L, _I, _I, _I, _P],
     "dalm_b200_gemm_bf16_swiglu": [_P, _L, _P, _L, _P, _L, _P, _L, _I, _I, _I, _P],
-    "dalm_b200_gemm_bf16_rope": [_P, _L, _P, _L, _P, _L, _I, _I, _I, _P, _P, _P, _I, _I, _P],
+    "dalm_b200_gemm_bf16_rope": [_P, _L, _P, _L, _P, _L, _I, _I, _I, _P, _P, _P, _I, _I, _P, _P, _I, _F, _P, _L, _P, _L, _P],
     "dalm_b200_gemm_bf16_gelu": [_P, _L, _P, _L, _P, _L, _P, _L, _I, _I, _I, _P, _P],
     "dalm_b200_gelu_fwd": [_P, _L, _P, _L, _I, _I, _P],
     "dalm_b200_gelu_bwd": [_P, _L, _P, _L, _I, _I, _P],
@@ -77,6 +77,8 @@ SIGNATURES = {
     "dalm_b200_nf4_dequant_bf16": [_P, _P, _L, _I, _P, _L, _P, _L, _I, _P],
     "dalm_b200_decode_gemm": [_P, _L, _P, _L, _P, _L, _I, _P, _P, _L, _I, _I, _I, _I, _I, _P],
     "dalm_b200_rope_pos": [_P, _L, _I, _I, _I, _P, _P, _P, _I, _I, _P],
+    "dalm_b200_qk_norm_rope": [_P, _L, _I, _I, _P, _P, _F, _P, _P, _I, _I, _P, _I, _P, _L, _P, _L, _P],
+    "dalm_b200_qk_norm_rope_bwd": [_P, _L, _I, _I, _P, _P, _P, _P, _I, _P, _L, _P, _L, _I, _P, _P, _P],
     "dalm_b200_attention_decode": [_P, _L, _I, _I, _I, _P, _P, _L, _L, _P, _L, _P, _L, _I, _I, _I, _I, _I, _P, _I, _F, _P],
     "dalm_b200_greedy_step": [_P, _L, _I, _I, _P, _I, _L, _P, _P, _L, _P, _L, _I, _P, _I, _P, _P, _P, _P],
     "dalm_b200_sample_step": [_P, _L, _I, _I, _P, _I, _L, _P, _P, _L, _P, _L, _I, _P, _I, _P, _P, _P, _F, _I, _F, _U, _P, _P, _P],

@@ -10,7 +10,7 @@ import sys
 from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-SOURCES = ["api.cu", "loss.cu", "gemm_wgmma.cu", "attention.cu", "rowwise.cu", "lora.cu", "dense_grad.cu", "topk.cu", "nf4.cu", "decode.cu"]
+SOURCES = ["api.cu", "loss.cu", "gemm_wgmma.cu", "attention.cu", "rowwise.cu", "lora.cu", "dense_grad.cu", "topk.cu", "nf4.cu", "decode.cu", "qk_norm.cu"]
 HEADERS = ["common.cuh", "ptx.cuh"]
 LIB = os.path.join(HERE, "libdalm_b200.so")
 NVCC_FLAGS = [

@@ -25,6 +25,8 @@ enum class Epi {
   RoPE,      // rotary position embedding (head_dim 128, HF rotate_half) on output columns < rope_cols    (gemm_bf16_rope)
   GeluPair,  // `out` = pre-activation (bf16, what the backward needs), tmap_out2 = gelu(pre) (bf16, the next GEMM's
              // operand): one launch instead of GEMM + a 2-pass kernel                                     (gemm_bf16_gelu)
+  NormRoPE,  // RoPE after a per-head RMSNorm (Qwen3 q_norm / k_norm); tmap_out2 = the pre-norm q|k columns (bf16), and
+             // the per-head rstd to ep.norm_rstd (fp32): what the backward needs                        (gemm_bf16_rope)
 };
 
 struct GemmEpilogue {
@@ -43,6 +45,11 @@ struct GemmEpilogue {
   int group_m;          // tile rasterisation: bands of group_m m-tiles, n-tiles walked serpentine inside a band (0 = m-fastest)
   const float* rope_cos; const float* rope_sin;   // Epi::RoPE: fp32 [rope_L, 64]; the position of output row m is m % rope_L
   int rope_L, rope_cols;
+  const float* q_norm; const float* k_norm;       // Epi::NormRoPE: fp32 [128] weights of the q heads / of the k heads
+  int nq_heads;                                   //   heads [0, nq_heads) of the rope columns are q heads, the rest k heads
+  float norm_eps;
+  float* norm_rstd; long long ld_rstd;            //   fp32 [M, rope_cols / 128] or nullptr
+  int norm_pre;                                   //   1: tmap_out2 receives the pre-norm q|k columns [M, rope_cols]
   int l2_hints;         // TMA L2 eviction priorities: bit 0 = A loads evict_last (the panel the resident CTAs share across waves),
                         // bit 1 = B loads evict_first (streamed once per band), bit 2 = output stores evict_first
 };
@@ -224,6 +231,92 @@ __device__ __forceinline__ void epilogue_drain_tile(const GemmEpilogue& ep, cons
         for (int g = 0; g < 4; ++g)
           *reinterpret_cast<bf16x8*>(st + (((h * 4 + g) ^ sw) << 4)) = pack8(f + g * 8);
       }
+    } else if (EPI == Epi::NormRoPE && col0 < ep.rope_cols) {
+      // per-head RMSNorm, then RoPE (Qwen3: q_norm / k_norm over each head's 128 columns, weight [128]). The thread's row of the
+      // head is in this tile's accumulator (both 64-column halves), so the sum of squares needs no exchange between threads.
+      // Both halves sum the head in column order (x1 then x2), so the two groups that store them use the same rstd.
+      // Order, all fp32 before the single bf16 store: + bias, x * rsqrt(mean(x^2) + eps) * w, rotate_half.
+      const bool second = ((col0 >> 6) & 1) != 0;
+      const int cp = second ? c - 64 : c + 64;
+      const int colp = tile_col0 + cp;
+      const int c1 = second ? cp : c;                           // the head's first half, in tile columns
+      const int head = col0 >> 7;
+      const float* nw = head < ep.nq_heads ? ep.q_norm : ep.k_norm;
+      const int jo = second ? 64 : 0, jp = 64 - jo;             // in-head offsets of this block and of its partner
+      float ss = 0.f;
+#pragma unroll 1
+      for (int h = 0; h < 4; ++h) {
+        uint32_t v[32];
+        acc_ld32(arow + (c1 + h * 32), v);
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+          float x = __uint_as_float(v[i]);
+          if (ep.bias) x += __ldg(ep.bias + tile_col0 + c1 + h * 32 + i);
+          ss = fmaf(x, x, ss);
+        }
+      }
+      const float rstd = rsqrtf(ss * (1.f / 128.f) + ep.norm_eps);
+      if (ep.norm_rstd && row_ok && !second) ep.norm_rstd[(size_t)row * ep.ld_rstd + head] = rstd;
+      const int pos = row_ok ? (row % ep.rope_L) : 0;
+      const float* cs = ep.rope_cos + (size_t)pos * 64;
+      const float* sn = ep.rope_sin + (size_t)pos * 64;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        uint32_t vo[32], vq[32]; float f[32];
+        acc_ld32(arow + (c + h * 32), vo);
+        acc_ld32(arow + (cp + h * 32), vq);
+        float cc[32], ss2[32];
+#pragma unroll
+        for (int i = 0; i < 32; i += 4) {
+          *reinterpret_cast<float4*>(cc + i) = __ldg(reinterpret_cast<const float4*>(cs + h * 32 + i));
+          *reinterpret_cast<float4*>(ss2 + i) = __ldg(reinterpret_cast<const float4*>(sn + h * 32 + i));
+        }
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+          float own = __uint_as_float(vo[i]), oth = __uint_as_float(vq[i]);
+          if (ep.bias) {
+            own += __ldg(ep.bias + col0 + h * 32 + i);
+            oth += __ldg(ep.bias + colp + h * 32 + i);
+          }
+          own = own * rstd * __ldg(nw + jo + h * 32 + i);
+          oth = oth * rstd * __ldg(nw + jp + h * 32 + i);
+          f[i] = second ? fmaf(own, cc[i], oth * ss2[i]) : fmaf(own, cc[i], -oth * ss2[i]);
+        }
+#pragma unroll
+        for (int g = 0; g < 4; ++g)
+          *reinterpret_cast<bf16x8*>(st + (((h * 4 + g) ^ sw) << 4)) = pack8(f + g * 8);
+      }
+      fence_proxy_async();
+      named_bar_sync(1 + grp, 128);
+      if (issuer) {
+        if (ep.l2_hints & 4) tma_store_2d_hint(tmap_out, tile, col0, tile_row0, l2_policy_evict_first());
+        else                 tma_store_2d(tmap_out, tile, col0, tile_row0);
+        bulk_commit();
+      }
+      if (!ep.norm_pre) continue;
+      // the pre-norm block (+ bias, rounded once to bf16) through the same staging tile, once the TMA unit has read it
+      if (issuer) bulk_wait_read<0>();
+      named_bar_sync(1 + grp, 128);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        uint32_t v[32]; float f[32];
+        acc_ld32(arow + (c + h * 32), v);
+#pragma unroll
+        for (int i = 0; i < 32; ++i) {
+          f[i] = __uint_as_float(v[i]);
+          if (ep.bias) f[i] += __ldg(ep.bias + col0 + h * 32 + i);
+        }
+#pragma unroll
+        for (int g = 0; g < 4; ++g)
+          *reinterpret_cast<bf16x8*>(st + (((h * 4 + g) ^ sw) << 4)) = pack8(f + g * 8);
+      }
+      fence_proxy_async();
+      named_bar_sync(1 + grp, 128);
+      if (issuer) {
+        tma_store_2d(tmap_out2, tile, col0, tile_row0);
+        bulk_commit();
+      }
+      continue;
     } else if (EPI == Epi::GeluPair) {
       // GELU forward, both tensors: the 64-column block goes out twice through the same staging tile - first the bf16
       // pre-activation, then gelu() of those ROUNDED values (exactly what gelu_fwd_kernel would read back from HBM).
@@ -385,7 +478,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
     prefetch_tmap(&tmap_a);
     prefetch_tmap(&tmap_b);
     prefetch_tmap(&tmap_out);
-    if constexpr (EPI == Epi::SwiGLU || EPI == Epi::GeluPair) prefetch_tmap(&tmap_out2);
+    if constexpr (EPI == Epi::SwiGLU || EPI == Epi::GeluPair || EPI == Epi::NormRoPE) prefetch_tmap(&tmap_out2);
   }
   if (threadIdx.x == 32) {
     // consumer releases: one arrive per consumer warp, of every CTA whose producer writes into this stage
@@ -797,9 +890,13 @@ extern "C" int dalm_b200_gemm_bf16_gelu(const void* A, long long lda, const void
 // fused q|k|v projection + rotary embedding: out[M,N] = A[M,K] B[N,K]^T + bias with HF's rotate_half RoPE (head_dim 128) applied to
 // the output columns [0, rope_cols) in the epilogue. cos / sin: fp32 [L, 64]; row m sits at position m % L (token-major [B*L] rows).
 // bias: fp32 [N] or NULL, added before the rotation on every column.
+// q_norm != NULL (Qwen3): each 128-column head of [0, rope_cols) is RMS-normalised before the rotation, with weight q_norm on heads
+// [0, nq_heads) and k_norm on the rest; pre_out (bf16 [M, rope_cols], ld_pre) receives the pre-norm columns and rstd_out (fp32
+// [M, rope_cols / 128], ld_rstd) the heads' rstd, each when non-NULL. q_norm == NULL launches the plain RoPE instance.
 extern "C" int dalm_b200_gemm_bf16_rope(const void* A, long long lda, const void* B, long long ldb, void* out, long long ldo, int M,
                                         int N, int K, const float* bias, const float* cos_t, const float* sin_t, int L, int rope_cols,
-                                        void* stream) {
+                                        const float* q_norm, const float* k_norm, int nq_heads, float eps, void* pre_out,
+                                        long long ld_pre, float* rstd_out, long long ld_rstd, void* stream) {
   DALM_REQUIRE(M > 0 && N > 0 && K > 0 && (N % 8) == 0 && (K % 8) == 0, "gemm_rope: bad shape M=%d N=%d K=%d", M, N, K);
   DALM_REQUIRE(rope_cols > 0 && rope_cols <= N && (rope_cols % 256) == 0, "gemm_rope: rope_cols=%d must be a multiple of 256 (whole 128-wide heads per tile)", rope_cols);
   DALM_REQUIRE(L > 0 && cos_t != nullptr && sin_t != nullptr && ((uintptr_t)cos_t & 15) == 0 && ((uintptr_t)sin_t & 15) == 0, "gemm_rope: cos / sin tables");
@@ -811,7 +908,20 @@ extern "C" int dalm_b200_gemm_bf16_rope(const void* A, long long lda, const void
   GemmEpilogue ep = gemm_epilogue(M, N, K, 256, out, ldo);
   ep.bias = bias;
   ep.rope_cos = cos_t; ep.rope_sin = sin_t; ep.rope_L = L; ep.rope_cols = rope_cols;
-  return launch_gemm<256, 0, Epi::RoPE>(ta, tb, to, ep, 0, (cudaStream_t)stream, nullptr);
+  if (q_norm == nullptr) {
+    DALM_REQUIRE(k_norm == nullptr && pre_out == nullptr && rstd_out == nullptr, "gemm_rope: k_norm / pre_out / rstd_out need q_norm");
+    return launch_gemm<256, 0, Epi::RoPE>(ta, tb, to, ep, 0, (cudaStream_t)stream, nullptr);
+  }
+  DALM_REQUIRE(k_norm != nullptr && nq_heads >= 0 && nq_heads <= rope_cols / 128 && eps >= 0.f, "gemm_rope: norm weights / nq_heads=%d", nq_heads);
+  DALM_REQUIRE(rstd_out == nullptr || ld_rstd >= rope_cols / 128, "gemm_rope: ld_rstd=%lld < %d heads", ld_rstd, rope_cols / 128);
+  CUtensorMap to2 = to;
+  if (pre_out != nullptr) {
+    DALM_REQUIRE(ld_pre >= rope_cols && (ld_pre % 8) == 0 && ((uintptr_t)pre_out & 15) == 0, "gemm_rope: pre_out leading dimension / alignment");
+    if (int e = get_tmap(pre_out, M, rope_cols, ld_pre, 128, &to2, 0)) return e;
+  }
+  ep.q_norm = q_norm; ep.k_norm = k_norm; ep.nq_heads = nq_heads; ep.norm_eps = eps;
+  ep.norm_rstd = rstd_out; ep.ld_rstd = ld_rstd; ep.norm_pre = pre_out != nullptr;
+  return launch_gemm<256, 0, Epi::NormRoPE>(ta, tb, to, ep, 0, (cudaStream_t)stream, &to2);
 }
 
 // drop cached tensor maps (call when operand buffers are freed / re-allocated at the same address with other shapes)

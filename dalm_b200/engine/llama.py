@@ -1,4 +1,4 @@
-"""Llama / Qwen2 decoder (Llama-2-7B / Qwen2.5-7B shape and smaller) forward + backward as a launch sequence over the C-ABI kernels.
+"""Llama / Qwen2 / Qwen3 decoder (Llama-2-7B / Qwen2.5-7B / Qwen3-8B shape and smaller) forward + backward as a launch sequence over the C-ABI kernels.
 
 Mirrors `self.generator_model(input_ids=..., attention_mask=...).logits` of the reference
 (dalm/models/rag_e2e_base_model.py:104-106) through HF LlamaForCausalLM: embed -> N x [RMSNorm -> QKV(+LoRA on q,v)
@@ -9,9 +9,12 @@ HBM layout per layer (bf16 unless noted):
   WqkvT_aug [H, Nq+2Nkv+Ra] resident transpose for dgrad, last Ra columns = A_q^T | A_v^T
   A_stack [64,H], Bblk [64, Nq+2Nkv]   LoRA down / mid-gradient operands (see bert.py)
   Wo [H,Nq], WoT; Wgu [2F,H] (gate rows, then up rows), WguT [H,2F]; Wd [H,F], WdT [F,H]; RMSNorm gains fp32
-  bqkv [Nq+2Nkv], bo [H] fp32: attention biases (Qwen2: q|k|v only; Llama with attention_bias: both), added in the GEMM epilogues
+  bqkv [Nq+2Nkv], bo [H] fp32: attention biases (Qwen2: q|k|v only; Llama / Qwen3 with attention_bias: both), added in the GEMM epilogues
+  qn, kn [128] fp32: Qwen3's per-head q_norm / k_norm weights (RMSNorm of each q / k head before RoPE)
 Residual stream and its gradient are fp32; every GEMM operand is bf16.
-Qwen2 is this architecture plus q/k/v biases (HF Qwen2ForCausalLM); configs are checked by params.check_llama_family.
+Qwen2 is this architecture plus q/k/v biases (HF Qwen2ForCausalLM); Qwen3 (HF Qwen3ForCausalLM) adds the per-head q/k RMSNorm,
+fused into the QKV GEMM's RoPE epilogue (training shapes) or applied by the qk_norm_rope row kernel (decode, prefill, other
+widths); the backward saves the pre-norm q|k columns and their rstd. Configs are checked by params.check_llama_family.
 """
 from __future__ import annotations
 
@@ -59,8 +62,9 @@ class LlamaDecoder(torch.nn.Module):
             self.nf4 = Nf4Store(device)
         check_llama_family(cfg)
         self.cfg = cfg
-        self.kind = "qwen2" if cfg.get("model_type") == "qwen2" else "llama"
+        self.kind = cfg.get("model_type") if cfg.get("model_type") in ("qwen2", "qwen3") else "llama"
         self.qkv_bias, self.o_bias = attention_biases(self.kind, cfg)
+        self.qk_norm = self.kind == "qwen3"
         self.H = H = cfg["hidden_size"]
         self.F = F = cfg["intermediate_size"]
         self.nl = cfg["num_hidden_layers"]
@@ -142,6 +146,8 @@ class LlamaDecoder(torch.nn.Module):
                 m.append((f"L{l}.bqkv", "acc", [p + f"self_attn.{n}_proj.bias" for n in "qkv"]))
             if self.o_bias:
                 m.append((f"L{l}.bo", "acc", [p + "self_attn.o_proj.bias"]))
+            if self.qk_norm:                                     # q / k norm weights: "acc" entries (the backward kernel's atomics)
+                m += [(f"L{l}.qn", "acc", [p + "self_attn.q_norm.weight"]), (f"L{l}.kn", "acc", [p + "self_attn.k_norm.weight"])]
             m += [(f"L{l}.Wqkv", "gemm", [p + f"self_attn.{n}_proj.weight" for n in "qkv"]),
                   (f"L{l}.Wo", "gemm", [p + "self_attn.o_proj.weight"]),
                   (f"L{l}.Wgu", "gemm", [p + "mlp.gate_proj.weight", p + "mlp.up_proj.weight"]),
@@ -181,7 +187,9 @@ class LlamaDecoder(torch.nn.Module):
             self.layers.append({"Wqkv_aug": bank.w16(k("Wqkv")), "Wo": bank.w16(k("Wo")), "Wgu": bank.w16(k("Wgu")),
                                 "Wd": bank.w16(k("Wd")), "g1": bank.w32(k("g1")), "g2": bank.w32(k("g2")),
                                 "bqkv": bank.w32(k("bqkv")) if self.qkv_bias else None,
-                                "bo": bank.w32(k("bo")) if self.o_bias else None})
+                                "bo": bank.w32(k("bo")) if self.o_bias else None,
+                                "qn": bank.w32(k("qn")) if self.qk_norm else None,
+                                "kn": bank.w32(k("kn")) if self.qk_norm else None})
 
     def hf_state_dict(self) -> Dict[str, torch.Tensor]:
         """fp32 CPU tensors under HF LlamaForCausalLM names (save_pretrained of a fully fine-tuned decoder)"""
@@ -304,10 +312,13 @@ class LlamaDecoder(torch.nn.Module):
         return W
 
     def _frozen_biases(self, W, p: str, g) -> None:
-        """frozen / LoRA modes: the attention biases are forward-only fp32 vectors (under use_bnb they take the fp16 cast of every
+        """frozen / LoRA modes: the attention biases (and Qwen3's q / k norm weights) are forward-only fp32 vectors (under use_bnb they take the fp16 cast of every
         non-Linear-weight tensor, never the NF4 round trip)"""
         W["bqkv"] = torch.cat([g(p + f"self_attn.{n}_proj.bias", f32) for n in "qkv"]) if self.qkv_bias else None
         W["bo"] = g(p + "self_attn.o_proj.bias", f32) if self.o_bias else None
+        # Qwen3's q / k norm weights: forward-only fp32 vectors here too (use_bnb: the fp16 cast, as every norm weight)
+        W["qn"] = g(p + "self_attn.q_norm.weight", f32) if self.qk_norm else None
+        W["kn"] = g(p + "self_attn.k_norm.weight", f32) if self.qk_norm else None
 
     def _drop(self, training: bool, call: int, layer: int):
         if not training or self.p_lora <= 0.0:
@@ -424,12 +435,21 @@ class LlamaDecoder(torch.nn.Module):
                 ops.skinny_gemm(a.h1_aug[:, :H], W["A_stack"], a.h1_aug[:, H:], K=H, R=Ra,   # u = dropout(h1) A^T [M,2r]
                                 dropx=self._drop(ctx.training, ctx.call, li))
             rope_cols = (self.nh + self.nkv) * self.hd
+            a.pre = a.qk_rstd = None
+            if self.qk_norm and save and self.trainable:                         # what the q/k norm backward reads
+                a.pre = torch.empty(M, rope_cols, dtype=bf16, device=self.dev)
+                a.qk_rstd = torch.empty(M, self.nh + self.nkv, dtype=f32, device=self.dev)
             if pos is None and self.fuse_rope and rope_cols % 256 == 0:
-                a.qkv = ops.gemm_rope(a.h1_aug, W["Wqkv_aug"], cos_t, sin_t, L, rope_cols,   # QKV (+LoRA, + bias) with RoPE in
-                                      bias=W["bqkv"])                                        # the epilogue
+                norm = dict(q_norm=W["qn"], k_norm=W["kn"], nq_heads=self.nh, eps=self.eps, pre_out=a.pre,
+                            rstd_out=a.qk_rstd) if self.qk_norm else {}
+                a.qkv = ops.gemm_rope(a.h1_aug, W["Wqkv_aug"], cos_t, sin_t, L, rope_cols,   # QKV (+LoRA, + bias) with (q/k norm
+                                      bias=W["bqkv"], **norm)                                # and) RoPE in the epilogue
             else:
                 a.qkv = ops.gemm(a.h1_aug, W["Wqkv_aug"], bias=W["bqkv"])        # [M, Nq+2Nkv]
-                if pos is None:
+                if self.qk_norm:
+                    ops.qk_norm_rope_(a.qkv, self.nh + self.nkv, self.nh, W["qn"], W["kn"], self.eps, cos_t, sin_t,
+                                      L=L if pos is None else 0, pos=pos, pre=a.pre, rstd=a.qk_rstd)
+                elif pos is None:
                     ops.rope_(a.qkv, 0, self.nh + self.nkv, self.hd, cos_t, sin_t, L)    # q heads then k heads are adjacent
                 else:
                     ops.rope_pos_(a.qkv, 0, self.nh + self.nkv, self.hd, cos_t, sin_t, pos)
@@ -466,7 +486,10 @@ class LlamaDecoder(torch.nn.Module):
             if Ra:
                 ops.skinny_gemm(h1_aug[:, :H], W["A_stack"], h1_aug[:, H:], K=H, R=Ra)
             qkv = ops.gemm_rows(h1_aug, W["Wqkv_aug"], bias=W["bqkv"])                # [B, Nq+2Nkv]
-            ops.rope_pos_(qkv, 0, self.nh + self.nkv, self.hd, cos_t, sin_t, pos)
+            if self.qk_norm:
+                ops.qk_norm_rope_(qkv, self.nh + self.nkv, self.nh, W["qn"], W["kn"], self.eps, cos_t, sin_t, pos=pos)
+            else:
+                ops.rope_pos_(qkv, 0, self.nh + self.nkv, self.hd, cos_t, sin_t, pos)
             att = ops.attention_decode(qkv, 0, self.Nq, self.Nq + self.Nkv, caches[li][0], caches[li][1], kmask, cur,
                                        self.nh, self.nkv, self.hd)
             x_mid = ops.gemm_rows(att, W["Wo"], out_dtype=f32, resid=x, bias=W["bo"])
@@ -550,7 +573,11 @@ class LlamaDecoder(torch.nn.Module):
                      ctx.mask, a.att, a.lse, datt, B, L, self.nh, self.nkv, self.hd, causal=True,
                      dq=dqkv[:, :self.Nq], dk=dqkv[:, self.Nq:self.Nq + self.Nkv],
                      dv=dqkv[:, self.Nq + self.Nkv:self.Nqkv])
-            ops.rope_(dqkv, 0, self.nh + self.nkv, self.hd, cos_t, sin_t, L, backward=True)
+            if self.qk_norm:                                                       # un-rotate, then the q/k RMSNorm backward
+                ops.qk_norm_rope_bwd_(dqkv, self.nh + self.nkv, self.nh, W["qn"], W["kn"], cos_t, sin_t, L, a.pre, a.qk_rstd,
+                                      dw_q=G(l, "qn") if bank is not None else None, dw_k=G(l, "kn") if bank is not None else None)
+            else:
+                ops.rope_(dqkv, 0, self.nh + self.nkv, self.hd, cos_t, sin_t, L, backward=True)
             if bank is not None:
                 ops.wgrad_(dqkv, a.h1_aug[:, :H], G(l, "Wqkv"), acc)
                 if self.qkv_bias:                                                  # d bqkv = column sums of d(pre-RoPE qkv)

@@ -19,10 +19,12 @@ def _normal(gen: torch.Generator, shape, std: float, dtype, device) -> torch.Ten
 
 
 def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, device="cpu",
-                      bias_std: Optional[float] = None) -> Dict[str, torch.Tensor]:
-    """HF parameter names for BertModel (no prefix) / LlamaForCausalLM / Qwen2ForCausalLM / FalconForCausalLM, init
-    N(0, initializer_range), LN = (1, 0). Decoder attention biases (Qwen2's q/k/v, Llama's `attention_bias`) are drawn from
-    N(0, bias_std) (default: initializer_range) rather than HF's zeros, so that a dropped bias changes the outputs."""
+                      bias_std: Optional[float] = None, qk_norm_std: Optional[float] = None) -> Dict[str, torch.Tensor]:
+    """HF parameter names for BertModel (no prefix) / LlamaForCausalLM / Qwen2ForCausalLM / Qwen3ForCausalLM /
+    FalconForCausalLM, init N(0, initializer_range), LN = (1, 0). Decoder attention biases (Qwen2's q/k/v, Llama's and Qwen3's
+    `attention_bias`) are drawn from N(0, bias_std) (default: initializer_range) rather than HF's zeros, so that a dropped bias
+    changes the outputs. Qwen3's q_norm / k_norm weights are 1 + N(0, qk_norm_std) (default: initializer_range), so that a
+    dropped or swapped norm shows."""
     on_device = torch.device(device).type == "cuda" and cfg.get("_device_rng", False)
     gen = torch.Generator(device=device) if on_device else torch.Generator()
     gen.manual_seed(seed)
@@ -55,7 +57,7 @@ def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, 
             sd[p + "output.LayerNorm.bias"] = _normal(gen, (H,), std, dtype, device)
         sd["pooler.dense.weight"] = _normal(gen, (H, H), std, dtype, device)   # loaded by AutoModel, unused by the path
         sd["pooler.dense.bias"] = zeros(H)
-    elif kind in ("llama", "qwen2"):
+    elif kind in ("llama", "qwen2", "qwen3"):
         F, V = cfg["intermediate_size"], cfg["vocab_size"]
         nh, nkv = cfg["num_attention_heads"], cfg.get("num_key_value_heads", cfg["num_attention_heads"])
         hd = cfg.get("head_dim") or H // nh
@@ -74,6 +76,10 @@ def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, 
                 sd[p + "self_attn.v_proj.bias"] = _normal(gen, (nkv * hd,), bstd, dtype, device)
             if o_bias:
                 sd[p + "self_attn.o_proj.bias"] = _normal(gen, (H,), bstd, dtype, device)
+            if kind == "qwen3":
+                nstd = std if qk_norm_std is None else float(qk_norm_std)
+                sd[p + "self_attn.q_norm.weight"] = ones(hd) + _normal(gen, (hd,), nstd, dtype, device)
+                sd[p + "self_attn.k_norm.weight"] = ones(hd) + _normal(gen, (hd,), nstd, dtype, device)
             sd[p + "mlp.gate_proj.weight"] = _normal(gen, (F, H), std, dtype, device)
             sd[p + "mlp.up_proj.weight"] = _normal(gen, (F, H), std, dtype, device)
             sd[p + "mlp.down_proj.weight"] = _normal(gen, (H, F), std, dtype, device)
@@ -145,13 +151,13 @@ def model_kind(cfg: Dict) -> str:
     mt = cfg.get("model_type", "")
     if mt == "bert":
         return "bert"
-    if mt in ("llama", "qwen2"):
+    if mt in ("llama", "qwen2", "qwen3"):
         check_llama_family(cfg)
         return mt
     if mt == "falcon":
         return "falcon"
     raise NotImplementedError(
-        f"model_type {mt!r} is not built in dalm_b200 (supported: bert encoders; llama, qwen2 and falcon decoders)")
+        f"model_type {mt!r} is not built in dalm_b200 (supported: bert encoders; llama, qwen2, qwen3 and falcon decoders)")
 
 
 def _rope_type(cfg: Dict) -> str:
@@ -165,21 +171,25 @@ def _rope_type(cfg: Dict) -> str:
 
 
 def check_llama_family(cfg: Dict) -> None:
-    """refuses the settings of a llama / qwen2 config that LlamaDecoder would otherwise silently compute wrong"""
+    """refuses the settings of a llama / qwen2 / qwen3 config that LlamaDecoder would otherwise silently compute wrong"""
     mt = cfg.get("model_type", "")
     if cfg.get("mlp_bias", False):
         raise NotImplementedError(f"{mt}: mlp_bias=true is not built (the fused SwiGLU MLP has no bias)")
-    if mt == "qwen2":
+    if mt == "qwen3":
+        hd = cfg.get("head_dim") or cfg["hidden_size"] // cfg["num_attention_heads"]
+        if hd != 128:
+            raise NotImplementedError(f"qwen3: head_dim={hd} is not built (the q/k norm kernels take head_dim 128)")
+    if mt in ("qwen2", "qwen3"):
         if cfg.get("use_sliding_window", False) or "sliding_attention" in (cfg.get("layer_types") or ()):
-            raise NotImplementedError("qwen2: sliding-window attention (use_sliding_window=true) is not built")
+            raise NotImplementedError(f"{mt}: sliding-window attention (use_sliding_window=true) is not built")
         rt = _rope_type(cfg)
         if rt != "default":
-            raise NotImplementedError(f"qwen2: RoPE type {rt!r} (rope_scaling / rope_parameters) is not built; only 'default'")
+            raise NotImplementedError(f"{mt}: RoPE type {rt!r} (rope_scaling / rope_parameters) is not built; only 'default'")
 
 
 def attention_biases(kind: str, cfg: Dict):
     """(q/k/v projections carry a bias, o_proj carries a bias) for a llama-family config: Qwen2 has q/k/v biases only, Llama
-    has all four when `attention_bias` is set"""
+    and Qwen3 have all four when `attention_bias` is set"""
     if kind == "qwen2":
         return True, False
     ab = bool(cfg.get("attention_bias", False))

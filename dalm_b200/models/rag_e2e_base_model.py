@@ -65,7 +65,7 @@ def load_tokenizer(name_or_path: str):
 
 def build_encoder(name_or_path: str, lora: bool, device: torch.device, state_dict: Optional[Dict] = None,
                   cfg: Optional[Dict] = None, autoregressive: bool = False, full: bool = False, bnb: bool = False):
-    """BERT-family encoder (bge-*), or — `retriever_is_autoregressive` — a Llama / Qwen2 decoder used as an encoder
+    """BERT-family encoder (bge-*), or — `retriever_is_autoregressive` — a Llama / Qwen2 / Qwen3 decoder used as an encoder
     (last hidden state, eos pooling; LoRA targets q_proj / v_proj: reference rag_e2e_base_model.py:66-70,84-90)"""
     cfg = cfg or params.load_config(name_or_path)
     kind = params.model_kind(cfg)
@@ -74,8 +74,8 @@ def build_encoder(name_or_path: str, lora: bool, device: torch.device, state_dic
     if not nf4:
         sd = _maybe_bnb(sd, bnb, full, device)
     if autoregressive:
-        if kind not in ("llama", "qwen2"):
-            raise NotImplementedError("autoregressive retrievers are built for Llama and Qwen2 models only")
+        if kind not in ("llama", "qwen2", "qwen3"):
+            raise NotImplementedError("autoregressive retrievers are built for Llama, Qwen2 and Qwen3 models only")
         return _named(LlamaDecoder(cfg, sd, device=device, lora=lora, lora_seed=0, full=full, nf4_storage=nf4), name_or_path)
     if kind != "bert":
         raise NotImplementedError("non-autoregressive retrievers must be BERT-family encoders (bge-*); pass "
@@ -131,7 +131,7 @@ def build_decoder(name_or_path: str, lora: bool, device: torch.device, state_dic
         sd = _maybe_bnb(sd, bnb, full, device)
     if kind == "falcon":
         dec = FalconDecoder(cfg, sd, device=device, lora=lora, full=full)      # raises for lora=True, like peft would
-    elif kind not in ("llama", "qwen2"):
+    elif kind not in ("llama", "qwen2", "qwen3"):
         raise NotImplementedError(f"generator of kind {kind!r} is not a causal decoder")
     else:
         dec = LlamaDecoder(cfg, sd, device=device, lora=lora, full=full, nf4_storage=nf4)

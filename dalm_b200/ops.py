@@ -493,26 +493,98 @@ def _chk_bias(bias: Optional[torch.Tensor], N: int, what: str) -> None:
 
 
 def gemm_rope(a: torch.Tensor, w: torch.Tensor, cos_t: torch.Tensor, sin_t: torch.Tensor, L: int, rope_cols: int,
-              out: Optional[torch.Tensor] = None, bias: Optional[torch.Tensor] = None) -> torch.Tensor:
+              out: Optional[torch.Tensor] = None, bias: Optional[torch.Tensor] = None, *, q_norm: Optional[torch.Tensor] = None,
+              k_norm: Optional[torch.Tensor] = None, nq_heads: int = 0, eps: float = 1e-6, pre_out: Optional[torch.Tensor] = None,
+              rstd_out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """q|k|v projection with RoPE (head_dim 128) on the first `rope_cols` output columns fused into the GEMM epilogue.
     a [M,K], w [N,K] bf16; cos_t / sin_t fp32 [L, 64]; rows are token-major (position = row % L). bias: fp32 [N], added in fp32
-    before the rotation (Qwen2's q/k/v biases)."""
+    before the rotation (Qwen2's q/k/v biases).
+    q_norm / k_norm (fp32 [128], Qwen3): each head of the rope columns is RMS-normalised (eps) before the rotation, heads
+    [0, nq_heads) with q_norm, the rest with k_norm. pre_out (bf16 [M, rope_cols]) / rstd_out (fp32 [M, rope_cols // 128])
+    receive the pre-norm columns and the heads' rstd, which `qk_norm_rope_bwd_` reads."""
     _chk(a, bf16, "gemm_rope a"); _chk(w, bf16, "gemm_rope w"); _chk(cos_t, f32, "gemm_rope cos"); _chk(sin_t, f32, "gemm_rope sin")
     M, K = a.shape
     N = w.shape[0]
     _chk_bias(bias, N, "gemm_rope bias")
     if cos_t.shape != (L, 64) or sin_t.shape != (L, 64) or not cos_t.is_contiguous() or not sin_t.is_contiguous():
         raise _lib.DalmB200Error("gemm_rope: cos / sin must be contiguous fp32 [L, 64] (head_dim 128)")
+    if (q_norm is None) != (k_norm is None) or (q_norm is None and (pre_out is not None or rstd_out is not None)):
+        raise _lib.DalmB200Error("gemm_rope: q_norm and k_norm go together; pre_out / rstd_out need them")
+    if q_norm is not None:
+        _chk_norm_w(q_norm, "gemm_rope q_norm"); _chk_norm_w(k_norm, "gemm_rope k_norm")
+        _chk_norm_saves(pre_out, rstd_out, M, rope_cols, "gemm_rope")
     if out is None:
         out = torch.empty(M, N, dtype=bf16, device=a.device)
     timer = GEMM_TIMER
     if timer is not None:
-        timer.begin(2.0 * M * N * K, (M, N, K, 0, "bfloat16", "rope", "bias" if bias is not None else "-"))
+        timer.begin(2.0 * M * N * K, (M, N, K, 0, "bfloat16", "rope" if q_norm is None else "norm_rope",
+                                      "bias" if bias is not None else "-"))
     _lib.call("dalm_b200_gemm_bf16_rope", _p(a), _ld(a), _p(w), _ld(w), _p(out), _ld(out), M, N, K, _p(bias), _p(cos_t), _p(sin_t),
-              int(L), int(rope_cols), _stream())
+              int(L), int(rope_cols), _p(q_norm), _p(k_norm), int(nq_heads), float(eps), _p(pre_out),
+              _ld(pre_out) if pre_out is not None else 0, _p(rstd_out), _ld(rstd_out) if rstd_out is not None else 0, _stream())
     if timer is not None:
         timer.end()
     return out
+
+
+def _chk_norm_w(w: torch.Tensor, what: str) -> None:
+    _chk(w, f32, what)
+    if w.shape != (128,) or not w.is_contiguous():
+        raise _lib.DalmB200Error(f"{what}: need a contiguous fp32 [128] weight, got {tuple(w.shape)}")
+
+
+def _chk_norm_saves(pre: Optional[torch.Tensor], rstd: Optional[torch.Tensor], M: int, cols: int, what: str) -> None:
+    if pre is not None:
+        _chk(pre, bf16, what + " pre")
+        if pre.dim() != 2 or pre.shape[0] != M or pre.shape[1] < cols:
+            raise _lib.DalmB200Error(f"{what}: pre must be bf16 [{M}, >= {cols}], got {tuple(pre.shape)}")
+    if rstd is not None:
+        _chk(rstd, f32, what + " rstd")
+        if rstd.dim() != 2 or rstd.shape[0] != M or rstd.shape[1] < cols // 128:
+            raise _lib.DalmB200Error(f"{what}: rstd must be fp32 [{M}, >= {cols // 128}], got {tuple(rstd.shape)}")
+
+
+def qk_norm_rope_(buf: torch.Tensor, nheads: int, nq_heads: int, q_norm: torch.Tensor, k_norm: torch.Tensor, eps: float,
+                  cos_t: torch.Tensor, sin_t: torch.Tensor, L: int = 0, pos: Optional[torch.Tensor] = None,
+                  pre: Optional[torch.Tensor] = None, rstd: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Qwen3's per-head q/k RMSNorm, then RoPE (head_dim 128), in place on the first `nheads` heads of buf [M, >= 128 nheads]
+    (bf16, token-major): heads [0, nq_heads) take q_norm, the rest k_norm. Positions: pos[M] (int64) when given, else row % L;
+    cos_t / sin_t fp32 [T, 64]. pre (bf16 [M, 128 nheads]) / rstd (fp32 [M, nheads]) optionally receive the pre-norm values and
+    the heads' rstd. Allocates nothing (safe under CUDA-graph capture)."""
+    _chk(buf, bf16, "qk_norm_rope buf"); _chk(cos_t, f32, "qk_norm_rope cos"); _chk(sin_t, f32, "qk_norm_rope sin")
+    _chk_norm_w(q_norm, "qk_norm_rope q_norm"); _chk_norm_w(k_norm, "qk_norm_rope k_norm")
+    M = buf.shape[0]
+    if cos_t.dim() != 2 or cos_t.shape[1] != 64 or sin_t.shape != cos_t.shape or not cos_t.is_contiguous() or not sin_t.is_contiguous():
+        raise _lib.DalmB200Error("qk_norm_rope: cos / sin must be contiguous fp32 [T, 64] (head_dim 128)")
+    if pos is not None:
+        _chk(pos, i64, "qk_norm_rope pos")
+        if pos.numel() != M or not pos.is_contiguous():
+            raise _lib.DalmB200Error(f"qk_norm_rope: need one contiguous position id per row ({pos.numel()} for {M} rows)")
+    _chk_norm_saves(pre, rstd, M, 128 * nheads, "qk_norm_rope")
+    _lib.call("dalm_b200_qk_norm_rope", _p(buf), _ld(buf), int(nheads), int(nq_heads), _p(q_norm), _p(k_norm), float(eps), _p(cos_t),
+              _p(sin_t), cos_t.shape[0], int(L), _p(pos), M, _p(pre), _ld(pre) if pre is not None else 0, _p(rstd),
+              _ld(rstd) if rstd is not None else 0, _stream())
+    return buf
+
+
+def qk_norm_rope_bwd_(dbuf: torch.Tensor, nheads: int, nq_heads: int, q_norm: torch.Tensor, k_norm: torch.Tensor,
+                      cos_t: torch.Tensor, sin_t: torch.Tensor, L: int, pre: torch.Tensor, rstd: torch.Tensor,
+                      dw_q: Optional[torch.Tensor] = None, dw_k: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """backward of `qk_norm_rope_` / the NormRoPE epilogue (positions row % L), in place on d(out)'s first `nheads` heads: they
+    become d(pre-norm q|k). dw_q / dw_k (fp32 [128], both or neither) accumulate the norm weights' gradients (+=)."""
+    _chk(dbuf, bf16, "qk_norm_rope_bwd dbuf"); _chk(cos_t, f32, "qk_norm_rope_bwd cos"); _chk(sin_t, f32, "qk_norm_rope_bwd sin")
+    _chk_norm_w(q_norm, "qk_norm_rope_bwd q_norm"); _chk_norm_w(k_norm, "qk_norm_rope_bwd k_norm")
+    M = dbuf.shape[0]
+    if cos_t.shape != (L, 64) or sin_t.shape != (L, 64) or not cos_t.is_contiguous() or not sin_t.is_contiguous():
+        raise _lib.DalmB200Error("qk_norm_rope_bwd: cos / sin must be contiguous fp32 [L, 64] (head_dim 128)")
+    _chk_norm_saves(pre, rstd, M, 128 * nheads, "qk_norm_rope_bwd")
+    if (dw_q is None) != (dw_k is None):
+        raise _lib.DalmB200Error("qk_norm_rope_bwd: dw_q and dw_k go together")
+    if dw_q is not None:
+        _chk_norm_w(dw_q, "qk_norm_rope_bwd dw_q"); _chk_norm_w(dw_k, "qk_norm_rope_bwd dw_k")
+    _lib.call("dalm_b200_qk_norm_rope_bwd", _p(dbuf), _ld(dbuf), int(nheads), int(nq_heads), _p(q_norm), _p(k_norm), _p(cos_t),
+              _p(sin_t), int(L), _p(pre), _ld(pre), _p(rstd), _ld(rstd), M, _p(dw_q), _p(dw_k), _stream())
+    return dbuf
 
 
 def interleave_gate_up(gate_w: torch.Tensor, up_w: torch.Tensor, block: int = 128) -> torch.Tensor:

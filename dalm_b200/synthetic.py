@@ -44,6 +44,20 @@ QWEN2_SHAPES: Dict[str, Dict] = {
 }
 
 
+# head_dim is 128 in every Qwen3 dense model and set explicitly; the q width nh * 128 need not equal hidden_size
+QWEN3_SHAPES: Dict[str, Dict] = {
+    "qwen3-tiny": dict(hidden_size=384, num_hidden_layers=2, num_attention_heads=4, num_key_value_heads=1,
+                       intermediate_size=768, tie_word_embeddings=True),    # 5 q|k heads: q/k norm + RoPE in the row kernel
+    "qwen3-hd128": dict(hidden_size=512, num_hidden_layers=2, num_attention_heads=6, num_key_value_heads=2,
+                        intermediate_size=1024, tie_word_embeddings=False),  # 8 q|k heads: q/k norm + RoPE in the QKV epilogue
+    # published Qwen/Qwen3-0.6B and Qwen/Qwen3-8B config.json values (written from the model cards; not re-fetched offline)
+    "qwen3-0.6b": dict(hidden_size=1024, num_hidden_layers=28, num_attention_heads=16, num_key_value_heads=8,
+                       intermediate_size=3072, tie_word_embeddings=True),
+    "qwen3-8b": dict(hidden_size=4096, num_hidden_layers=36, num_attention_heads=32, num_key_value_heads=8,
+                     intermediate_size=12288, tie_word_embeddings=False),
+}
+
+
 FALCON_SHAPES: Dict[str, Dict] = {
     "falcon-tiny": dict(hidden_size=128, num_hidden_layers=2, num_attention_heads=2),
     "falcon-mini": dict(hidden_size=448, num_hidden_layers=2, num_attention_heads=7),          # 7 q heads x 64, one KV head
@@ -88,6 +102,19 @@ def qwen2_config(name: str, vocab_size: int = 152064) -> Dict:
         architectures=["Qwen2ForCausalLM"], model_type="qwen2", vocab_size=vocab_size, max_position_embeddings=32768,
         hidden_act="silu", rms_norm_eps=1e-6, rope_theta=1000000.0, initializer_range=0.02, bos_token_id=0, eos_token_id=0,
         use_sliding_window=False, sliding_window=None, max_window_layers=s["num_hidden_layers"], attention_dropout=0.0, **s,
+    )
+
+
+def qwen3_config(name: str, vocab_size: int = 151936) -> Dict:
+    """Qwen3 dense (HF Qwen3ForCausalLM): Llama plus a per-head RMSNorm of q and k before RoPE (q_norm / k_norm, weight [128]),
+    head_dim 128, no attention biases, rope_theta 1e6, rms_norm_eps 1e-6, full attention on every layer. Token ids follow the
+    synthetic ChatML tokenizer (<|endoftext|> = 0), not the published 151643 / 151645."""
+    s = QWEN3_SHAPES[name]
+    return dict(
+        architectures=["Qwen3ForCausalLM"], model_type="qwen3", vocab_size=vocab_size, max_position_embeddings=40960,
+        hidden_act="silu", rms_norm_eps=1e-6, rope_theta=1000000.0, rope_scaling=None, initializer_range=0.02, bos_token_id=0,
+        eos_token_id=0, head_dim=128, attention_bias=False, attention_dropout=0.0, use_sliding_window=False, sliding_window=None,
+        max_window_layers=s["num_hidden_layers"], **s,
     )
 
 
@@ -234,15 +261,24 @@ QWEN2_GENERATION = {
 }
 
 
+# Qwen3 base checkpoints decode greedily; the hybrid-thinking / Instruct ones sample (temperature 0.6, top-k 20, top-p 0.95)
+# and stop at <|im_end|> or <|endoftext|>. Ids mapped onto the synthetic tokenizer.
+QWEN3_GENERATION = {
+    "base": dict(bos_token_id=0, eos_token_id=0, do_sample=False, max_new_tokens=2048),
+    "instruct": dict(bos_token_id=0, eos_token_id=[2, 0], pad_token_id=0, do_sample=True, temperature=0.6, top_k=20, top_p=0.95),
+}
+
+
 # ---------------------------------------------------------------------------------------------------------------
 # model directories
 # ---------------------------------------------------------------------------------------------------------------
 def write_model_dir(out_dir: str, kind: str, name: str, vocab_size: Optional[int] = None, with_weights: bool = True,
-                    seed: int = 0, generation_config: Optional[Dict] = None, bias_std: Optional[float] = None) -> str:
-    """kind: 'bert' | 'llama' | 'qwen2' | 'falcon'. Writes config.json, tokenizer files and (optionally) seeded random-init
+                    seed: int = 0, generation_config: Optional[Dict] = None, bias_std: Optional[float] = None,
+                    qk_norm_std: Optional[float] = None) -> str:
+    """kind: 'bert' | 'llama' | 'qwen2' | 'qwen3' | 'falcon'. Writes config.json, tokenizer files and (optionally) seeded random-init
     safetensors in HF parameter naming so both transformers (oracle) and dalm_b200 (product) can load the same directory.
     generation_config: written as generation_config.json when given (e.g. QWEN2_GENERATION["base"]). bias_std: std of the
-    random attention biases (engine/params.random_state_dict)."""
+    random attention biases, qk_norm_std the spread of Qwen3's q / k norm weights around 1 (engine/params.random_state_dict)."""
     os.makedirs(out_dir, exist_ok=True)
     if kind == "bert":
         cfg = bert_config(name, vocab_size or 30522)
@@ -253,6 +289,9 @@ def write_model_dir(out_dir: str, kind: str, name: str, vocab_size: Optional[int
     elif kind == "qwen2":
         cfg = qwen2_config(name, vocab_size or 152064)
         build_qwen2_tokenizer(out_dir, cfg["vocab_size"])
+    elif kind == "qwen3":
+        cfg = qwen3_config(name, vocab_size or 151936)
+        build_qwen2_tokenizer(out_dir, cfg["vocab_size"])          # Qwen3 keeps Qwen2's byte-level BPE and Qwen2Tokenizer
     elif kind == "falcon":
         cfg = falcon_config(name, vocab_size or 65024)
         build_llama_tokenizer(out_dir, cfg["vocab_size"])       # any causal-LM tokenizer works for the synthetic fixture
@@ -272,6 +311,6 @@ def write_model_dir(out_dir: str, kind: str, name: str, vocab_size: Optional[int
 
         from .engine.params import random_state_dict
 
-        sd = random_state_dict(kind, cfg, seed=seed, dtype=torch.float32, device="cpu", bias_std=bias_std)
+        sd = random_state_dict(kind, cfg, seed=seed, dtype=torch.float32, device="cpu", bias_std=bias_std, qk_norm_std=qk_norm_std)
         save_file({k: v.contiguous() for k, v in sd.items()}, os.path.join(out_dir, "model.safetensors"))
     return out_dir

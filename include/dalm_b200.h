@@ -91,8 +91,15 @@ int dalm_b200_gemm_bf16_swiglu(const void* A, long long lda, const void* B, long
  * fp32 [L, 64]; output row m is at position m % L. Replaces q_proj / k_proj / v_proj + apply_rotary_pos_emb of HF LlamaAttention.
  * bias: fp32 [N] or NULL (Qwen2's q/k/v biases): added to the fp32 accumulator before the rotation and the single bf16 rounding,
  * on every column; NULL leaves the results bit-identical to a bias-free projection. */
+/* q_norm != NULL (Qwen3): every 128-column head of [0, rope_cols) is RMS-normalised before the rotation, all in fp32 before the
+ * single bf16 store: x * rsqrt(mean(x^2) + eps) * w, with w = q_norm (fp32 [128]) on heads [0, nq_heads) and k_norm on the
+ * rest. pre_out (bf16 [M, rope_cols], row stride ld_pre) receives the pre-norm columns (bias included) and rstd_out (fp32
+ * [M, rope_cols / 128], row stride ld_rstd) each head's rstd, when non-NULL. q_norm == NULL requires k_norm, pre_out and
+ * rstd_out NULL and computes exactly the norm-free projection. */
 int dalm_b200_gemm_bf16_rope(const void* A, long long lda, const void* B, long long ldb, void* out, long long ldo, int M, int N,
-                             int K, const float* bias, const float* cos_t, const float* sin_t, int L, int rope_cols, void* stream);
+                             int K, const float* bias, const float* cos_t, const float* sin_t, int L, int rope_cols,
+                             const float* q_norm, const float* k_norm, int nq_heads, float eps, void* pre_out, long long ld_pre,
+                             float* rstd_out, long long ld_rstd, void* stream);
 /* gemm_bf16_gelu: pre[M,N] = A B^T + bias (bf16) AND act[M,N] = gelu_erf(pre) (bf16) from one launch: BertIntermediate
  * (dense + GELU, HF modeling_bert) / Falcon's dense_h_to_4h + act; the backward multiplies by gelu'(pre) inside the next dgrad
  * GEMM (gemm_bf16 with act = 2 and resid = pre), so neither direction runs a separate activation kernel. */
@@ -243,6 +250,19 @@ int dalm_b200_decode_gemm(const void* A, long long lda, const void* W, long long
                           void* stream);
 int dalm_b200_rope_pos(void* buf, long long ld, int col0, int nheads, int D, const float* cos_t, const float* sin_t,
                        const int64_t* pos, int M, int T, void* stream);
+/* qk_norm_rope: Qwen3's per-head q/k RMSNorm followed by RoPE (head_dim 128, HF rotate_half), in place on heads [0, nheads) of
+ * a token-major bf16 buffer [M, ld] (heads [0, nq_heads) use q_norm, the rest k_norm; both fp32 [128]). Position of row m:
+ * clamp(pos[m], 0, T-1) when pos != NULL, else m % L; cos / sin fp32 [T, 64]. pre (bf16, ld_pre) and rstd (fp32 [M, nheads],
+ * ld_rstd) optionally receive the pre-norm values and each head's rstd. No allocation, no host synchronisation.
+ * qk_norm_rope_bwd: in place on d(out) of the same heads (positions m % L): un-rotates, then the RMSNorm backward from the
+ * saved pre / rstd, dx = rstd (w dy - x_hat mean(w dy x_hat)), x_hat = pre rstd; dw_q / dw_k (fp32 [128], both or neither)
+ * accumulate sum(dy x_hat) over rows and heads with atomics. */
+int dalm_b200_qk_norm_rope(void* buf, long long ld, int nheads, int nq_heads, const float* q_norm, const float* k_norm, float eps,
+                           const float* cos_t, const float* sin_t, int T, int L, const int64_t* pos, int M, void* pre,
+                           long long ld_pre, float* rstd, long long ld_rstd, void* stream);
+int dalm_b200_qk_norm_rope_bwd(void* dbuf, long long ld, int nheads, int nq_heads, const float* q_norm, const float* k_norm,
+                               const float* cos_t, const float* sin_t, int L, const void* pre, long long ld_pre, const float* rstd,
+                               long long ld_rstd, int M, float* dw_q, float* dw_k, void* stream);
 int dalm_b200_attention_decode(const void* qkv, long long ldq, int q_col, int k_col, int v_col, void* cache_k, void* cache_v,
                                long long cache_sb, long long cache_st, const int64_t* mask, long long ldm, void* out,
                                long long ldo, int B, int Hq, int Hkv, int D, int cur, const int* cur_dev, int T, float scale,

@@ -148,12 +148,15 @@ __device__ __forceinline__ uint4 philox4x32_7(uint2 key, uint4 c) {
 __device__ __forceinline__ unsigned long long drop_stream(const DropCfg& d) {
   return d.stream + (d.offset ? (*d.offset) * 0x9E3779B97F4A7C15ull : 0ull);
 }
-// One Philox call serves EIGHT consecutive elements (16 random bits each): scale[j] = 0 or 1/(1-p_eff) for elements
-// [8*idx8, 8*idx8 + 8) of the tensor the mask applies to.
+// One Philox call serves EIGHT consecutive elements (16 random bits each): word j holds the bits of elements 2j (low half)
+// and 2j + 1 (high half) of [8*idx8, 8*idx8 + 8).
+__device__ __forceinline__ uint4 drop_bits8(const DropCfg& d, unsigned long long stream, unsigned long long idx8) {
+  return philox4x32_7(make_uint2((unsigned int)d.seed, (unsigned int)(d.seed >> 32)),
+                      make_uint4((unsigned int)idx8, (unsigned int)(idx8 >> 32), (unsigned int)stream, (unsigned int)(stream >> 32)));
+}
+// scale[j] = 0 or 1/(1-p_eff) for elements [8*idx8, 8*idx8 + 8) of the tensor the mask applies to.
 __device__ __forceinline__ void drop_scale8(const DropCfg& d, unsigned long long stream, unsigned long long idx8, float* scale) {
-  const uint4 r = philox4x32_7(make_uint2((unsigned int)d.seed, (unsigned int)(d.seed >> 32)),
-                               make_uint4((unsigned int)idx8, (unsigned int)(idx8 >> 32), (unsigned int)stream,
-                                          (unsigned int)(stream >> 32)));
+  const uint4 r = drop_bits8(d, stream, idx8);
   const unsigned int w[4] = {r.x, r.y, r.z, r.w};
 #pragma unroll
   for (int j = 0; j < 4; ++j) {

@@ -71,346 +71,344 @@ __device__ __forceinline__ void tile_coords(int tile, int num_m, int num_n, int 
   n_blk = (band & 1) ? (num_n - 1 - n) : n;
 }
 
-// Epilogue math for one thread = one output row, 32 consecutive columns [col0, col0+32): alpha, bias, GELU, residual.
-template <bool PRE = false>
-__device__ __forceinline__ void epilogue_math(const GemmEpilogue& ep, const uint32_t* v, float* f, int row, int col0, bool row_ok,
-                                              const float4* rpre = nullptr) {
+// The epilogue runs on the accumulator registers, in the wgmma fragment layout. In a consumer warpgroup (64 rows of the tile),
+// thread (warp q, lane) holds acc[4 j + 2 h + e] = row 16 q + lane / 4 + 8 h, column 8 j + 2 (lane & 3) + e of the tile,
+// for j < BN / 8, h, e in {0, 1}. Each warpgroup drains its own 64 rows through a 128B-swizzled staging box and TMA stores:
+// 128 bytes of columns per store block (64 bf16 or 32 fp32). HBM sees full 128-byte lines, and the TMA unit clips ragged
+// M / N edges. Nothing goes through the stage ring, so the producer loads the next tile while this one is stored.
+constexpr int kBoxRows = 64;                                    // output tensor maps: [64 rows x 128 bytes] boxes
+constexpr int kBoxBytes = kBoxRows * 128;                       // one staging box
+constexpr int kStageTileBytes = 2 * kBoxBytes;                  // per consumer warpgroup: two boxes used in turn
+constexpr int kEpiGroups = 2;                                   // the two consumer warpgroups, each its own epilogue
+constexpr int kGemmThreads = 128 + kEpiGroups * 128;            // warpgroup 0: TMA producer ; warpgroups 1-2: wgmma + epilogue
+
+// A consumer warpgroup's staging: two boxes used in turn, so that the math of one store block overlaps the TMA unit reading
+// the previous one. begin() hands out the box once its last store has read it; end() stores it as a [64 rows x 128 B] box.
+struct EpiStage {
+  unsigned char* boxes;                                         // 1024-aligned, 2 x kBoxBytes
+  int bar;                                                      // named barrier of the warpgroup's 128 threads
+  bool issuer;                                                  // the warpgroup's first thread issues and waits for the stores
+  int buf;
+  __device__ __forceinline__ unsigned char* begin() {
+    if (issuer) bulk_wait_read<1>();                            // the store issued two blocks ago has finished reading this box
+    named_bar_sync(bar, 128);
+    return boxes + buf * kBoxBytes;
+  }
+  __device__ __forceinline__ void end(const CUtensorMap* tm, int col, int row, bool evict_first) {
+    fence_proxy_async();                                        // generic-proxy smem writes -> visible to the TMA unit
+    named_bar_sync(bar, 128);
+    if (issuer) {
+      const unsigned char* box = boxes + buf * kBoxBytes;
+      if (evict_first) tma_store_2d_hint(tm, box, col, row, l2_policy_evict_first());
+      else             tma_store_2d(tm, box, col, row);
+      bulk_commit();
+    }
+    buf ^= 1;
+  }
+};
+
+// Box row r, byte b of the row: 16-byte pieces XOR-swizzled by r % 8, the layout CU_TENSOR_MAP_SWIZZLE_128B expects. A warp's
+// 8 rows (r % 8 all different) x 4 lanes fill all 32 banks: conflict-free.
+__device__ __forceinline__ void box_st_bf16x2(unsigned char* box, int r, int b, float lo, float hi) {
+  *reinterpret_cast<__nv_bfloat162*>(box + r * 128 + ((((b >> 4) ^ (r & 7)) << 4) | (b & 15))) = __floats2bfloat162_rn(lo, hi);
+}
+__device__ __forceinline__ void box_st_f32x2(unsigned char* box, int r, int b, float lo, float hi) {
+  *reinterpret_cast<float2*>(box + r * 128 + ((((b >> 4) ^ (r & 7)) << 4) | (b & 15))) = make_float2(lo, hi);
+}
+
+// The plain epilogue on the 8 values a thread holds of fragment columns j0, j0 + 1: x[4 jj + 2 h + e] is row `row` + 8 h,
+// column `col` + 8 jj + e (col = 8 j0 + 2 (lane & 3) in output columns). Per element, in this order: alpha, + bias, act 1
+// (GELU), dropout, then the residual (act 2: the value rounded to bf16, times gelu'(resid)). resid_loaded: the caller adds
+// an fp32 residual it has already loaded, so it is not read here.
+__device__ __forceinline__ void epilogue_math(const GemmEpilogue& ep, float* x, int row, int col, bool ok0, bool ok1,
+                                              unsigned long long dstream, bool resid_loaded = false) {
   const int N = ep.N;
 #pragma unroll
-  for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(v[i]) * ep.alpha;
+  for (int i = 0; i < 8; ++i) x[i] *= ep.alpha;
   if (ep.bias) {
 #pragma unroll
-    for (int i = 0; i < 32; ++i) if (col0 + i < N) f[i] += __ldg(ep.bias + col0 + i);
+    for (int jj = 0; jj < 2; ++jj) {
+      if (col + 8 * jj < N) {                                   // N % 8 == 0: both columns of the pair are in or out
+        const float b0 = __ldg(ep.bias + col + 8 * jj), b1 = __ldg(ep.bias + col + 8 * jj + 1);
+        x[4 * jj + 0] += b0; x[4 * jj + 1] += b1; x[4 * jj + 2] += b0; x[4 * jj + 3] += b1;
+      }
+    }
   }
   if (ep.act == 1) {
 #pragma unroll
-    for (int i = 0; i < 32; ++i) f[i] = gelu_erf(f[i]);
+    for (int i = 0; i < 8; ++i) x[i] = gelu_erf(x[i]);
   }
   if (ep.drop.p > 0.f) {
-    const unsigned long long dstream = drop_stream(ep.drop);
-    const unsigned long long base = ((unsigned long long)row * (unsigned long long)N + (unsigned long long)col0) >> 3;
+    // The values lie in 4 groups of 8 columns, g = 2 jj + h, and every lane of the quad holds 2 columns of each: word k of
+    // the group's Philox output (k = lane & 3). Lane k draws group k, and the quad transposes the words with shuffles.
+    const int k = threadIdx.x & 3;
+    const unsigned long long idx8 = ((unsigned long long)(row + 8 * (k & 1)) * (unsigned long long)N +
+                                     (unsigned long long)(col - 2 * k + 8 * (k >> 1))) >> 3;
+    const uint4 r = drop_bits8(ep.drop, dstream, idx8);
+    unsigned int m0 = 0u, m1 = 0u, m2 = 0u, m3 = 0u;            // word k of groups 0..3 (scalars: no local-memory array)
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      // send word k ^ s of this lane's group (what lane k ^ s needs), receive word k of group k ^ s
+      const int t = k ^ s;
+      const unsigned int v = t == 0 ? r.x : t == 1 ? r.y : t == 2 ? r.z : r.w;
+      const unsigned int got = s ? __shfl_xor_sync(0xffffffffu, v, s) : v;
+      m0 = t == 0 ? got : m0; m1 = t == 1 ? got : m1; m2 = t == 2 ? got : m2; m3 = t == 3 ? got : m3;
+    }
+    const unsigned int m[4] = {m0, m1, m2, m3};
 #pragma unroll
     for (int g = 0; g < 4; ++g) {
-      float sc[8];
-      drop_scale8(ep.drop, dstream, base + g, sc);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) f[g * 8 + j] *= sc[j];
+      x[2 * g + 0] *= (m[g] & 0xFFFFu) >= ep.drop.thresh ? ep.drop.inv_keep : 0.f;
+      x[2 * g + 1] *= (m[g] >> 16) >= ep.drop.thresh ? ep.drop.inv_keep : 0.f;
     }
   }
-  if constexpr (PRE) {                                          // fp32 residual already in registers (prefetched a block ahead)
-#pragma unroll
-    for (int g = 0; g < 8; ++g) { f[g * 4 + 0] += rpre[g].x; f[g * 4 + 1] += rpre[g].y; f[g * 4 + 2] += rpre[g].z; f[g * 4 + 3] += rpre[g].w; }
-  } else if (ep.resid && row_ok) {
-    if (ep.resid_f32) {
-      const float* r = reinterpret_cast<const float*>(ep.resid) + (size_t)row * ep.ldr + col0;
-#pragma unroll
-      for (int g = 0; g < 8; ++g) {
-        if (col0 + g * 4 < N) {
-          const float4 t = *reinterpret_cast<const float4*>(r + g * 4);
-          f[g * 4 + 0] += t.x; f[g * 4 + 1] += t.y; f[g * 4 + 2] += t.z; f[g * 4 + 3] += t.w;
-        }
-      }
-    } else {
-      const __nv_bfloat16* r = reinterpret_cast<const __nv_bfloat16*>(ep.resid) + (size_t)row * ep.ldr + col0;
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        if (col0 + g * 8 < N) {
-          const bf16x8 t = *reinterpret_cast<const bf16x8*>(r + g * 8);
-          float tf[8];
-          unpack8(t, tf);
-          if (ep.act == 2) {     // same roundings as the un-fused pair (bf16 dgrad output, then gelu_bwd_kernel): bit-identical results
-#pragma unroll
-            for (int i = 0; i < 8; ++i) f[g * 8 + i] = __bfloat162float(__float2bfloat16_rn(f[g * 8 + i])) * gelu_erf_grad(tf[i]);
-          } else {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) f[g * 8 + i] += tf[i];
-          }
-        }
-      }
-    }
-  }
-}
-
-// Accumulator row access for the epilogue: 32 consecutive fp32 columns of this thread's row of the tile.
-__device__ __forceinline__ void acc_ld32(const float* p, uint32_t* v) {
-#pragma unroll
-  for (int g = 0; g < 8; ++g) {
-    const float4 t = *reinterpret_cast<const float4*>(p + g * 4);
-    v[g * 4 + 0] = __float_as_uint(t.x); v[g * 4 + 1] = __float_as_uint(t.y);
-    v[g * 4 + 2] = __float_as_uint(t.z); v[g * 4 + 3] = __float_as_uint(t.w);
-  }
-}
-
-// Drains one 128 x BN fp32 accumulator parked in shared memory (this thread: row row_in_tile) to HBM through a 128B-swizzled staging tile
-// and TMA stores: the 128 epilogue threads write their rows into shared memory (16-byte pieces XOR-swizzled by row % 8:
-// conflict-free per quarter warp, and exactly the layout CU_TENSOR_MAP_SWIZZLE_128B expects), one thread issues
-// cp.async.bulk.tensor stores of [128 rows x 128 bytes] boxes. HBM sees full 128-byte lines; ragged M / N edges are
-// clipped by the TMA unit. Two groups of four epilogue warps (each group covers all 128 rows) take alternate
-// store blocks, each with its own staging tile, so one group's TMA store overlaps the other's accumulator reads and math.
-constexpr int kStageTileBytes = 128 * 128;
-constexpr int kEpiGroups = 2;                                   // two groups of 4 epilogue warps split a tile's store blocks
-constexpr int kGemmThreads = 128 + kEpiGroups * 128;            // warpgroup 0: TMA producer ; warpgroups 1-2: wgmma + epilogue
-template <int BN, Epi EPI>
-__device__ __forceinline__ void epilogue_drain_tile(const GemmEpilogue& ep, const CUtensorMap* tmap_out, const CUtensorMap* tmap_out2,
-                                                    unsigned char* staging, int grp, const float* arow, int row_in_tile, int tile_row0,
-                                                    int tile_col0) {
-  static_assert(BN == 256 || EPI == Epi::Plain || EPI == Epi::GeluPair, "the SwiGLU and RoPE epilogues need 256-wide tiles");
-  const int N = ep.N;
-  const int row = tile_row0 + row_in_tile;
-  const bool row_ok = row < ep.M;
-  constexpr bool F32_OUT = EPI == Epi::Plain;                   // the fused epilogues write bf16 only
-  const int sb_cols = (F32_OUT && ep.out_f32) ? 32 : 64;       // 128 bytes of output per row per store block
-  const bool issuer = (threadIdx.x == 128 + grp * 128);        // first thread of this epilogue group
-  unsigned char* tile = staging + grp * kStageTileBytes;       // one staging tile per group
-  unsigned char* st = tile + row_in_tile * 128;
-  const int sw = row_in_tile & 7;
-  // fp32 residual (o_proj / down-projection: x_out = x + y): this thread's 128 bytes of the NEXT store block are fetched
-  // as soon as the current block's math has consumed its own, so the HBM latency of the residual no longer sits in the
-  // block's serial chain (accumulator ld -> residual ld -> math -> st.shared -> TMA store)
-  const bool rpf = F32_OUT && ep.out_f32 && ep.resid != nullptr && ep.resid_f32;
-  float4 rnext[8];
-  auto fetch_resid = [&](int cc) {
-    const int cg0 = tile_col0 + cc;
-    const float* r = reinterpret_cast<const float*>(ep.resid) + (size_t)row * ep.ldr + cg0;
-#pragma unroll
-    for (int g = 0; g < 8; ++g)
-      rnext[g] = (row_ok && cc < BN && cg0 + g * 4 < N) ? *reinterpret_cast<const float4*>(r + g * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
-  };
-  if (rpf) fetch_resid(grp * sb_cols);
-#pragma unroll 1
-  for (int c = grp * sb_cols; c < BN; c += kEpiGroups * sb_cols) {   // the two groups interleave store blocks
-    const int col0 = tile_col0 + c;
-    if (col0 >= N) break;                                       // uniform across the group's 4 warps
-    if (issuer) bulk_wait_read<0>();                            // the previous store has finished reading the staging tile
-    named_bar_sync(1 + grp, 128);
-    if (F32_OUT && ep.out_f32) {
-      uint32_t v[32]; float f[32];
-      acc_ld32(arow + c, v);
-      if (rpf) {                                                // one block of residual in registers at a time
-        epilogue_math<true>(ep, v, f, row, col0, row_ok, rnext);
-        fetch_resid(c + kEpiGroups * sb_cols);
-      } else {
-        epilogue_math<false>(ep, v, f, row, col0, row_ok);
-      }
-#pragma unroll
-      for (int g = 0; g < 8; ++g)
-        *reinterpret_cast<float4*>(st + ((g ^ sw) << 4)) = make_float4(f[g * 4], f[g * 4 + 1], f[g * 4 + 2], f[g * 4 + 3]);
-    } else if (EPI == Epi::RoPE && col0 < ep.rope_cols) {
-      // RoPE in the QKV epilogue: this 64-column block is one rotate_half HALF of a head (x1 = columns 0..63, x2 = 64..127 of the
-      // head; tiles are 256 columns = two whole heads); its partner half sits 64 columns away in the same accumulator.
-      //   x1' = x1 cos - x2 sin ,  x2' = x2 cos + x1 sin        (cos / sin of the row's position, element j = column % 64)
-      // Replaces a separate in-place pass over the q|k columns of every layer's QKV output. A q/k/v bias (Qwen2) is added to both
-      // halves in fp32 before the rotation, so the only rounding is the final bf16 store.
-      const bool second = ((col0 >> 6) & 1) != 0;               // this block holds x2
-      const int cp = second ? c - 64 : c + 64;
-      const int colp = tile_col0 + cp;
-      const int pos = row_ok ? (row % ep.rope_L) : 0;
-      const float* cs = ep.rope_cos + (size_t)pos * 64;
-      const float* sn = ep.rope_sin + (size_t)pos * 64;
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        uint32_t vo[32], vq[32]; float f[32];
-        acc_ld32(arow + (c + h * 32), vo);
-        acc_ld32(arow + (cp + h * 32), vq);
-        float cc[32], ss[32];
-#pragma unroll
-        for (int i = 0; i < 32; i += 4) {
-          *reinterpret_cast<float4*>(cc + i) = __ldg(reinterpret_cast<const float4*>(cs + h * 32 + i));
-          *reinterpret_cast<float4*>(ss + i) = __ldg(reinterpret_cast<const float4*>(sn + h * 32 + i));
-        }
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          float own = __uint_as_float(vo[i]), oth = __uint_as_float(vq[i]);
-          if (ep.bias) {
-            own += __ldg(ep.bias + col0 + h * 32 + i);
-            oth += __ldg(ep.bias + colp + h * 32 + i);
-          }
-          f[i] = second ? fmaf(own, cc[i], oth * ss[i]) : fmaf(own, cc[i], -oth * ss[i]);
-        }
-#pragma unroll
-        for (int g = 0; g < 4; ++g)
-          *reinterpret_cast<bf16x8*>(st + (((h * 4 + g) ^ sw) << 4)) = pack8(f + g * 8);
-      }
-    } else if (EPI == Epi::NormRoPE && col0 < ep.rope_cols) {
-      // per-head RMSNorm, then RoPE (Qwen3: q_norm / k_norm over each head's 128 columns, weight [128]). The thread's row of the
-      // head is in this tile's accumulator (both 64-column halves), so the sum of squares needs no exchange between threads.
-      // Both halves sum the head in column order (x1 then x2), so the two groups that store them use the same rstd.
-      // Order, all fp32 before the single bf16 store: + bias, x * rsqrt(mean(x^2) + eps) * w, rotate_half.
-      const bool second = ((col0 >> 6) & 1) != 0;
-      const int cp = second ? c - 64 : c + 64;
-      const int colp = tile_col0 + cp;
-      const int c1 = second ? cp : c;                           // the head's first half, in tile columns
-      const int head = col0 >> 7;
-      const float* nw = head < ep.nq_heads ? ep.q_norm : ep.k_norm;
-      const int jo = second ? 64 : 0, jp = 64 - jo;             // in-head offsets of this block and of its partner
-      float ss = 0.f;
-#pragma unroll 1
-      for (int h = 0; h < 4; ++h) {
-        uint32_t v[32];
-        acc_ld32(arow + (c1 + h * 32), v);
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          float x = __uint_as_float(v[i]);
-          if (ep.bias) x += __ldg(ep.bias + tile_col0 + c1 + h * 32 + i);
-          ss = fmaf(x, x, ss);
-        }
-      }
-      const float rstd = rsqrtf(ss * (1.f / 128.f) + ep.norm_eps);
-      if (ep.norm_rstd && row_ok && !second) ep.norm_rstd[(size_t)row * ep.ld_rstd + head] = rstd;
-      const int pos = row_ok ? (row % ep.rope_L) : 0;
-      const float* cs = ep.rope_cos + (size_t)pos * 64;
-      const float* sn = ep.rope_sin + (size_t)pos * 64;
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        uint32_t vo[32], vq[32]; float f[32];
-        acc_ld32(arow + (c + h * 32), vo);
-        acc_ld32(arow + (cp + h * 32), vq);
-        float cc[32], ss2[32];
-#pragma unroll
-        for (int i = 0; i < 32; i += 4) {
-          *reinterpret_cast<float4*>(cc + i) = __ldg(reinterpret_cast<const float4*>(cs + h * 32 + i));
-          *reinterpret_cast<float4*>(ss2 + i) = __ldg(reinterpret_cast<const float4*>(sn + h * 32 + i));
-        }
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          float own = __uint_as_float(vo[i]), oth = __uint_as_float(vq[i]);
-          if (ep.bias) {
-            own += __ldg(ep.bias + col0 + h * 32 + i);
-            oth += __ldg(ep.bias + colp + h * 32 + i);
-          }
-          own = own * rstd * __ldg(nw + jo + h * 32 + i);
-          oth = oth * rstd * __ldg(nw + jp + h * 32 + i);
-          f[i] = second ? fmaf(own, cc[i], oth * ss2[i]) : fmaf(own, cc[i], -oth * ss2[i]);
-        }
-#pragma unroll
-        for (int g = 0; g < 4; ++g)
-          *reinterpret_cast<bf16x8*>(st + (((h * 4 + g) ^ sw) << 4)) = pack8(f + g * 8);
-      }
-      fence_proxy_async();
-      named_bar_sync(1 + grp, 128);
-      if (issuer) {
-        if (ep.l2_hints & 4) tma_store_2d_hint(tmap_out, tile, col0, tile_row0, l2_policy_evict_first());
-        else                 tma_store_2d(tmap_out, tile, col0, tile_row0);
-        bulk_commit();
-      }
-      if (!ep.norm_pre) continue;
-      // the pre-norm block (+ bias, rounded once to bf16) through the same staging tile, once the TMA unit has read it
-      if (issuer) bulk_wait_read<0>();
-      named_bar_sync(1 + grp, 128);
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        uint32_t v[32]; float f[32];
-        acc_ld32(arow + (c + h * 32), v);
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          f[i] = __uint_as_float(v[i]);
-          if (ep.bias) f[i] += __ldg(ep.bias + col0 + h * 32 + i);
-        }
-#pragma unroll
-        for (int g = 0; g < 4; ++g)
-          *reinterpret_cast<bf16x8*>(st + (((h * 4 + g) ^ sw) << 4)) = pack8(f + g * 8);
-      }
-      fence_proxy_async();
-      named_bar_sync(1 + grp, 128);
-      if (issuer) {
-        tma_store_2d(tmap_out2, tile, col0, tile_row0);
-        bulk_commit();
-      }
-      continue;
-    } else if (EPI == Epi::GeluPair) {
-      // GELU forward, both tensors: the 64-column block goes out twice through the same staging tile - first the bf16
-      // pre-activation, then gelu() of those ROUNDED values (exactly what gelu_fwd_kernel would read back from HBM).
-      bf16x8 pk[8];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        if (col0 + h * 32 < N) {
-          uint32_t v[32]; float f[32];
-          acc_ld32(arow + (c + h * 32), v);
-          epilogue_math(ep, v, f, row, col0 + h * 32, row_ok);
-#pragma unroll
-          for (int g = 0; g < 4; ++g) pk[h * 4 + g] = pack8(f + g * 8);
-        } else {
-#pragma unroll
-          for (int g = 0; g < 4; ++g) pk[h * 4 + g] = bf16x8{};
-        }
-      }
-#pragma unroll
-      for (int g = 0; g < 8; ++g) *reinterpret_cast<bf16x8*>(st + ((g ^ sw) << 4)) = pk[g];
-      fence_proxy_async();
-      named_bar_sync(1 + grp, 128);
-      if (issuer) {
-        if (ep.l2_hints & 4) tma_store_2d_hint(tmap_out, tile, col0, tile_row0, l2_policy_evict_first());
-        else                 tma_store_2d(tmap_out, tile, col0, tile_row0);
-        bulk_commit();
-      }
-#pragma unroll
-      for (int g = 0; g < 8; ++g) {                             // overlaps the TMA unit reading the staging tile
-        float x[8];
-        unpack8(pk[g], x);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) x[i] = gelu_erf(x[i]);
-        pk[g] = pack8(x);
-      }
-      if (issuer) bulk_wait_read<0>();
-      named_bar_sync(1 + grp, 128);
-#pragma unroll
-      for (int g = 0; g < 8; ++g) *reinterpret_cast<bf16x8*>(st + ((g ^ sw) << 4)) = pk[g];
-      fence_proxy_async();
-      named_bar_sync(1 + grp, 128);
-      if (issuer) {
-        tma_store_2d(tmap_out2, tile, col0, tile_row0);
-        bulk_commit();
-      }
-      continue;
-    } else {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        if (col0 + h * 32 < N) {
-          uint32_t v[32]; float f[32];
-          acc_ld32(arow + (c + h * 32), v);
-          epilogue_math(ep, v, f, row, col0 + h * 32, row_ok);
-#pragma unroll
-          for (int g = 0; g < 4; ++g)
-            *reinterpret_cast<bf16x8*>(st + (((h * 4 + g) ^ sw) << 4)) = pack8(f + g * 8);
-        }
-      }
-    }
-    fence_proxy_async();                                        // generic-proxy smem writes -> visible to the TMA unit
-    named_bar_sync(1 + grp, 128);
-    if (issuer) {
-      if (ep.l2_hints & 4) tma_store_2d_hint(tmap_out, tile, col0, tile_row0, l2_policy_evict_first());
-      else                 tma_store_2d(tmap_out, tile, col0, tile_row0);
-      bulk_commit();
-    }
-  }
-  if constexpr (EPI == Epi::SwiGLU) {
-    // SwiGLU forward: act[:, 128 n_blk + 64 j + ...] = silu(gate) * up from the fp32 accumulators (gate columns 64j.., up columns
-    // 128 + 64j..): two more 128-byte-wide store blocks per tile, one per epilogue group. Replaces a separate pass that re-read
-    // the 203 MB gate|up buffer.
-    const int j = grp;
-    const int acol0 = (tile_col0 >> 1) + j * 64;                // column of the [M, N/2] activation matrix
-    if (issuer) bulk_wait_read<0>();
-    named_bar_sync(1 + grp, 128);
+  if (ep.resid && !resid_loaded) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      uint32_t vg[32], vu[32]; float f[32];
-      acc_ld32(arow + (j * 64 + h * 32), vg);
-      acc_ld32(arow + (128 + j * 64 + h * 32), vu);
+      if (!(h ? ok1 : ok0)) continue;
+      const size_t roff = (size_t)(row + 8 * h) * ep.ldr;
 #pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        const float g = __uint_as_float(vg[i]);
-        f[i] = g / (1.f + __expf(-g)) * __uint_as_float(vu[i]);
+      for (int jj = 0; jj < 2; ++jj) {
+        const int c = col + 8 * jj;
+        if (c >= N) continue;
+        float* v = x + 4 * jj + 2 * h;
+        if (ep.resid_f32) {
+          const float2 t = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(ep.resid) + roff + c);
+          v[0] += t.x; v[1] += t.y;
+        } else {
+          const float2 t = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(reinterpret_cast<const __nv_bfloat16*>(ep.resid) + roff + c));
+          if (ep.act == 2) {     // same roundings as the un-fused pair (bf16 dgrad output, then gelu_bwd_kernel): bit-identical results
+            v[0] = __bfloat162float(__float2bfloat16_rn(v[0])) * gelu_erf_grad(t.x);
+            v[1] = __bfloat162float(__float2bfloat16_rn(v[1])) * gelu_erf_grad(t.y);
+          } else {
+            v[0] += t.x; v[1] += t.y;
+          }
+        }
       }
+    }
+  }
+}
+
+// Drains this warpgroup's 64 x BN accumulator (rows row0 .., tile columns tile_col0 ..) to HBM; see above for the layout.
+// The plain store blocks run as a loop that is not unrolled: each iteration reads the 8 fragment columns at the front of acc
+// (static indices, so acc stays in registers) and then shifts the rest down, which consumes acc. Unrolled, the epilogue is
+// straight-line code several times the size of the instruction cache, and its GELU and dropout variants ran slower than
+// the loop over an accumulator parked in shared memory that they replace.
+template <int BN, Epi EPI>
+__device__ __forceinline__ void epilogue_tile(const GemmEpilogue& ep, const CUtensorMap* tmap_out, const CUtensorMap* tmap_out2,
+                                              EpiStage& sg, float (&acc)[BN / 2], int row0, int tile_col0) {
+  static_assert(BN == 256 || EPI == Epi::Plain || EPI == Epi::GeluPair, "the SwiGLU and RoPE epilogues need 256-wide tiles");
+  const int N = ep.N;
+  const int lane = threadIdx.x & 31, k = lane & 3;
+  const int rb = 16 * ((threadIdx.x >> 5) & 3) + (lane >> 2);  // box row of the thread's first row; the second is rb + 8
+  const int row = row0 + rb;
+  const bool ok0 = row < ep.M, ok1 = row + 8 < ep.M;
+  const int cq = tile_col0 + 2 * k;                             // output column of x[0] of fragment column 0
+  const bool hint = (ep.l2_hints & 4) != 0;
+  const unsigned long long dstream = ep.drop.p > 0.f ? drop_stream(ep.drop) : 0ull;
+  auto frag8 = [&](float* x, int j0) {                          // fragment columns j0, j0 + 1 (j0 a constant once unrolled)
 #pragma unroll
-      for (int g4 = 0; g4 < 4; ++g4) *reinterpret_cast<bf16x8*>(st + (((h * 4 + g4) ^ sw) << 4)) = pack8(f + g4 * 8);
+    for (int i = 0; i < 8; ++i) x[i] = acc[4 * j0 + i];
+  };
+  auto shift8 = [&]() {                                         // fragment columns 8.. to the front
+#pragma unroll
+    for (int i = 0; i + 32 < BN / 2; ++i) acc[i] = acc[i + 32];
+  };
+
+  if (EPI == Epi::Plain && ep.out_f32) {
+    // fp32 out: 32 columns = fragment columns 4 b .. 4 b + 3 of the front per store block, two blocks per iteration. An
+    // fp32 residual (o_proj / down-projection: x_out = x + y) is fetched one block ahead, so its HBM latency is not in the
+    // block's serial chain.
+    const bool rpf = ep.resid != nullptr && ep.resid_f32;
+    float2 rn[8];                                               // [4 u + 2 jj + h]: the next block's residual
+    auto fetch_resid = [&](int c) {
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const int h = i & 1, cc = cq + c + 8 * (i >> 1);
+        rn[i] = ((h ? ok1 : ok0) && c < BN && cc < N)
+                    ? *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(ep.resid) + (size_t)(row + 8 * h) * ep.ldr + cc)
+                    : make_float2(0.f, 0.f);
+      }
+    };
+    if (rpf) fetch_resid(0);
+#pragma unroll 1
+    for (int c = 0; c < BN && tile_col0 + c < N; c += 64) {    // uniform across the warpgroup
+#pragma unroll
+      for (int b = 0; b < 2; ++b) {
+        const int cb = c + 32 * b;
+        if (tile_col0 + cb >= N) break;
+        unsigned char* box = sg.begin();
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          float x[8];
+          frag8(x, 4 * b + 2 * u);
+          epilogue_math(ep, x, row, cq + cb + 16 * u, ok0, ok1, dstream, rpf);
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {                       // the residual, last (zero where out of bounds)
+            if (rpf) { x[2 * i] += rn[4 * u + i].x; x[2 * i + 1] += rn[4 * u + i].y; }
+          }
+#pragma unroll
+          for (int i = 0; i < 4; ++i) box_st_f32x2(box, rb + 8 * (i & 1), 64 * u + 32 * (i >> 1) + 8 * k, x[2 * i], x[2 * i + 1]);
+        }
+        if (rpf) fetch_resid(cb + 32);
+        sg.end(tmap_out, tile_col0 + cb, row0, hint);
+      }
+      shift8();
     }
-    fence_proxy_async();
-    named_bar_sync(1 + grp, 128);
-    if (issuer) {
-      if (ep.l2_hints & 4) tma_store_2d_hint(tmap_out2, tile, acol0, tile_row0, l2_policy_evict_first());
-      else                 tma_store_2d(tmap_out2, tile, acol0, tile_row0);
-      bulk_commit();
+    return;
+  }
+
+  if constexpr (EPI == Epi::SwiGLU) {
+    // SwiGLU forward: act[:, 128 n_blk + 64 b + ...] = silu(gate) * up from the fp32 accumulators (gate columns 64 b.., up
+    // columns 128 + 64 b..: fragment columns j and j + 16 of the same thread), two more store blocks per tile. Replaces a
+    // separate pass that re-read the 203 MB gate|up buffer. First, while acc is whole.
+#pragma unroll
+    for (int b = 0; b < 2; ++b) {
+      unsigned char* box = sg.begin();
+#pragma unroll
+      for (int jl = 0; jl < 8; ++jl) {
+        const int j = 8 * b + jl;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float f[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const float g = acc[4 * j + 2 * h + e];
+            f[e] = g / (1.f + __expf(-g)) * acc[4 * (j + 16) + 2 * h + e];
+          }
+          box_st_bf16x2(box, rb + 8 * h, 16 * jl + 4 * k, f[0], f[1]);
+        }
+      }
+      sg.end(tmap_out2, (tile_col0 >> 1) + 64 * b, row0, hint);
     }
+  }
+  // bf16 out: 64 columns = fragment columns 8 b .. 8 b + 7 per store block
+  const bool rope_tile = (EPI == Epi::RoPE || EPI == Epi::NormRoPE) && tile_col0 < ep.rope_cols;   // rope_cols % 256 == 0
+  float rstd[2][2];                                             // NormRoPE: [head of the tile][h]
+  const float* nwt[2];
+  if (EPI == Epi::NormRoPE && rope_tile) {
+    // per-head RMSNorm (Qwen3 q_norm / k_norm over each head's 128 columns, weight [128]): a thread holds 32 of a head's
+    // columns in each of its two rows; the quad's partial sums of squares are combined with a butterfly, so all 4 lanes
+    // (and both halves of the head) use the same rstd.
+#pragma unroll
+    for (int hd = 0; hd < 2; ++hd) {
+      const int head = (tile_col0 >> 7) + hd;
+      nwt[hd] = head < ep.nq_heads ? ep.q_norm : ep.k_norm;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float ss = 0.f;
+#pragma unroll
+        for (int jl = 0; jl < 16; ++jl) {
+          const int j = 16 * hd + jl;
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            float x = acc[4 * j + 2 * h + e];
+            if (ep.bias) x += __ldg(ep.bias + cq + 8 * j + e);
+            ss = fmaf(x, x, ss);
+          }
+        }
+        ss += __shfl_xor_sync(0xffffffffu, ss, 1);
+        ss += __shfl_xor_sync(0xffffffffu, ss, 2);
+        rstd[hd][h] = rsqrtf(ss * (1.f / 128.f) + ep.norm_eps);
+        if (ep.norm_rstd && (h ? ok1 : ok0) && k == 0) ep.norm_rstd[(size_t)(row + 8 * h) * ep.ld_rstd + head] = rstd[hd][h];
+      }
+    }
+  }
+  if ((EPI == Epi::RoPE || EPI == Epi::NormRoPE) && rope_tile) {
+#pragma unroll
+    for (int c = 0; c < BN; c += 64) {                         // rope tiles lie inside N
+      const int col0 = tile_col0 + c;
+      const int jb = c / 8;
+      // RoPE in the QKV epilogue (head_dim 128, HF rotate_half): this 64-column block is one half of a head (x1 = columns
+      // 0..63, x2 = 64..127; tiles are 256 columns = two whole heads). Its partner half is fragment column j -+ 8, in the
+      // same thread.    x1' = x1 cos - x2 sin ,  x2' = x2 cos + x1 sin    (cos / sin of the row's position, index column % 64)
+      // A q/k/v bias (Qwen2) is added to both halves in fp32 before the rotation; NormRoPE (Qwen3) then applies
+      // x * rstd * w. The only rounding is the final bf16 store.
+      const bool second = ((c >> 6) & 1) != 0;
+      const int jp = second ? -8 : 8;
+      const int hd = c >> 7;
+      const int io = (c & 64) + 2 * k, ip = ((c & 64) ^ 64) + 2 * k;   // in-head index of the own / partner value of jl = 0
+      unsigned char* box = sg.begin();
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int pos = (h ? ok1 : ok0) ? (row + 8 * h) % ep.rope_L : 0;
+        const float* cs = ep.rope_cos + (size_t)pos * 64 + 2 * k;
+        const float* sn = ep.rope_sin + (size_t)pos * 64 + 2 * k;
+#pragma unroll
+        for (int jl = 0; jl < 8; ++jl) {
+          const int j = jb + jl;
+          const float2 cc = __ldg(reinterpret_cast<const float2*>(cs + 8 * jl));
+          const float2 s2 = __ldg(reinterpret_cast<const float2*>(sn + 8 * jl));
+          float f[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            float own = acc[4 * j + 2 * h + e], oth = acc[4 * (j + jp) + 2 * h + e];
+            if (ep.bias) {
+              own += __ldg(ep.bias + cq + 8 * j + e);
+              oth += __ldg(ep.bias + cq + 8 * (j + jp) + e);
+            }
+            if constexpr (EPI == Epi::NormRoPE) {
+              own = own * rstd[hd][h] * __ldg(nwt[hd] + io + 8 * jl + e);
+              oth = oth * rstd[hd][h] * __ldg(nwt[hd] + ip + 8 * jl + e);
+            }
+            const float cv = e ? cc.y : cc.x, sv = e ? s2.y : s2.x;
+            f[e] = second ? fmaf(own, cv, oth * sv) : fmaf(own, cv, -oth * sv);
+          }
+          box_st_bf16x2(box, rb + 8 * h, 16 * jl + 4 * k, f[0], f[1]);
+        }
+      }
+      sg.end(tmap_out, col0, row0, hint);
+      if (EPI == Epi::NormRoPE && ep.norm_pre) {
+        // the pre-norm block (+ bias, rounded once to bf16) for the backward
+        box = sg.begin();
+#pragma unroll
+        for (int jl = 0; jl < 8; ++jl) {
+          const int j = jb + jl;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float f[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              f[e] = acc[4 * j + 2 * h + e];
+              if (ep.bias) f[e] += __ldg(ep.bias + cq + 8 * j + e);
+            }
+            box_st_bf16x2(box, rb + 8 * h, 16 * jl + 4 * k, f[0], f[1]);
+          }
+        }
+        sg.end(tmap_out2, col0, row0, false);
+      }
+    }
+    return;
+  }
+  // plain math, bf16 out: fragment columns 0..7 of the front per store block; GeluPair also writes gelu() of the ROUNDED
+  // values (exactly what gelu_fwd_kernel would read back from HBM) to tmap_out2
+#pragma unroll 1
+  for (int c = 0; c < BN && tile_col0 + c < N; c += 64) {      // uniform across the warpgroup
+    const int col0 = tile_col0 + c;
+    __nv_bfloat162 pk[16];                                      // [4 u + 2 jj + h]
+    unsigned char* box = sg.begin();
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      float x[8];
+      frag8(x, 2 * u);
+      epilogue_math(ep, x, row, cq + c + 16 * u, ok0, ok1, dstream);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        pk[4 * u + i] = __floats2bfloat162_rn(x[2 * i], x[2 * i + 1]);
+        *reinterpret_cast<__nv_bfloat162*>(box + (rb + 8 * (i & 1)) * 128 +
+                                           ((((2 * u + (i >> 1)) ^ (rb & 7)) << 4) | (4 * k))) = pk[4 * u + i];
+      }
+    }
+    sg.end(tmap_out, col0, row0, hint);
+    if constexpr (EPI == Epi::GeluPair) {
+      box = sg.begin();
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        const float2 p = __bfloat1622float2(pk[i]);
+        box_st_bf16x2(box, rb + 8 * (i & 1), 16 * (i >> 1) + 4 * k, gelu_erf(p.x), gelu_erf(p.y));
+      }
+      sg.end(tmap_out2, col0, row0, false);
+    }
+    shift8();
   }
 }
 
@@ -420,9 +418,7 @@ template <int BN> struct GemmCfg {
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STAGES = (BN == 256) ? 4 : (BN == 128 ? 6 : 8);
-  static constexpr int ACC_LD = BN + 4;                            // fp32 row stride of the accumulator tile in shared memory
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 2 * kStageTileBytes + 1024 /*alignment slack*/ + 256 /*barriers*/;
-  static_assert(BM * ACC_LD * 4 <= STAGES * STAGE_BYTES, "the accumulator tile reuses the stage ring");
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + kEpiGroups * kStageTileBytes + 1024 /*alignment slack*/ + 256 /*barriers*/;
   static_assert(SMEM_BYTES <= 232448, "exceeds 227 KB of shared memory per block");
 };
 
@@ -444,9 +440,10 @@ __device__ __forceinline__ void wgmma_tile(float* d, uint64_t da, uint64_t db, i
 // Structure (persistent CTAs, 384 threads = three warpgroups):
 //   warpgroup 0 : TMA producer (one thread) - 128B-swizzled tiles into a STAGES-deep shared-memory ring
 //   warpgroups 1, 2 : consumers - each issues m64 x BN x 16 wgmma for its 64 rows of the 128-row tile, accumulators in
-//                 registers; after the k loop they park the fp32 tile in the (then idle) stage ring and act as the two
-//                 epilogue groups of epilogue_drain_tile (each thread = one row, the groups alternate 128-byte store blocks).
-// The producer starts the next tile's loads once both epilogue groups have left the parked accumulator.
+//                 registers; after the k loop each runs epilogue_tile on its own accumulator registers and stores its
+//                 64 rows through its own staging boxes.
+// The consumers release a stage as soon as the wgmmas reading it have retired, at the end of a tile as inside it, and the
+// producer refills it at once: while the consumers run a tile's epilogue, the next tile's first STAGES k-blocks load.
 // CL = 2: a cluster of two CTAs computes a 256 x BN tile (128 rows each); each CTA loads half of the shared B tile and
 // multicasts it to both, so every B panel is read from L2 once per two CTAs (block_n 2128 / 2256).
 template <int BN, int LAYOUT, Epi EPI, int CL>
@@ -459,11 +456,9 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
   extern __shared__ unsigned char smem_raw[];
   // 128B swizzle atoms need 1024-byte aligned tile bases
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  unsigned char* staging = smem + STAGES * Cfg::STAGE_BYTES;             // 2 x [128 rows x 128 B], 1024-aligned
-  uint64_t* full_bar  = reinterpret_cast<uint64_t*>(staging + 2 * kStageTileBytes);
+  unsigned char* staging = smem + STAGES * Cfg::STAGE_BYTES;             // per consumer warpgroup 2 x [64 rows x 128 B], 1024-aligned
+  uint64_t* full_bar  = reinterpret_cast<uint64_t*>(staging + kEpiGroups * kStageTileBytes);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* epi_bar   = empty_bar + STAGES;                              // the epilogue has left the parked accumulator
-  float* acc_smem = reinterpret_cast<float*>(smem);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t rank = CL == 2 ? cluster_ctarank() : 0u;
@@ -483,7 +478,6 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
   if (threadIdx.x == 32) {
     // consumer releases: one arrive per consumer warp, of every CTA whose producer writes into this stage
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8 * CL); }
-    mbar_init(epi_bar, 8 * CL);
     fence_mbar_init();
   }
   if constexpr (CL == 2) cluster_sync_all();
@@ -501,11 +495,9 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
         if (hinted) tma_load_2d_hint(dst, tm, bar, c0, c1, pol);
         else        tma_load_2d(dst, tm, bar, c0, c1);
       };
-      int it = 0;
-      for (int tile = unit; tile < num_tiles; tile += num_units, ++it) {
+      for (int tile = unit; tile < num_tiles; tile += num_units) {
         int m_blk, n_blk;
         tile_coords(tile, num_m, num_n, group_m, m_blk, n_blk);
-        if (it > 0) mbar_wait(epi_bar, (uint32_t)(it - 1) & 1u);        // the stage ring holds the previous accumulator
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           unsigned char* sa = smem + stage * Cfg::STAGE_BYTES;
@@ -536,7 +528,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
     // =============================== consumers: wgmma, then epilogue ===============================
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
     const int grp = (warp - 4) >> 2;                            // warpgroup 0 / 1 = rows [64 grp, 64 grp + 64) of the tile
-    const int q = warp & 3;
+    EpiStage sg{staging + grp * kStageTileBytes, 1 + grp, (threadIdx.x & 127) == 0, 0};
     constexpr int TA = LAYOUT == 2 ? 1 : 0, TB = LAYOUT >= 1 ? 1 : 0;
     // k-step (16 elements of K) in 16-byte units of the descriptor start address: K-major +32 B inside the swizzle atom,
     // MN-major +16 rows * 128 B
@@ -573,31 +565,9 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
         mbar_arrive(&empty_bar[prev]);
         if constexpr (CL == 2) mbar_arrive_remote(&empty_bar[prev], rank ^ 1u);
       }
-      // park the accumulator in the stage ring: every stage has landed and no wgmma of either warpgroup still reads it
-      named_bar_sync(3, 256);
-      {
-        const int r0 = grp * 64 + q * 16 + (lane >> 2);
-        float* p0 = acc_smem + (size_t)r0 * Cfg::ACC_LD + 2 * (lane & 3);
-        float* p1 = p0 + 8 * Cfg::ACC_LD;
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          *reinterpret_cast<float2*>(p0 + 8 * j) = make_float2(acc[4 * j], acc[4 * j + 1]);
-          *reinterpret_cast<float2*>(p1 + 8 * j) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
-        }
-      }
-      named_bar_sync(3, 256);
-      const int row_in_tile = q * 32 + lane;
-      epilogue_drain_tile<BN, EPI>(ep, &tmap_out, &tmap_out2, staging, grp, acc_smem + (size_t)row_in_tile * Cfg::ACC_LD,
-                                   row_in_tile, (m_blk * CL + (int)rank) * BM, n_blk * BN);
-      // the next tile's TMA loads (async proxy) may overwrite what this warp has read
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(epi_bar);
-        if constexpr (CL == 2) mbar_arrive_remote(epi_bar, rank ^ 1u);
-      }
+      epilogue_tile<BN, EPI>(ep, &tmap_out, &tmap_out2, sg, acc, (m_blk * CL + (int)rank) * BM + grp * 64, n_blk * BN);
     }
-    if ((threadIdx.x & 127) == 0) bulk_wait<0>();               // staging tiles must outlive their TMA reads
+    if (sg.issuer) bulk_wait<0>();                              // staging boxes must outlive their TMA reads
   }
   if constexpr (CL == 2) cluster_sync_all();                    // the peer may still multicast into / signal this CTA
 }
@@ -841,7 +811,7 @@ extern "C" int dalm_b200_gemm_bf16(int layout, const void* A, long long lda, con
   else             { if (int e = get_tmap(A, M, K, lda, 128, &ta)) return e; }
   if (layout >= 1) { if (int e = get_tmap(B, K, N, ldb, 64, &tb)) return e; }
   else             { if (int e = get_tmap(B, N, K, ldb, pair ? tile_n / 2 : tile_n, &tb)) return e; }
-  if (int e = get_tmap(out, M, N, ldo, 128, &to, out_f32)) return e;
+  if (int e = get_tmap(out, M, N, ldo, kBoxRows, &to, out_f32)) return e;
   DALM_REQUIRE(drop_p >= 0.f && drop_p < 1.f, "gemm: dropout p must be in [0,1)");
   GemmEpilogue ep = gemm_epilogue(M, N, K, tile_n, out, ldo, out_f32, resid, ldr, resid_f32);
   ep.bias = bias; ep.act = act; ep.alpha = alpha;
@@ -863,8 +833,8 @@ extern "C" int dalm_b200_gemm_bf16_swiglu(const void* A, long long lda, const vo
   CUtensorMap ta, tb, to, to2;
   if (int e = get_tmap(A, M, K, lda, 128, &ta)) return e;
   if (int e = get_tmap(B, N, K, ldb, 256, &tb)) return e;
-  if (int e = get_tmap(gu, M, N, ldgu, 128, &to, 0)) return e;
-  if (int e = get_tmap(act, M, N / 2, ldact, 128, &to2, 0)) return e;
+  if (int e = get_tmap(gu, M, N, ldgu, kBoxRows, &to, 0)) return e;
+  if (int e = get_tmap(act, M, N / 2, ldact, kBoxRows, &to2, 0)) return e;
   const GemmEpilogue ep = gemm_epilogue(M, N, K, 256, gu, ldgu);
   return launch_gemm<256, 0, Epi::SwiGLU>(ta, tb, to, ep, 0, (cudaStream_t)stream, &to2);
 }
@@ -880,8 +850,8 @@ extern "C" int dalm_b200_gemm_bf16_gelu(const void* A, long long lda, const void
   CUtensorMap ta, tb, to, to2;
   if (int e = get_tmap(A, M, K, lda, 128, &ta)) return e;
   if (int e = get_tmap(B, N, K, ldb, bn, &tb)) return e;
-  if (int e = get_tmap(pre, M, N, ldpre, 128, &to, 0)) return e;
-  if (int e = get_tmap(act, M, N, ldact, 128, &to2, 0)) return e;
+  if (int e = get_tmap(pre, M, N, ldpre, kBoxRows, &to, 0)) return e;
+  if (int e = get_tmap(act, M, N, ldact, kBoxRows, &to2, 0)) return e;
   GemmEpilogue ep = gemm_epilogue(M, N, K, bn, pre, ldpre);
   ep.bias = bias;
   return launch_gemm_bn<0, Epi::GeluPair>(bn, ta, tb, to, ep, 0, (cudaStream_t)stream, &to2);
@@ -904,7 +874,7 @@ extern "C" int dalm_b200_gemm_bf16_rope(const void* A, long long lda, const void
   CUtensorMap ta, tb, to;
   if (int e = get_tmap(A, M, K, lda, 128, &ta)) return e;
   if (int e = get_tmap(B, N, K, ldb, 256, &tb)) return e;
-  if (int e = get_tmap(out, M, N, ldo, 128, &to, 0)) return e;
+  if (int e = get_tmap(out, M, N, ldo, kBoxRows, &to, 0)) return e;
   GemmEpilogue ep = gemm_epilogue(M, N, K, 256, out, ldo);
   ep.bias = bias;
   ep.rope_cos = cos_t; ep.rope_sin = sin_t; ep.rope_L = L; ep.rope_cols = rope_cols;
@@ -917,7 +887,7 @@ extern "C" int dalm_b200_gemm_bf16_rope(const void* A, long long lda, const void
   CUtensorMap to2 = to;
   if (pre_out != nullptr) {
     DALM_REQUIRE(ld_pre >= rope_cols && (ld_pre % 8) == 0 && ((uintptr_t)pre_out & 15) == 0, "gemm_rope: pre_out leading dimension / alignment");
-    if (int e = get_tmap(pre_out, M, rope_cols, ld_pre, 128, &to2, 0)) return e;
+    if (int e = get_tmap(pre_out, M, rope_cols, ld_pre, kBoxRows, &to2, 0)) return e;
   }
   ep.q_norm = q_norm; ep.k_norm = k_norm; ep.nq_heads = nq_heads; ep.norm_eps = eps;
   ep.norm_rstd = rstd_out; ep.ld_rstd = ld_rstd; ep.norm_pre = pre_out != nullptr;

@@ -34,6 +34,9 @@ void count_launch(int n = 1);                 // bumps the global launch counter
     }                                                                                     \
   } while (0)
 
+// true when p (which may be null) is a multiple of `bytes`: vector loads / stores of that width are legal at p
+__host__ __device__ inline bool aligned(const void* p, unsigned bytes) { return (reinterpret_cast<uintptr_t>(p) % bytes) == 0; }
+
 // SM count and L2 size of the device the library first runs on (read once; persistent grids and L2 heuristics use them)
 int num_sms();
 long long l2_bytes();

@@ -61,7 +61,7 @@ __global__ void __launch_bounds__(256) embed_scatter_kernel(const float* __restr
                                                             int L, int V) {
   const int m = blockIdx.x;
   long long id = ids[m];
-  id = id < 0 ? 0 : (id >= V ? V - 1 : id);                         // same clamp as the forward gather
+  if (id < 0 || id >= V) id = 0;                                      // the forward gathers read row 0 for any out-of-range id
   const float* src = d + (size_t)m * H;
   float* w = dword + (size_t)id * H;
   float* pp = dpos ? dpos + (size_t)(m % L) * H : nullptr;
@@ -142,6 +142,7 @@ extern "C" int dalm_b200_col_reduce(const float* dy_f32, const void* dy_bf16, lo
   DALM_REQUIRE(!dy_bf16 || (lddy % 4) == 0, "col_reduce: lddy=%lld must be a multiple of 4", lddy);
   DALM_REQUIRE(out_sum || out_prod, "col_reduce: no output");
   DALM_REQUIRE(!out_prod || (z && rstd), "col_reduce: out_prod needs z and rstd");
+  DALM_REQUIRE(aligned(dy_f32, 16) && aligned(z, 16) && aligned(dy_bf16, 8), "col_reduce: fp32 rows must be 16-byte, bf16 rows 8-byte aligned");
   const int colblocks = (H + kCrCols - 1) / kCrCols;
   int splits = (4 * num_sms() + colblocks - 1) / colblocks;
   const int max_splits = (M + 63) / 64;
@@ -158,6 +159,7 @@ extern "C" int dalm_b200_col_reduce(const float* dy_f32, const void* dy_bf16, lo
 extern "C" int dalm_b200_embed_scatter_add(const float* d, const int64_t* ids, float* dword, float* dpos, int M, int H, int L,
                                            int V, void* stream) {
   DALM_REQUIRE(M > 0 && (H % 4) == 0 && L > 0 && V > 0, "embed_scatter_add: bad shape M=%d H=%d L=%d V=%d", M, H, L, V);
+  DALM_REQUIRE(aligned(d, 16), "embed_scatter_add: d must be 16-byte aligned");
   embed_scatter_kernel<<<M, 256, 0, ST(stream)>>>(d, (const long long*)ids, dword, dpos, M, H, L, V);
   count_launch();
   return check_launch("embed_scatter_kernel");
@@ -169,6 +171,7 @@ extern "C" int dalm_b200_masked_add(const float* a, const void* b, long long ldb
   DALM_REQUIRE(a || b, "masked_add: no input");
   DALM_REQUIRE(!b || (ldb % 8) == 0, "masked_add: ldb must be a multiple of 8");
   DALM_REQUIRE(p >= 0.f && p < 1.f, "masked_add: p must be in [0,1)");
+  DALM_REQUIRE(aligned(a, 16) && aligned(out, 16) && aligned(b, 16), "masked_add: operands must be 16-byte aligned");
   const long long n = (long long)M * (H / 8);
   masked_add_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ST(stream)>>>(a, (const __nv_bfloat16*)b, ldb, out, M, H,
                                                                          make_drop(p, seed, stream_id, offset));

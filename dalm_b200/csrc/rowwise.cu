@@ -21,8 +21,10 @@ __global__ void __launch_bounds__(256) layernorm_fwd_kernel(const float* __restr
   __shared__ float red[32];
   const size_t r = blockIdx.x;
   const float* zr = z + r * H;
+  // the vector paths need 16-byte aligned fp32 operands and a y16 aligned to its access width (a view may start mid-row)
+  const bool v32 = aligned(z, 16) && aligned(gamma, 16) && aligned(beta, 16) && aligned(y32, 16);
   float s = 0.f;
-  if ((H & 3) == 0) {
+  if ((H & 3) == 0 && aligned(z, 16)) {
     const float4* z4 = reinterpret_cast<const float4*>(zr);
     float4* row4 = reinterpret_cast<float4*>(row);
     for (int i = threadIdx.x; i < H / 4; i += blockDim.x) { const float4 v = z4[i]; row4[i] = v; s += (v.x + v.y) + (v.z + v.w); }
@@ -35,8 +37,9 @@ __global__ void __launch_bounds__(256) layernorm_fwd_kernel(const float* __restr
   const float var = block_sum(q, red) / H;
   const float rstd = rsqrtf(var + eps);
   if (threadIdx.x == 0) { mean_out[r] = mean; rstd_out[r] = rstd; }
-  if (drop.p > 0.f && (H & 7) == 0) {                          // embeddings dropout: one Philox call per 8 outputs
+  if (drop.p > 0.f && (H & 7) == 0 && v32) {                   // embeddings dropout: one Philox call per 8 outputs
     const unsigned long long dstream = drop_stream(drop);
+    const bool y16_v8 = (ld16 & 7) == 0 && aligned(y16, 16);
     for (int i8 = threadIdx.x; i8 < H / 8; i8 += blockDim.x) {
       float sc[8];
       drop_scale8(drop, dstream, ((unsigned long long)r * H >> 3) + i8, sc);
@@ -52,7 +55,7 @@ __global__ void __launch_bounds__(256) layernorm_fwd_kernel(const float* __restr
         *reinterpret_cast<float4*>(y32 + r * H + i0) = make_float4(v[0], v[1], v[2], v[3]);
         *reinterpret_cast<float4*>(y32 + r * H + i0 + 4) = make_float4(v[4], v[5], v[6], v[7]);
       }
-      if ((ld16 & 7) == 0) *reinterpret_cast<bf16x8*>(y16 + r * ld16 + i0) = pack8(v);
+      if (y16_v8) *reinterpret_cast<bf16x8*>(y16 + r * ld16 + i0) = pack8(v);
       else {
 #pragma unroll
         for (int j = 0; j < 8; ++j) y16[r * ld16 + i0 + j] = __float2bfloat16_rn(v[j]);
@@ -60,7 +63,7 @@ __global__ void __launch_bounds__(256) layernorm_fwd_kernel(const float* __restr
     }
     return;
   }
-  if (drop.p == 0.f && (H & 3) == 0 && (ld16 & 3) == 0) {        // vectorised plain path: 4 outputs per thread per iteration
+  if (drop.p == 0.f && (H & 3) == 0 && v32 && (ld16 & 3) == 0 && aligned(y16, 8)) {   // vectorised plain path: 4 outputs per thread
     const float4* row4 = reinterpret_cast<const float4*>(row);
     const float4* g4 = reinterpret_cast<const float4*>(gamma);
     const float4* b4 = reinterpret_cast<const float4*>(beta);
@@ -101,7 +104,8 @@ __global__ void __launch_bounds__(256) layernorm_bwd_kernel(const float* __restr
   const size_t r = blockIdx.x;
   const float mean = mean_in[r], rstd = rstd_in[r];
   float s1 = 0.f, s2 = 0.f;
-  if ((H & 3) == 0 && (ldb & 3) == 0) {
+  const bool v32 = aligned(dz32, 16) && aligned(dres, 16);         // vector stores of the fp32 output
+  if ((H & 3) == 0 && (ldb & 3) == 0 && aligned(z, 16) && aligned(gamma, 16) && aligned(dy_a, 16) && aligned(dy_b, 8)) {
     const float4* z4 = reinterpret_cast<const float4*>(z + r * H);
     const float4* a4 = dy_a ? reinterpret_cast<const float4*>(dy_a + r * H) : nullptr;
     const uint2* b2 = dy_b ? reinterpret_cast<const uint2*>(dy_b + r * ldb) : nullptr;
@@ -136,8 +140,9 @@ __global__ void __launch_bounds__(256) layernorm_bwd_kernel(const float* __restr
   s1 = block_sum(s1, red) / H;
   s2 = block_sum(s2, red) / H;
   // z = dropout(dense_out) + residual: the residual branch takes dz as is (dz32), the dense branch takes mask*dz/(1-p)
-  if (drop16.p > 0.f && (H & 7) == 0) {
+  if (drop16.p > 0.f && (H & 7) == 0 && v32) {
     const unsigned long long dstream = drop_stream(drop16);
+    const bool dz16_v8 = (ld16 & 7) == 0 && aligned(dz16, 16);
     for (int i8 = threadIdx.x; i8 < H / 8; i8 += blockDim.x) {
       float sc[8];
       drop_scale8(drop16, dstream, ((unsigned long long)r * H >> 3) + i8, sc);
@@ -150,7 +155,7 @@ __global__ void __launch_bounds__(256) layernorm_bwd_kernel(const float* __restr
         *reinterpret_cast<float4*>(dz32 + r * H + i0 + 4) = make_float4(d[4], d[5], d[6], d[7]);
       }
       if (dz16) {
-        if ((ld16 & 7) == 0) *reinterpret_cast<bf16x8*>(dz16 + r * ld16 + i0) = pack8(dm);
+        if (dz16_v8) *reinterpret_cast<bf16x8*>(dz16 + r * ld16 + i0) = pack8(dm);
         else {
 #pragma unroll
           for (int j = 0; j < 8; ++j) dz16[r * ld16 + i0 + j] = __float2bfloat16_rn(dm[j]);
@@ -159,7 +164,7 @@ __global__ void __launch_bounds__(256) layernorm_bwd_kernel(const float* __restr
     }
     return;
   }
-  if (drop16.p == 0.f && (H & 3) == 0 && (ld16 & 3) == 0) {
+  if (drop16.p == 0.f && (H & 3) == 0 && v32 && (ld16 & 3) == 0 && aligned(dz16, 8)) {
     for (int i = threadIdx.x; i < H / 4; i += blockDim.x) {
       const float4 g = reinterpret_cast<const float4*>(gbuf)[i], zz = reinterpret_cast<const float4*>(zh)[i];
       float4 d = make_float4(rstd * (g.x - s1 - zz.x * s2), rstd * (g.y - s1 - zz.y * s2), rstd * (g.z - s1 - zz.z * s2),
@@ -771,19 +776,28 @@ __global__ void pack_table_kernel(const PackEntry* __restrict__ table) {
 // out_bf16 [rows, ldo] <- fp32 [rows, cols]  (plain cast, vectorised)
 __global__ void cast_f32_bf16_kernel(const float* __restrict__ in, long long ldi, __nv_bfloat16* __restrict__ out,
                                      long long ldo, int rows, int cols) {
-  const size_t r = blockIdx.y;
   const int c = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
   if (c >= cols) return;
-  const float4 v = *reinterpret_cast<const float4*>(in + r * ldi + c);
-  __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
-  uint2 pk; pk.x = *reinterpret_cast<uint32_t*>(&a); pk.y = *reinterpret_cast<uint32_t*>(&b);
-  *reinterpret_cast<uint2*>(out + r * ldo + c) = pk;
+  for (size_t r = blockIdx.y; r < (size_t)rows; r += gridDim.y) {     // gridDim.y is capped at 65535: rows stride over it
+    const float4 v = *reinterpret_cast<const float4*>(in + r * ldi + c);
+    __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
+    uint2 pk; pk.x = *reinterpret_cast<uint32_t*>(&a); pk.y = *reinterpret_cast<uint32_t*>(&b);
+    *reinterpret_cast<uint2*>(out + r * ldo + c) = pk;
+  }
 }
 
 }  // namespace dalm
 
 using namespace dalm;
 #define ST(s) ((cudaStream_t)(s))
+
+// The CTA-per-row norms stage rows in dynamic shared memory up to 48 KB. The default per-kernel limit leaves out the
+// kernel's static shared memory (`red`), so each of them opts in to the full size once.
+static int allow_ln_bwd_smem() {
+  static bool attr = false;
+  if (!attr) { DALM_CUDA(cudaFuncSetAttribute(layernorm_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 48 * 1024)); attr = true; }
+  return 0;
+}
 
 extern "C" int dalm_b200_layernorm_fwd(const float* z, const float* gamma, const float* beta, float* y32, void* y16,
                                        long long ld16, float* mean, float* rstd, int M, int H, float eps, float drop_p,
@@ -801,6 +815,9 @@ extern "C" int dalm_b200_layernorm_fwd(const float* z, const float* gamma, const
       default: return launch_ln_fwd_warp<8>(z, gamma, beta, y32, y, ld16, mean, rstd, M, eps, d, ST(stream));
     }
   }
+  // the row is staged in H * 4 bytes of dynamic shared memory: above 48 KB (less the static `red`) only with the opt-in
+  static bool attr = false;
+  if (!attr) { DALM_CUDA(cudaFuncSetAttribute(layernorm_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024)); attr = true; }
   layernorm_fwd_kernel<<<M, 256, H * sizeof(float), ST(stream)>>>(z, gamma, beta, y32, (__nv_bfloat16*)y16, ld16, mean, rstd, H, eps,
                                                                   make_drop(drop_p, drop_seed, drop_stream_id, drop_offset));
   count_launch();
@@ -822,6 +839,7 @@ extern "C" int dalm_b200_layernorm_bwd(const float* z, const float* gamma, const
       default: return launch_ln_bwd_warp<8>(z, gamma, mean, rstd, dy_f32, b, ldb, dz32, o, ld16, M, d, nullptr, ST(stream));
     }
   }
+  if (int e = allow_ln_bwd_smem()) return e;
   layernorm_bwd_kernel<<<M, 256, 2 * H * sizeof(float), ST(stream)>>>(z, gamma, mean, rstd, dy_f32, (const __nv_bfloat16*)dy_bf16, ldb,
                                                                      dz32, (__nv_bfloat16*)dz16, ld16, H,
                                                                      make_drop(drop_p, drop_seed, drop_stream_id, drop_offset), nullptr);
@@ -845,6 +863,7 @@ extern "C" int dalm_b200_layernorm_bwd_res(const float* z, const float* gamma, c
       default: return launch_ln_bwd_warp<8>(z, gamma, mean, rstd, dy_f32, b, ldb, dz32, o, ld16, M, d, dres, ST(stream));
     }
   }
+  if (int e = allow_ln_bwd_smem()) return e;
   layernorm_bwd_kernel<<<M, 256, 2 * H * sizeof(float), ST(stream)>>>(z, gamma, mean, rstd, dy_f32, (const __nv_bfloat16*)dy_bf16, ldb,
                                                                      dz32, (__nv_bfloat16*)dz16, ld16, H, make_drop(0.f, 0, 0, nullptr), dres);
   count_launch();
@@ -853,6 +872,9 @@ extern "C" int dalm_b200_layernorm_bwd_res(const float* z, const float* gamma, c
 extern "C" int dalm_b200_rmsnorm_fwd(const float* x, const float* g, void* h, long long ldh, float* rstd, int M, int H,
                                      float eps, void* stream) {
   DALM_REQUIRE(M > 0 && H > 0 && (H % 4) == 0 && H * 4 <= 48 * 1024 && (ldh % 4) == 0, "rmsnorm_fwd: bad shape M=%d H=%d", M, H);
+  DALM_REQUIRE(aligned(x, 16) && aligned(g, 16) && aligned(h, 8), "rmsnorm_fwd: x / g must be 16-byte and h 8-byte aligned");
+  static bool attr = false;
+  if (!attr) { DALM_CUDA(cudaFuncSetAttribute(rmsnorm_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 48 * 1024)); attr = true; }
   rmsnorm_fwd_kernel<<<M, 256, H * sizeof(float), ST(stream)>>>(x, g, (__nv_bfloat16*)h, ldh, rstd, H, eps);
   count_launch();
   return check_launch("rmsnorm_fwd_kernel");
@@ -862,6 +884,8 @@ extern "C" int dalm_b200_rmsnorm_bwd(const float* x, const float* g, const float
                                      void* stream) {
   DALM_REQUIRE(M > 0 && H > 0 && (H % 4) == 0 && H * 8 <= 96 * 1024 && (lddh % 4) == 0 && (ld16 % 4) == 0,
                "rmsnorm_bwd: bad shape M=%d H=%d", M, H);
+  DALM_REQUIRE(aligned(x, 16) && aligned(g, 16) && aligned(dres_in, 16) && aligned(dres_out, 16) && aligned(dh, 8) && aligned(dres16, 8),
+               "rmsnorm_bwd: fp32 operands must be 16-byte and bf16 ones 8-byte aligned");
   static bool attr = false;
   if (!attr) { DALM_CUDA(cudaFuncSetAttribute(rmsnorm_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024)); attr = true; }
   rmsnorm_bwd_kernel<<<M, 256, 2 * H * sizeof(float), ST(stream)>>>(x, g, rstd, (const __nv_bfloat16*)dh, lddh, dres_in, dres_out,
@@ -1000,7 +1024,9 @@ extern "C" int dalm_b200_pack_table(const void* table, int n_entries, void* stre
 }
 extern "C" int dalm_b200_cast_f32_bf16(const float* in, long long ldi, void* out, long long ldo, int rows, int cols, void* stream) {
   DALM_REQUIRE((cols % 4) == 0 && (ldi % 4) == 0 && (ldo % 4) == 0, "cast: cols/strides must be multiples of 4");
-  dim3 grid((cols / 4 + 255) / 256, rows);
+  DALM_REQUIRE(aligned(in, 16) && aligned(out, 8), "cast: in must be 16-byte and out 8-byte aligned");
+  if (rows <= 0 || cols <= 0) return 0;
+  dim3 grid((cols / 4 + 255) / 256, rows < 65535 ? rows : 65535);
   cast_f32_bf16_kernel<<<grid, 256, 0, ST(stream)>>>(in, ldi, (__nv_bfloat16*)out, ldo, rows, cols);
   count_launch();
   return check_launch("cast_f32_bf16_kernel");

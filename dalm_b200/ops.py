@@ -35,6 +35,25 @@ def _chk(t: torch.Tensor, dtype, name: str, inner_contig: bool = True) -> None:
         raise _lib.DalmB200Error(f"{name}: innermost dimension must be contiguous")
 
 
+def _rows32(t: Optional[torch.Tensor], name: str, H: int, M: Optional[int] = None) -> None:
+    """fp32 [M (any when None), H] operand that the kernels index as dense rows (ptr + r * H): a row-strided view would be
+    read at the wrong elements, so it is refused"""
+    if t is None:
+        return
+    _chk(t, f32, name)
+    if t.dim() != 2 or t.shape[1] != H or (M is not None and t.shape[0] != M) or not t.is_contiguous():
+        want = f"[{M if M is not None else 'rows'}, {H}]"
+        raise _lib.DalmB200Error(f"{name}: expected dense fp32 rows {want}, got shape {tuple(t.shape)} strides {t.stride()}")
+
+
+def _tables16(*named) -> None:
+    """bf16 embedding tables, which the gathers index as dense rows (id * H)"""
+    for name, t in named:
+        _chk(t, bf16, name)
+        if not t.is_contiguous():
+            raise _lib.DalmB200Error(f"{name}: expected a dense bf16 table, got strides {t.stride()}")
+
+
 class Drop:
     """dropout site descriptor: probability, seed, stream id (identifies layer / tensor / call) and an optional device
     uint64 counter added to the stream id (see include/dalm_b200.h)"""
@@ -348,6 +367,7 @@ def attention_auto_bwd(q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal,
 def layernorm_fwd(z, gamma, beta, eps: float, y16=None, want_f32: bool = True, drop: Optional[Drop] = None):
     _chk(z, f32, "z")
     M, H = z.shape
+    _rows32(z, "layernorm_fwd z", H)
     y32 = torch.empty_like(z) if want_f32 else None
     if y16 is None:
         y16 = torch.empty(M, H, dtype=bf16, device=z.device)
@@ -360,6 +380,9 @@ def layernorm_fwd(z, gamma, beta, eps: float, y16=None, want_f32: bool = True, d
 def layernorm_bwd(z, gamma, mean, rstd, dy_f32=None, dy_bf16=None, want_f32: bool = True, dz16=None, want_bf16: bool = True,
                   drop16: Optional[Drop] = None):
     M, H = z.shape
+    _rows32(z, "layernorm_bwd z", H); _rows32(dy_f32, "layernorm_bwd dy_f32", H, M)
+    if dy_bf16 is not None:
+        _chk(dy_bf16, bf16, "layernorm_bwd dy_bf16")
     dz32 = torch.empty_like(z) if want_f32 else None
     if want_bf16 and dz16 is None:
         dz16 = torch.empty(M, H, dtype=bf16, device=z.device)
@@ -372,6 +395,8 @@ def layernorm_bwd(z, gamma, mean, rstd, dy_f32=None, dy_bf16=None, want_f32: boo
 def layernorm_bwd_res(z, gamma, mean, rstd, dy_bf16, dres, dz32=None, dz16=None):
     """pre-LN residual block: dz = LayerNorm-backward(dy) + dres  -> (dz32, dz16); dz32 may be `dres` itself (in place)"""
     M, H = z.shape
+    _rows32(z, "layernorm_bwd_res z", H); _rows32(dres, "layernorm_bwd_res dres", H, M); _rows32(dz32, "layernorm_bwd_res dz32", H, M)
+    _chk(dy_bf16, bf16, "layernorm_bwd_res dy_bf16")
     if dz32 is None:
         dz32 = torch.empty_like(z)
     if dz16 is None:
@@ -384,6 +409,7 @@ def layernorm_bwd_res(z, gamma, mean, rstd, dy_bf16, dres, dz32=None, dz16=None)
 def rmsnorm_fwd(x, g, eps: float, h=None):
     _chk(x, f32, "x")
     M, H = x.shape
+    _rows32(x, "rmsnorm_fwd x", H)
     if h is None:
         h = torch.empty(M, H, dtype=bf16, device=x.device)
     rstd = torch.empty(M, dtype=f32, device=x.device)
@@ -393,6 +419,8 @@ def rmsnorm_fwd(x, g, eps: float, h=None):
 
 def rmsnorm_bwd(x, g, rstd, dh, dres_in=None, dres_out=None, dres16=None, want_bf16: bool = True):
     M, H = x.shape
+    _rows32(x, "rmsnorm_bwd x", H); _rows32(dres_in, "rmsnorm_bwd dres_in", H, M); _rows32(dres_out, "rmsnorm_bwd dres_out", H, M)
+    _chk(dh, bf16, "rmsnorm_bwd dh")
     if dres_out is None:
         dres_out = torch.empty_like(x)
     if want_bf16 and dres16 is None:
@@ -405,6 +433,8 @@ def rmsnorm_bwd(x, g, rstd, dh, dres_in=None, dres_out=None, dres16=None, want_b
 def bert_embed(ids, word, pos, type_emb, out=None):
     B, L = ids.shape
     V, H = word.shape
+    _rows32(out, "bert_embed out", H, B * L)
+    _tables16(("bert_embed word", word), ("bert_embed pos", pos), ("bert_embed type", type_emb))
     z = torch.empty(B * L, H, dtype=f32, device=ids.device) if out is None else out
     _lib.call("dalm_b200_bert_embed", _p(ids.contiguous()), _p(word), _p(pos), _p(type_emb), _p(z), B * L, L, H, V, _stream())
     return z
@@ -413,6 +443,7 @@ def bert_embed(ids, word, pos, type_emb, out=None):
 def embed_gather(ids, table):
     M = ids.numel()
     V, H = table.shape
+    _tables16(("embed_gather table", table))
     x = torch.empty(M, H, dtype=f32, device=ids.device)
     _lib.call("dalm_b200_embed_gather", _p(ids.contiguous()), _p(table), _p(x), M, H, V, _stream())
     return x
@@ -684,6 +715,10 @@ def pack_table_(table: torch.Tensor) -> None:
 
 
 def cast_f32_bf16(src, dst=None):
+    """dst bf16 [M,N] = src fp32 [M,N] (both with contiguous rows; a transposed source is refused, not misread)"""
+    _chk(src, f32, "cast_f32_bf16 src")
+    if dst is not None:
+        _chk(dst, bf16, "cast_f32_bf16 dst")
     M, N = src.shape
     if dst is None:
         dst = torch.empty(M, N, dtype=bf16, device=src.device)
@@ -701,8 +736,7 @@ def col_reduce_(dy_f32=None, dy_bf16=None, z=None, mean=None, rstd=None, out_sum
     """out_sum[h] += sum_m dy[m,h]; out_prod[h] += sum_m dy[m,h] * (z[m,h]-mean[m]) * rstd[m]   (dy = dy_f32 + dy_bf16)"""
     ref = dy_f32 if dy_f32 is not None else dy_bf16
     M, H = ref.shape
-    if dy_f32 is not None:
-        _chk(dy_f32, f32, "col_reduce dy_f32", inner_contig=False)
+    _rows32(dy_f32, "col_reduce dy_f32", H, M); _rows32(z, "col_reduce z", H, M)
     if dy_bf16 is not None:
         _chk(dy_bf16, bf16, "col_reduce dy_bf16")
     _lib.call("dalm_b200_col_reduce", _p(dy_f32), _p(dy_bf16), _ld(dy_bf16) if dy_bf16 is not None else 0, _p(z), _p(mean),
@@ -711,12 +745,19 @@ def col_reduce_(dy_f32=None, dy_bf16=None, z=None, mean=None, rstd=None, out_sum
 
 def embed_scatter_add_(d, ids, dword, dpos=None, L: int = 1) -> None:
     M, H = d.shape
+    _rows32(d, "embed_scatter_add d", H); _rows32(dword, "embed_scatter_add dword", H); _rows32(dpos, "embed_scatter_add dpos", H)
+    _chk(ids, i64, "embed_scatter_add ids")
+    if ids.numel() != M or not ids.is_contiguous():
+        raise _lib.DalmB200Error(f"embed_scatter_add: need one contiguous id per row ({ids.numel()} for {M} rows)")
     _lib.call("dalm_b200_embed_scatter_add", _p(d), _p(ids), _p(dword), _p(dpos), M, H, int(L), dword.shape[0], _stream())
 
 
 def masked_add(a=None, b=None, drop: Optional[Drop] = None, out=None):
     ref = a if a is not None else b
     M, H = ref.shape
+    _rows32(a, "masked_add a", H, M); _rows32(out, "masked_add out", H, M)
+    if b is not None:
+        _chk(b, bf16, "masked_add b")
     if out is None:
         out = torch.empty(M, H, dtype=f32, device=ref.device)
     _lib.call("dalm_b200_masked_add", _p(a), _p(b), _ld(b) if b is not None else 0, _p(out), M, H, *_d(drop), _stream())

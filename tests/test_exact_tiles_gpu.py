@@ -18,11 +18,9 @@ import random
 import pytest
 import torch
 
-bf16, f32, f64 = torch.bfloat16, torch.float32, torch.float64
+from exact_helpers import PAD_R, Guarded, _expect_close, _expect_equal, _poisoned, _ulp_bf16, _ulp_f32
 
-GUARD_R, GUARD_C = 128, 256                      # guard band around every output: one tile of rows / a 256-wide tile of columns
-PAD_R, PAD_C = 128, 64                           # NaN rows after / NaN columns right of every input view
-_SENTINEL_BITS = {bf16: (torch.int16, 0x7FA5), f32: (torch.int32, 0x7FA5A5A5)}   # NaN payloads no kernel writes
+bf16, f32, f64 = torch.bfloat16, torch.float32, torch.float64
 
 
 @pytest.fixture(scope="module")
@@ -38,78 +36,6 @@ def dev():
 def ops(dev):
     from dalm_b200 import ops as _ops
     return _ops
-
-
-# ----------------------------------------------------------------------------------------------------------------
-# poisoned inputs, guarded outputs
-# ----------------------------------------------------------------------------------------------------------------
-def _poisoned(x: torch.Tensor) -> torch.Tensor:
-    """x [r, c] copied into the top-left of a NaN buffer [r + 128, c + 64]: a view whose row stride runs into NaN columns
-    and whose rows are followed by NaN rows (1-D: N values followed by 256 NaNs)"""
-    if x.dim() == 1:
-        buf = torch.full((x.shape[0] + 256,), float("nan"), dtype=x.dtype, device=x.device)
-        buf[: x.shape[0]] = x
-        return buf[: x.shape[0]]
-    r, c = x.shape
-    buf = torch.full((r + PAD_R, c + PAD_C), float("nan"), dtype=x.dtype, device=x.device)
-    buf[:r, :c] = x
-    return buf[:r, :c]
-
-
-class Guarded:
-    """an output view [rows, cols] inside a sentinel-filled buffer with GUARD_R rows above / below and GUARD_C columns left /
-    right (16-byte aligned: the view starts 256 elements into a row and the row stride is cols + 512)"""
-
-    def __init__(self, rows, cols, dtype, dev, init=None):
-        itype, bits = _SENTINEL_BITS[dtype]
-        self.buf = torch.full((rows + 2 * GUARD_R, cols + 2 * GUARD_C), bits, dtype=itype, device=dev).view(dtype)
-        self.rows, self.cols, self.itype, self.bits = rows, cols, itype, bits
-        self.view = self.buf[GUARD_R:GUARD_R + rows, GUARD_C:GUARD_C + cols]
-        if init is not None:
-            self.view.copy_(init)
-
-    def check(self, what):
-        b = self.buf.view(self.itype).clone()
-        b[GUARD_R:GUARD_R + self.rows, GUARD_C:GUARD_C + self.cols] = self.bits
-        bad = b != self.bits
-        if bad.any():
-            r, c = bad.nonzero()[0].tolist()
-            pytest.fail(f"{what}: {int(bad.sum())} guard elements overwritten; first at buffer ({r}, {c}) = output "
-                        f"({r - GUARD_R}, {c - GUARD_C}) of a [{self.rows}, {self.cols}] view")
-
-
-def _ulp_bf16(x):
-    """spacing of bf16 numbers at |x| (fp64), normal range"""
-    return torch.pow(2.0, torch.floor(torch.log2(x.abs().clamp_min(2.0 ** -126))) - 7)
-
-
-def _ulp_f32(x):
-    return torch.pow(2.0, torch.floor(torch.log2(x.abs().clamp_min(2.0 ** -126))) - 23)
-
-
-def _where(bad, what, tile_m=128, tile_n=None):
-    r, c = bad.nonzero()[0].tolist()
-    tile = f" = tile (m {r // tile_m}, n {c // tile_n})" if tile_n else ""
-    return f"{what}: {int(bad.sum())} of {bad.numel()} elements wrong; first at (row {r}, col {c}){tile}"
-
-
-def _expect_equal(got, want, what, tile_m=128, tile_n=None):
-    """got (kernel output, any float dtype) == want (same dtype) element for element (+0 == -0), no NaN"""
-    g, w = got.double(), want.double()
-    bad = (g != w) | torch.isnan(g)
-    if bad.any():
-        r, c = bad.nonzero()[0].tolist()
-        pytest.fail(_where(bad, what, tile_m, tile_n) + f": got {g[r, c].item()!r}, want {w[r, c].item()!r}")
-
-
-def _expect_close(got, ref, tol, what, tile_m=128, tile_n=None):
-    """|got - ref| <= tol element-wise (fp64), no NaN"""
-    g = got.double()
-    bad = ~((g - ref).abs() <= tol)
-    if bad.any():
-        r, c = bad.nonzero()[0].tolist()
-        pytest.fail(_where(bad, what, tile_m, tile_n) + f": got {g[r, c].item()!r}, ref {ref[r, c].item()!r}, "
-                    f"tol {tol[r, c].item() if torch.is_tensor(tol) else tol!r}")
 
 
 # ----------------------------------------------------------------------------------------------------------------

@@ -9,8 +9,8 @@ not a CTA cap, is what makes the CTAs walk several tiles.
 import pytest
 import torch
 
-from test_exact_tiles_gpu import (STAGES, Guarded, _expect_close, _expect_equal, _gelu64, _ints, _pick_block_n, _poisoned,
-                                  _ulp_bf16, _ulp_f32)
+from exact_helpers import Guarded, _expect_close, _expect_equal, _poisoned, _ulp_bf16, _ulp_f32
+from test_exact_tiles_gpu import STAGES, _gelu64, _ints, _pick_block_n
 from test_qwen3_gpu import EPS, _norm_w, _ref_norm_rope, _tables
 
 pytestmark = pytest.mark.gpu

@@ -11,7 +11,8 @@ import os
 import pytest
 import torch
 
-from test_exact_tiles_gpu import M_EDGE, Guarded, _expect_close, _expect_equal, _ints, _poisoned, _ulp_bf16
+from exact_helpers import Guarded, _expect_close, _expect_equal, _poisoned, _ulp_bf16
+from test_exact_tiles_gpu import M_EDGE, _ints
 
 pytestmark = pytest.mark.gpu
 bf16, f32, f64 = torch.bfloat16, torch.float32, torch.float64

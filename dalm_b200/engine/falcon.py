@@ -25,6 +25,7 @@ import torch
 
 from .. import ops
 from .dense import DenseBank
+from .params import rope_inv_freq
 
 bf16, f32 = torch.bfloat16, torch.float32
 
@@ -54,7 +55,7 @@ class FalconDecoder(torch.nn.Module):
         self.V = cfg["vocab_size"]
         self.F = cfg.get("ffn_hidden_size") or 4 * H
         self.eps = float(cfg.get("layer_norm_epsilon", 1e-5))
-        self.theta = float(cfg.get("rope_theta", 10000.0))
+        self.inv_freq = rope_inv_freq(cfg, self.hd)           # default RoPE only: a scaled one is refused
         self.dev = torch.device(device)
         if self.hd not in (32, 64, 128):
             raise NotImplementedError(f"head_dim {self.hd} not supported by the attention kernels")
@@ -159,8 +160,7 @@ class FalconDecoder(torch.nn.Module):
 
     def _rope(self, L: int):
         if L not in self._rope_cache:
-            inv = 1.0 / (self.theta ** (torch.arange(0, self.hd, 2, dtype=torch.float32) / self.hd))
-            fr = torch.outer(torch.arange(L, dtype=torch.float32), inv)
+            fr = torch.outer(torch.arange(L, dtype=torch.float32), self.inv_freq)
             self._rope_cache[L] = (fr.cos().to(self.dev).contiguous(), fr.sin().to(self.dev).contiguous())
         return self._rope_cache[L]
 

@@ -15,6 +15,8 @@ Residual stream and its gradient are fp32; every GEMM operand is bf16.
 Qwen2 is this architecture plus q/k/v biases (HF Qwen2ForCausalLM); Qwen3 (HF Qwen3ForCausalLM) adds the per-head q/k RMSNorm,
 fused into the QKV GEMM's RoPE epilogue (training shapes) or applied by the qk_norm_rope row kernel (decode, prefill, other
 widths); the backward saves the pre-norm q|k columns and their rstd. Configs are checked by params.check_llama_family.
+Llama 3.x is this architecture with GQA and frequency-scaled RoPE: params.rope_inv_freq builds the default, `linear` and
+`llama3` frequencies, and every RoPE kernel reads the cos / sin tables `_rope` makes from them.
 """
 from __future__ import annotations
 
@@ -25,7 +27,7 @@ import torch
 from .. import ops
 from .dense import DenseBank
 from .lora import LoraBank
-from .params import attention_biases, check_llama_family
+from .params import attention_biases, check_llama_family, rope_inv_freq
 
 bf16, f32 = torch.bfloat16, torch.float32
 
@@ -73,11 +75,10 @@ class LlamaDecoder(torch.nn.Module):
         self.hd = cfg.get("head_dim") or H // self.nh
         self.V = cfg["vocab_size"]
         self.eps = float(cfg.get("rms_norm_eps", 1e-5))
-        rp = cfg.get("rope_parameters") or {}
-        self.theta = float(cfg.get("rope_theta", rp.get("rope_theta", 10000.0)))
         self.dev = torch.device(device)
         if self.hd not in (32, 64, 128):
             raise NotImplementedError(f"head_dim {self.hd} not supported by the attention kernels")
+        self.inv_freq = rope_inv_freq(cfg, self.hd)           # default, linear or llama3 frequencies (fp32, CPU)
         self.Nq, self.Nkv = self.nh * self.hd, self.nkv * self.hd
         self.Nqkv = self.Nq + 2 * self.Nkv
         self.r = 8
@@ -352,12 +353,11 @@ class LlamaDecoder(torch.nn.Module):
         ops.pack_table_(self._pack_tab)
 
     def _rope(self, L: int):
+        """fp32 cos / sin tables [L, hd/2] at positions 0..L-1: what every RoPE kernel reads (the QKV epilogue, the row kernels,
+        decode); the frequency scaling of the config lives in `inv_freq` only"""
         if L not in self._rope_cache:
-            half = self.hd // 2
-            inv = 1.0 / (self.theta ** (torch.arange(0, self.hd, 2, dtype=torch.float32) / self.hd))   # HF inv_freq
-            fr = torch.outer(torch.arange(L, dtype=torch.float32), inv)                                 # [L, hd/2]
+            fr = torch.outer(torch.arange(L, dtype=torch.float32), self.inv_freq)                      # [L, hd/2]
             self._rope_cache[L] = (fr.cos().to(self.dev).contiguous(), fr.sin().to(self.dev).contiguous())
-            assert fr.shape[1] == half
         return self._rope_cache[L]
 
     # ------------------------------------------------------------------------------------------------------------

@@ -2,6 +2,7 @@
 from __future__ import annotations
 
 import json
+import math
 import os
 from typing import Dict, Optional
 
@@ -155,6 +156,7 @@ def model_kind(cfg: Dict) -> str:
         check_llama_family(cfg)
         return mt
     if mt == "falcon":
+        check_rope_type(cfg)
         return "falcon"
     raise NotImplementedError(
         f"model_type {mt!r} is not built in dalm_b200 (supported: bert encoders; llama, qwen2, qwen3 and falcon decoders)")
@@ -170,9 +172,63 @@ def _rope_type(cfg: Dict) -> str:
     return "default"
 
 
+def rope_parameters(cfg: Dict) -> Dict:
+    """the RoPE settings of an HF config as transformers reads them: the hub spelling `rope_scaling` when it is set, else
+    transformers 5's `rope_parameters`; `rope_type` (or the legacy `type`, default 'default') and `rope_theta` (the dict's own,
+    else the top-level key, else 10000) always present"""
+    rp = cfg.get("rope_scaling") or cfg.get("rope_parameters") or {}
+    rp = dict(rp) if isinstance(rp, dict) else {}
+    rp["rope_type"] = rp.get("rope_type", rp.get("type")) or "default"
+    rp.setdefault("rope_theta", cfg.get("rope_theta", 10000.0))
+    return rp
+
+
+# RoPE types whose frequencies are a fixed table: a position-indexed cos / sin table represents them exactly. `dynamic` changes
+# the frequencies with the sequence length, `yarn` / `longrope` also scale the attention, `proportional` rotates part of a head.
+BUILT_ROPE_TYPES = {"llama": ("default", "linear", "llama3")}
+
+
+def check_rope_type(cfg: Dict) -> str:
+    """the config's RoPE type; raises NotImplementedError, naming it, when the model family does not build it"""
+    mt = cfg.get("model_type", "")
+    rt = rope_parameters(cfg)["rope_type"]
+    built = BUILT_ROPE_TYPES.get(mt, ("default",))
+    if rt not in built:
+        raise NotImplementedError(f"{mt}: RoPE type {rt!r} (rope_scaling / rope_parameters) is not built; built: "
+                                  + ", ".join(repr(t) for t in built))
+    return rt
+
+
+def rope_inv_freq(cfg: Dict, head_dim: int) -> torch.Tensor:
+    """fp32 [head_dim / 2] inverse frequencies of the config's RoPE, bit for bit what transformers' rope init functions
+    (modeling_rope_utils: default, `linear`, `llama3`) compute on the CPU: the same fp32 operations in the same order. All
+    three have attention factor 1, so cos / sin tables built from these frequencies are the whole of the position encoding."""
+    rt = check_rope_type(cfg)
+    rp = rope_parameters(cfg)
+    base = rp["rope_theta"]
+    inv_freq = 1.0 / (base ** (torch.arange(0, head_dim, 2, dtype=torch.int64).to(dtype=torch.float) / head_dim))
+    if rt == "linear":
+        inv_freq /= rp["factor"]
+    elif rt == "llama3":
+        factor, low, high = rp["factor"], rp["low_freq_factor"], rp["high_freq_factor"]
+        old_len = rp.get("original_max_position_embeddings") or cfg.get("original_max_position_embeddings") \
+            or cfg["max_position_embeddings"]
+        low_freq_wavelen, high_freq_wavelen = old_len / low, old_len / high
+        wavelen = 2 * math.pi / inv_freq
+        # wavelengths above old_len / low are divided by factor, those below old_len / high kept, the band between blended
+        scaled = torch.where(wavelen > low_freq_wavelen, inv_freq / factor, inv_freq)
+        smooth = (old_len / wavelen - low) / (high - low)
+        smoothed = (1 - smooth) * scaled / factor + smooth * scaled
+        medium = ~(wavelen < high_freq_wavelen) * ~(wavelen > low_freq_wavelen)
+        inv_freq = torch.where(medium, smoothed, scaled)
+    return inv_freq
+
+
 def check_llama_family(cfg: Dict) -> None:
     """refuses the settings of a llama / qwen2 / qwen3 config that LlamaDecoder would otherwise silently compute wrong"""
     mt = cfg.get("model_type", "")
+    if mt == "llama":
+        check_rope_type(cfg)
     if cfg.get("mlp_bias", False):
         raise NotImplementedError(f"{mt}: mlp_bias=true is not built (the fused SwiGLU MLP has no bias)")
     if mt == "qwen3":

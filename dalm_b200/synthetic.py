@@ -34,6 +34,32 @@ LLAMA_SHAPES: Dict[str, Dict] = {
 }
 
 
+# Llama 3.x (model_type "llama", GQA, rope_theta 5e5, llama3 RoPE frequency scaling). The tiny shapes use an
+# original_max_position_embeddings of 64 so that every band of the llama3 rule occurs at their head_dim: the short wavelengths
+# (kept), the long ones (divided by factor) and the band between (blended)
+LLAMA3_SHAPES: Dict[str, Dict] = {
+    "llama3-tiny": dict(hidden_size=512, num_hidden_layers=2, num_attention_heads=4, num_key_value_heads=2, head_dim=128,
+                        intermediate_size=1024, tie_word_embeddings=False,                # 6 q|k heads x 128: RoPE in the QKV epilogue
+                        rope_scaling=dict(factor=8.0, original_max_position_embeddings=64)),
+    "llama3.2-tiny": dict(hidden_size=256, num_hidden_layers=2, num_attention_heads=4, num_key_value_heads=2, head_dim=64,
+                          intermediate_size=512, tie_word_embeddings=True,                 # head_dim 64: the RoPE row kernel
+                          rope_scaling=dict(factor=32.0, original_max_position_embeddings=64)),
+    # published meta-llama config.json values (written from the model cards; not re-fetched offline)
+    "llama-3.1-8b": dict(hidden_size=4096, num_hidden_layers=32, num_attention_heads=32, num_key_value_heads=8, head_dim=128,
+                         intermediate_size=14336, tie_word_embeddings=False,
+                         rope_scaling=dict(factor=8.0, original_max_position_embeddings=8192)),
+    "llama-3.2-1b": dict(hidden_size=2048, num_hidden_layers=16, num_attention_heads=32, num_key_value_heads=8, head_dim=64,
+                         intermediate_size=8192, tie_word_embeddings=True,
+                         rope_scaling=dict(factor=32.0, original_max_position_embeddings=8192)),
+    "llama-3.2-3b": dict(hidden_size=3072, num_hidden_layers=28, num_attention_heads=24, num_key_value_heads=8, head_dim=128,
+                         intermediate_size=8192, tie_word_embeddings=True,
+                         rope_scaling=dict(factor=32.0, original_max_position_embeddings=8192)),
+    "llama-3.3-70b": dict(hidden_size=8192, num_hidden_layers=80, num_attention_heads=64, num_key_value_heads=8, head_dim=128,
+                          intermediate_size=28672, tie_word_embeddings=False,
+                          rope_scaling=dict(factor=8.0, original_max_position_embeddings=8192)),
+}
+
+
 QWEN2_SHAPES: Dict[str, Dict] = {
     "qwen2-tiny": dict(hidden_size=896, num_hidden_layers=2, num_attention_heads=14, num_key_value_heads=2,
                        intermediate_size=1152, tie_word_embeddings=True),                  # head_dim 64: un-fused RoPE
@@ -91,6 +117,19 @@ def llama_config(name: str, vocab_size: int = 32000) -> Dict:
         hidden_act="silu", rms_norm_eps=1e-5, rope_theta=10000.0, initializer_range=0.02, bos_token_id=1, eos_token_id=2,
         tie_word_embeddings=False, attention_bias=False, mlp_bias=False, attention_dropout=0.0,
         head_dim=s["hidden_size"] // s["num_attention_heads"], **s,
+    )
+
+
+def llama3_config(name: str, vocab_size: int = 128256) -> Dict:
+    """Llama 3.x (HF LlamaForCausalLM): Llama-2's layer with GQA, rope_theta 5e5 and the llama3 RoPE frequency scaling
+    (low_freq_factor 1, high_freq_factor 4). Token ids follow the synthetic tokenizer (`build_llama3_tokenizer`:
+    <|begin_of_text|> = 0, <|end_of_text|> = 1), not the published 128000 / 128001."""
+    s = dict(LLAMA3_SHAPES[name])
+    rs = dict(rope_type="llama3", low_freq_factor=1.0, high_freq_factor=4.0, **s.pop("rope_scaling"))
+    return dict(
+        architectures=["LlamaForCausalLM"], model_type="llama", vocab_size=vocab_size, max_position_embeddings=131072,
+        hidden_act="silu", rms_norm_eps=1e-5, rope_theta=500000.0, rope_scaling=rs, initializer_range=0.02, bos_token_id=0,
+        eos_token_id=1, attention_bias=False, mlp_bias=False, attention_dropout=0.0, pretraining_tp=1, **s,
     )
 
 
@@ -225,6 +264,46 @@ def build_llama_tokenizer(out_dir: str, vocab_size: int = 32000) -> str:
     return out_dir
 
 
+LLAMA3_SPECIAL = ["<|begin_of_text|>", "<|end_of_text|>", "<|eot_id|>", "<|eom_id|>"]
+# Llama 3's pre-tokenizer split (published tokenizer.json), ahead of the byte-level mapping
+LLAMA3_SPLIT = (r"(?i:'s|'t|'re|'ve|'m|'ll|'d)|[^\r\n\p{L}\p{N}]?\p{L}+|\p{N}{1,3}| ?[^\s\p{L}\p{N}]+[\r\n]*|\s*[\r\n]+|"
+                r"\s+(?!\S)|\s+")
+
+
+def build_llama3_tokenizer(out_dir: str, vocab_size: int = 128256) -> str:
+    """Llama-3-style byte-level BPE trained on the synthetic corpus, saved as a `PreTrainedTokenizerFast` like the published
+    one: the specials <|begin_of_text|> / <|end_of_text|> / <|eot_id|> / <|eom_id|> are ids 0-3, BOS is prepended by a
+    TemplateProcessing post-processor, and tokenizer_config.json carries no add_bos_token / add_eos_token. So setting
+    `add_eos_token = True` (the trainer does, as the reference does) rebuilds the post-processor from those flags, exactly as
+    it does for a real Llama 3 tokenizer under the installed transformers."""
+    from tokenizers import Regex, Tokenizer, decoders, models, pre_tokenizers, processors, trainers
+    from transformers import PreTrainedTokenizerFast
+
+    tok = Tokenizer(models.BPE(ignore_merges=True))
+    tok.pre_tokenizer = pre_tokenizers.Sequence([pre_tokenizers.Split(Regex(LLAMA3_SPLIT), behavior="isolated"),
+                                                 pre_tokenizers.ByteLevel(add_prefix_space=False, use_regex=False)])
+    tok.decoder = decoders.ByteLevel()
+    trainer = trainers.BpeTrainer(vocab_size=min(vocab_size, 6000), special_tokens=LLAMA3_SPECIAL, show_progress=False,
+                                  initial_alphabet=pre_tokenizers.ByteLevel.alphabet())
+    tok.train_from_iterator(_corpus(), trainer)
+    nxt = tok.get_vocab_size()
+    tok.add_special_tokens([f"<|reserved_special_token_{i}|>" for i in range(vocab_size - nxt)])   # fill the embedding table
+    bos = LLAMA3_SPECIAL[0]
+    tok.post_processor = processors.TemplateProcessing(single=f"{bos} $A", pair=f"{bos} $A {bos}:1 $B:1", special_tokens=[(bos, 0)])
+    ft = PreTrainedTokenizerFast(tokenizer_object=tok, bos_token=bos, eos_token=LLAMA3_SPECIAL[1], model_max_length=131072)
+    os.makedirs(out_dir, exist_ok=True)
+    ft.save_pretrained(out_dir)
+    path = os.path.join(out_dir, "tokenizer_config.json")
+    with open(path) as f:
+        tc = json.load(f)
+    for k in ("add_bos_token", "add_eos_token"):
+        tc.pop(k, None)
+    tc["tokenizer_class"] = "PreTrainedTokenizerFast"
+    with open(path, "w") as f:
+        json.dump(tc, f, indent=1)
+    return out_dir
+
+
 QWEN2_SPECIAL = ["<|endoftext|>", "<|im_start|>", "<|im_end|>"]
 
 
@@ -261,6 +340,14 @@ QWEN2_GENERATION = {
 }
 
 
+# Llama 3.x base and Instruct checkpoints both sample (temperature 0.6, top-p 0.9); the Instruct ones stop at <|end_of_text|>,
+# <|eom_id|> or <|eot_id|>. Ids mapped onto the synthetic tokenizer.
+LLAMA3_GENERATION = {
+    "base": dict(bos_token_id=0, eos_token_id=1, do_sample=True, temperature=0.6, top_p=0.9),
+    "instruct": dict(bos_token_id=0, eos_token_id=[1, 3, 2], do_sample=True, temperature=0.6, top_p=0.9),
+}
+
+
 # Qwen3 base checkpoints decode greedily; the hybrid-thinking / Instruct ones sample (temperature 0.6, top-k 20, top-p 0.95)
 # and stop at <|im_end|> or <|endoftext|>. Ids mapped onto the synthetic tokenizer.
 QWEN3_GENERATION = {
@@ -275,7 +362,8 @@ QWEN3_GENERATION = {
 def write_model_dir(out_dir: str, kind: str, name: str, vocab_size: Optional[int] = None, with_weights: bool = True,
                     seed: int = 0, generation_config: Optional[Dict] = None, bias_std: Optional[float] = None,
                     qk_norm_std: Optional[float] = None) -> str:
-    """kind: 'bert' | 'llama' | 'qwen2' | 'qwen3' | 'falcon'. Writes config.json, tokenizer files and (optionally) seeded random-init
+    """kind: 'bert' | 'llama' | 'qwen2' | 'qwen3' | 'falcon' (a Llama 3.x shape of LLAMA3_SHAPES takes kind 'llama' and gets the
+    Llama 3 tokenizer). Writes config.json, tokenizer files and (optionally) seeded random-init
     safetensors in HF parameter naming so both transformers (oracle) and dalm_b200 (product) can load the same directory.
     generation_config: written as generation_config.json when given (e.g. QWEN2_GENERATION["base"]). bias_std: std of the
     random attention biases, qk_norm_std the spread of Qwen3's q / k norm weights around 1 (engine/params.random_state_dict)."""
@@ -283,6 +371,9 @@ def write_model_dir(out_dir: str, kind: str, name: str, vocab_size: Optional[int
     if kind == "bert":
         cfg = bert_config(name, vocab_size or 30522)
         build_bert_tokenizer(out_dir, cfg["vocab_size"])
+    elif kind == "llama" and name in LLAMA3_SHAPES:
+        cfg = llama3_config(name, vocab_size or 128256)
+        build_llama3_tokenizer(out_dir, cfg["vocab_size"])
     elif kind == "llama":
         cfg = llama_config(name, vocab_size or 32000)
         build_llama_tokenizer(out_dir, cfg["vocab_size"])

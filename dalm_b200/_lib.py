@@ -49,6 +49,7 @@ SIGNATURES = {
     "dalm_b200_rmsnorm_fwd": [_P, _P, _P, _L, _P, _I, _I, _F, _P],
     "dalm_b200_rmsnorm_bwd": [_P, _P, _P, _P, _L, _P, _P, _P, _L, _I, _I, _P],
     "dalm_b200_bert_embed": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P],
+    "dalm_b200_roberta_embed": [_P, _P, _P, _P, _I, _P, _P, _I, _I, _I, _I, _I, _P],
     "dalm_b200_embed_gather": [_P, _P, _P, _I, _I, _I, _P],
     "dalm_b200_rope": [_P, _L, _I, _I, _I, _P, _P, _I, _I, _I, _P],
     "dalm_b200_swiglu_fwd": [_P, _L, _P, _L, _I, _I, _I, _P],
@@ -67,7 +68,7 @@ SIGNATURES = {
     "dalm_b200_cast_f32_bf16": [_P, _L, _P, _L, _I, _I, _P],
     "dalm_b200_adam_step": [_P, _P, _P, _P, _L, _F, _F, _F, _F, _I, _F, _P],
     "dalm_b200_col_reduce": [_P, _P, _L, _P, _P, _P, _P, _P, _I, _I, _P],
-    "dalm_b200_embed_scatter_add": [_P, _P, _P, _P, _I, _I, _I, _I, _P],
+    "dalm_b200_embed_scatter_add": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P],
     "dalm_b200_masked_add": [_P, _P, _L, _P, _I, _I, *_DROP, _P],
     "dalm_b200_adam_step_shadow": [_P, _P, _P, _P, _P, _L, _F, _F, _F, _F, _I, _F, _P],
     "dalm_b200_topk_ip_workspace": [_I, _I],

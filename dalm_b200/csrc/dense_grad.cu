@@ -55,19 +55,26 @@ __global__ void __launch_bounds__(256) col_reduce_kernel(const float* __restrict
   }
 }
 
-// dword[ids[m], :] += d[m, :] ;  dpos[m % L, :] += d[m, :]  (dpos optional). One CTA per token row, float4 reads, fp32 atomics.
+// dword[ids[m], :] += d[m, :] ;  dpos[pos_ids ? pos_ids[m] : m % L, :] += d[m, :]  (dpos optional). With pad >= 0, tokens whose
+// id is pad add nothing to dword and positions equal to pad add nothing to dpos (nn.Embedding padding_idx). One CTA per token
+// row, float4 reads, fp32 atomics.
 __global__ void __launch_bounds__(256) embed_scatter_kernel(const float* __restrict__ d, const long long* __restrict__ ids,
-                                                            float* __restrict__ dword, float* __restrict__ dpos, int M, int H,
-                                                            int L, int V) {
+                                                            const long long* __restrict__ pos_ids, float* __restrict__ dword,
+                                                            float* __restrict__ dpos, int M, int H, int L, int V, long long pad) {
   const int m = blockIdx.x;
-  long long id = ids[m];
-  if (id < 0 || id >= V) id = 0;                                      // the forward gathers read row 0 for any out-of-range id
+  const long long raw = ids[m];
+  const long long id = (raw < 0 || raw >= V) ? 0 : raw;               // the forward gathers read row 0 for any out-of-range id
   const float* src = d + (size_t)m * H;
-  float* w = dword + (size_t)id * H;
-  float* pp = dpos ? dpos + (size_t)(m % L) * H : nullptr;
+  float* w = (pad >= 0 && raw == pad) ? nullptr : dword + (size_t)id * H;
+  float* pp = nullptr;
+  if (dpos) {
+    const long long p = pos_ids ? pos_ids[m] : m % L;
+    if (pad < 0 || p != pad) pp = dpos + (size_t)p * H;
+  }
+  if (!w && !pp) return;
   for (int i = threadIdx.x * 4; i < H; i += blockDim.x * 4) {
     const float4 v = *reinterpret_cast<const float4*>(src + i);
-    atomicAdd(w + i, v.x); atomicAdd(w + i + 1, v.y); atomicAdd(w + i + 2, v.z); atomicAdd(w + i + 3, v.w);
+    if (w) { atomicAdd(w + i, v.x); atomicAdd(w + i + 1, v.y); atomicAdd(w + i + 2, v.z); atomicAdd(w + i + 3, v.w); }
     if (pp) { atomicAdd(pp + i, v.x); atomicAdd(pp + i + 1, v.y); atomicAdd(pp + i + 2, v.z); atomicAdd(pp + i + 3, v.w); }
   }
 }
@@ -156,11 +163,13 @@ extern "C" int dalm_b200_col_reduce(const float* dy_f32, const void* dy_bf16, lo
   return check_launch("col_reduce_kernel");
 }
 
-extern "C" int dalm_b200_embed_scatter_add(const float* d, const int64_t* ids, float* dword, float* dpos, int M, int H, int L,
-                                           int V, void* stream) {
-  DALM_REQUIRE(M > 0 && (H % 4) == 0 && L > 0 && V > 0, "embed_scatter_add: bad shape M=%d H=%d L=%d V=%d", M, H, L, V);
+extern "C" int dalm_b200_embed_scatter_add(const float* d, const int64_t* ids, const int64_t* pos_ids, float* dword, float* dpos,
+                                           int M, int H, int L, int V, int pad_id, void* stream) {
+  DALM_REQUIRE(M > 0 && (H % 4) == 0 && L > 0 && V > 0 && pad_id >= -1, "embed_scatter_add: bad shape M=%d H=%d L=%d V=%d pad_id=%d",
+               M, H, L, V, pad_id);
   DALM_REQUIRE(aligned(d, 16), "embed_scatter_add: d must be 16-byte aligned");
-  embed_scatter_kernel<<<M, 256, 0, ST(stream)>>>(d, (const long long*)ids, dword, dpos, M, H, L, V);
+  embed_scatter_kernel<<<M, 256, 0, ST(stream)>>>(d, (const long long*)ids, (const long long*)pos_ids, dword, dpos, M, H, L, V,
+                                                  pad_id);
   count_launch();
   return check_launch("embed_scatter_kernel");
 }

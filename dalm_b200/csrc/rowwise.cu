@@ -281,6 +281,53 @@ __global__ void bert_embed_kernel(const int64_t* __restrict__ ids, const __nv_bf
     z[r * H + i] = __bfloat162float(word[(size_t)id * H + i]) + __bfloat162float(pos[(size_t)l * H + i]) +
                    __bfloat162float(type0[i]);
 }
+// RoBERTa / XLM-RoBERTa: the position comes from the ids (HF create_position_ids_from_input_ids), not the column:
+// pos = pad + (id != pad) * (number of non-pad ids in columns 0..l of the row), clamped into [0, P) as a guard. One CTA per
+// (row, chunk of 32 columns), so the grid scales with B*L: the CTA counts the row's non-pad ids before its chunk, one warp
+// ballot ranks the chunk, then z = word[id] + pos[position] + type[0] in bert_embed's order of additions. Position ids of the
+// chunk go to pos_ids (may be NULL) for the backward's scatter.
+constexpr int kReChunk = 32;
+__global__ void __launch_bounds__(256) roberta_embed_kernel(const int64_t* __restrict__ ids, const __nv_bfloat16* __restrict__ word,
+                                                            const __nv_bfloat16* __restrict__ pos,
+                                                            const __nv_bfloat16* __restrict__ type0, long long pad,
+                                                            float* __restrict__ z, int64_t* __restrict__ pos_ids, int L, int H,
+                                                            int V, int P) {
+  __shared__ int red[32];
+  __shared__ long long s_pos[kReChunk];
+  const int c0 = blockIdx.x * kReChunk;
+  const int64_t* row = ids + (size_t)blockIdx.y * L;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  int cnt = 0;
+  for (int l = threadIdx.x; l < c0; l += blockDim.x) cnt += row[l] != pad;
+  cnt = __reduce_add_sync(0xffffffffu, cnt);
+  if (lane == 0) red[warp] = cnt;
+  __syncthreads();
+  if (warp == 0) {
+    const int before = __reduce_add_sync(0xffffffffu, lane < (int)(blockDim.x >> 5) ? red[lane] : 0);
+    const int l = c0 + lane;
+    const bool tok = l < L && row[l] != pad;
+    const unsigned bal = __ballot_sync(0xffffffffu, tok);
+    long long p = tok ? pad + before + __popc(bal & (0xffffffffu >> (31 - lane))) : pad;
+    p = p < 0 ? 0 : (p >= P ? P - 1 : p);
+    s_pos[lane] = p;
+    if (pos_ids && l < L) pos_ids[(size_t)blockIdx.y * L + l] = p;
+  }
+  __syncthreads();
+  const int n = min(kReChunk, L - c0), H4 = H >> 2;
+  for (int e = threadIdx.x; e < n * H4; e += blockDim.x) {           // 4 columns per thread: 8-byte bf16 reads, float4 store
+    const int t = e / H4, c = (e - t * H4) * 4;
+    int64_t id = row[c0 + t];
+    if (id < 0 || id >= V) id = 0;
+    const uint2 w = *reinterpret_cast<const uint2*>(word + (size_t)id * H + c);
+    const uint2 q = *reinterpret_cast<const uint2*>(pos + (size_t)s_pos[t] * H + c);
+    const uint2 y = *reinterpret_cast<const uint2*>(type0 + c);
+    const float2 w0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w.x)), w1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w.y));
+    const float2 q0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&q.x)), q1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&q.y));
+    const float2 y0 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&y.x)), y1 = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&y.y));
+    *reinterpret_cast<float4*>(z + ((size_t)blockIdx.y * L + c0 + t) * H + c) =
+        make_float4(w0.x + q0.x + y0.x, w0.y + q0.y + y0.y, w1.x + q1.x + y1.x, w1.y + q1.y + y1.y);
+  }
+}
 // decoder: x[r,:] = table[id,:] (bf16 -> fp32 residual stream)
 __global__ void embed_gather_kernel(const int64_t* __restrict__ ids, const __nv_bfloat16* __restrict__ table,
                                     float* __restrict__ x, int H, int V) {
@@ -899,6 +946,17 @@ extern "C" int dalm_b200_bert_embed(const int64_t* ids, const void* word, const 
                                                (const __nv_bfloat16*)type0, z, L, H, V);
   count_launch();
   return check_launch("bert_embed_kernel");
+}
+extern "C" int dalm_b200_roberta_embed(const int64_t* ids, const void* word, const void* pos, const void* type0, int pad_id,
+                                       float* z, int64_t* pos_ids_out, int B, int L, int H, int V, int P, void* stream) {
+  DALM_REQUIRE(B > 0 && B <= 65535 && L > 0 && V > 0 && P > 0 && H > 0 && (H % 4) == 0 && pad_id >= 0,
+               "roberta_embed: bad shape B=%d L=%d H=%d V=%d P=%d pad_id=%d", B, L, H, V, P, pad_id);
+  DALM_REQUIRE(aligned(word, 8) && aligned(pos, 8) && aligned(type0, 8) && aligned(z, 16),
+               "roberta_embed: tables must be 8-byte and z 16-byte aligned");
+  roberta_embed_kernel<<<dim3((L + kReChunk - 1) / kReChunk, B), 256, 0, ST(stream)>>>(
+      ids, (const __nv_bfloat16*)word, (const __nv_bfloat16*)pos, (const __nv_bfloat16*)type0, pad_id, z, pos_ids_out, L, H, V, P);
+  count_launch();
+  return check_launch("roberta_embed_kernel");
 }
 extern "C" int dalm_b200_embed_gather(const int64_t* ids, const void* table, float* x, int M, int H, int V, void* stream) {
   embed_gather_kernel<<<M, 256, 0, ST(stream)>>>(ids, (const __nv_bfloat16*)table, x, H, V);

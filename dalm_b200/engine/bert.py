@@ -1,4 +1,7 @@
-"""BERT encoder (bge-small / bge-large shapes) forward + backward as a launch sequence over the C-ABI kernels.
+"""BERT encoder (bge-small / bge-large shapes) forward + backward as a launch sequence over the C-ABI kernels. The same class
+serves RoBERTa / XLM-RoBERTa encoders (multilingual-e5, bge-m3): identical layers and parameter names; their embeddings take
+positions from the ids (pad + running count of non-pad tokens, HF create_position_ids_from_input_ids) instead of the column,
+and the padding_idx rows of the word and position tables receive no gradient.
 
 Mirrors what `self.retriever_model(input_ids, attention_mask)[0]` computes in the reference
 (dalm/models/rag_e2e_base_model.py:93, dalm/models/retriever_only_base_model.py:58) through HF BertModel:
@@ -21,10 +24,25 @@ from typing import Dict, List, Optional
 import torch
 
 from .. import ops
+from . import params
 from .dense import DenseBank
 from .lora import LoraBank
 
 bf16, f32 = torch.bfloat16, torch.float32
+
+
+def _hf_names(sd: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+    """checkpoint names relative to the encoder: the `bert.` / `roberta.` prefix of *ForMaskedLM-style checkpoints stripped,
+    their masked-LM head (`lm_head.*`) left out"""
+    out = {}
+    for k, v in sd.items():
+        for pre in ("bert.", "roberta."):
+            if k.startswith(pre):
+                k = k[len(pre):]
+                break
+        if not k.startswith("lm_head."):
+            out[k] = v
+    return out
 
 
 def _aug_buf(rows: int, cols: int, ra: int, device, zero: bool = False) -> torch.Tensor:
@@ -66,11 +84,16 @@ class BertEncoder(torch.nn.Module):
         self.V = cfg["vocab_size"]
         self.eps = float(cfg.get("layer_norm_eps", 1e-12))
         self.dev = torch.device(device)
+        self.roberta = cfg.get("model_type") in ("roberta", "xlm-roberta")
+        if self.roberta:
+            params.check_roberta(cfg)
+            self.pad = int(cfg.get("pad_token_id", 1))
+            self.max_len = params.roberta_max_len(cfg)
         if self.hd not in (32, 64, 128):
             raise NotImplementedError(f"head_dim {self.hd} not supported by the attention kernels")
         self.r = 8
         self.Ra = 3 * self.r if lora else 0
-        sd = {k[len("bert."):] if k.startswith("bert.") else k: v for k, v in state_dict.items()}
+        sd = _hf_names(state_dict)
         if self.nf4 is not None:                              # everything that is not an nn.Linear weight: transformers' fp16 cast
             g = lambda k, dt: sd[k].to(device=self.dev, dtype=torch.float16).to(dt).contiguous()
         else:
@@ -166,7 +189,8 @@ class BertEncoder(torch.nn.Module):
                                 "bo2": bank.w32(k("bo2")), "ln2_g": bank.w32(k("ln2_g")), "ln2_b": bank.w32(k("ln2_b"))})
 
     def hf_state_dict(self) -> Dict[str, torch.Tensor]:
-        """fp32 CPU tensors under HF BertModel names (save_pretrained of a fully fine-tuned encoder)"""
+        """fp32 CPU tensors under HF BertModel / XLMRobertaModel names (save_pretrained of a fully fine-tuned encoder); the pooler
+        only when the checkpoint had one"""
         if self.full is None:
             raise RuntimeError("hf_state_dict: only fully fine-tuned models own their weights (PEFT mode saves adapters)")
         out = {}
@@ -179,7 +203,7 @@ class BertEncoder(torch.nn.Module):
         return out
 
     def load_hf_state_dict(self, sd: Dict[str, torch.Tensor]) -> None:
-        sd = {k[len("bert."):] if k.startswith("bert.") else k: v for k, v in sd.items()}
+        sd = _hf_names(sd)
         for key, parts in self._rows.items():
             w, r = self.full.w32(key), 0
             for name, rows in parts:
@@ -331,6 +355,12 @@ class BertEncoder(torch.nn.Module):
         rows (M = sum B_i L_i: bigger, better-filled tensor-core tiles, half the launches); only attention is launched
         per segment. Returns ([hidden_i fp32 [B_i,L_i,H]], ctx)."""
         H, F, Ra = self.H, self.F, self.Ra
+        if self.roberta:
+            for ids, _ in segments:
+                if ids.shape[1] > self.max_len:
+                    raise ValueError(f"sequence length {ids.shape[1]} exceeds the {self.max_len} positions this encoder's table "
+                                     f"serves (max_position_embeddings {self.cfg['max_position_embeddings']} - pad_token_id "
+                                     f"{self.pad} - 1)")
         ctx = _Ctx()
         ctx.segs = []
         r0 = 0
@@ -344,14 +374,20 @@ class BertEncoder(torch.nn.Module):
         ctx.call = call = self._call
         ctx.training = self.training
         z = torch.empty(M, H, dtype=f32, device=self.dev)
+        pos_ids = torch.empty(M, dtype=torch.int64, device=self.dev) if self.roberta else None
         for (ids, _), (B, L, _, s0) in zip(segments, ctx.segs):
-            ops.bert_embed(ids, self.word, self.pos, self.type0, out=z[s0:s0 + B * L])
+            if self.roberta:
+                ops.roberta_embed(ids, self.word, self.pos, self.type0, self.pad, out=z[s0:s0 + B * L],
+                                  pos_ids=pos_ids[s0:s0 + B * L])
+            else:
+                ops.bert_embed(ids, self.word, self.pos, self.type0, out=z[s0:s0 + B * L])
         x_aug = _aug_buf(M, H, Ra, self.dev)
         x32, _, mean, rstd = ops.layernorm_fwd(z, self.emb_g, self.emb_b, self.eps, y16=x_aug[:, :H],
                                                drop=self._drop(self.p_hidden, call, 255, 0))
         if save and self.full is not None:                     # the embedding tables are trainable: keep their LN state
             ctx.z_emb, ctx.mean_e, ctx.rstd_e = z, mean, rstd
             ctx.ids = [ids.contiguous() for ids, _ in segments]
+            ctx.pos_ids = pos_ids
         for li, W in enumerate(self.layers):
             a = _Ctx()
             a.x_aug = x_aug
@@ -501,5 +537,9 @@ class BertEncoder(torch.nn.Module):
         ops.col_reduce_(dy_f32=g, z=ctx.z_emb, mean=ctx.mean_e, rstd=ctx.rstd_e, out_sum=bank.g("emb_b"), out_prod=bank.g("emb_g"))
         dz, _ = ops.layernorm_bwd(ctx.z_emb, self.emb_g, ctx.mean_e, ctx.rstd_e, dy_f32=g, want_bf16=False)
         for ids, (B, L, _, s0) in zip(ctx.ids, ctx.segs):
-            ops.embed_scatter_add_(dz[s0:s0 + B * L], ids, bank.g("word"), bank.g("pos"), L)
+            if self.roberta:                                              # positions of the forward; padding_idx rows get nothing
+                ops.embed_scatter_add_(dz[s0:s0 + B * L], ids, bank.g("word"), bank.g("pos"), L,
+                                       pos_ids=ctx.pos_ids[s0:s0 + B * L], pad_id=self.pad)
+            else:
+                ops.embed_scatter_add_(dz[s0:s0 + B * L], ids, bank.g("word"), bank.g("pos"), L)
         ops.col_reduce_(dy_f32=dz, out_sum=bank.g("type")[0])                 # token_type_ids are all zero (reference quirk 7)

@@ -21,8 +21,8 @@ def _normal(gen: torch.Generator, shape, std: float, dtype, device) -> torch.Ten
 
 def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, device="cpu",
                       bias_std: Optional[float] = None, qk_norm_std: Optional[float] = None) -> Dict[str, torch.Tensor]:
-    """HF parameter names for BertModel (no prefix) / LlamaForCausalLM / Qwen2ForCausalLM / Qwen3ForCausalLM /
-    FalconForCausalLM, init N(0, initializer_range), LN = (1, 0). Decoder attention biases (Qwen2's q/k/v, Llama's and Qwen3's
+    """HF parameter names for BertModel / XLMRobertaModel / RobertaModel (no prefix) / LlamaForCausalLM / Qwen2ForCausalLM /
+    Qwen3ForCausalLM / FalconForCausalLM, init N(0, initializer_range), LN = (1, 0). Decoder attention biases (Qwen2's q/k/v, Llama's and Qwen3's
     `attention_bias`) are drawn from N(0, bias_std) (default: initializer_range) rather than HF's zeros, so that a dropped bias
     changes the outputs. Qwen3's q_norm / k_norm weights are 1 + N(0, qk_norm_std) (default: initializer_range), so that a
     dropped or swapped norm shows."""
@@ -34,7 +34,7 @@ def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, 
     sd: Dict[str, torch.Tensor] = {}
     ones = lambda n: torch.ones(n, dtype=dtype, device=device)
     zeros = lambda n: torch.zeros(n, dtype=dtype, device=device)
-    if kind == "bert":
+    if kind in ("bert", "roberta"):                              # RoBERTa / XLM-R keep BertModel's parameter names and shapes
         F, V = cfg["intermediate_size"], cfg["vocab_size"]
         sd["embeddings.word_embeddings.weight"] = _normal(gen, (V, H), std, dtype, device)
         sd["embeddings.position_embeddings.weight"] = _normal(gen, (cfg["max_position_embeddings"], H), std, dtype, device)
@@ -152,6 +152,9 @@ def model_kind(cfg: Dict) -> str:
     mt = cfg.get("model_type", "")
     if mt == "bert":
         return "bert"
+    if mt in ("roberta", "xlm-roberta"):
+        check_roberta(cfg)
+        return "roberta"
     if mt in ("llama", "qwen2", "qwen3"):
         check_llama_family(cfg)
         return mt
@@ -159,7 +162,7 @@ def model_kind(cfg: Dict) -> str:
         check_rope_type(cfg)
         return "falcon"
     raise NotImplementedError(
-        f"model_type {mt!r} is not built in dalm_b200 (supported: bert encoders; llama, qwen2, qwen3 and falcon decoders)")
+        f"model_type {mt!r} is not built in dalm_b200 (supported: bert, roberta and xlm-roberta encoders; llama, qwen2, qwen3 and falcon decoders)")
 
 
 def _rope_type(cfg: Dict) -> str:
@@ -241,6 +244,27 @@ def check_llama_family(cfg: Dict) -> None:
         rt = _rope_type(cfg)
         if rt != "default":
             raise NotImplementedError(f"{mt}: RoPE type {rt!r} (rope_scaling / rope_parameters) is not built; only 'default'")
+
+
+def check_roberta(cfg: Dict) -> None:
+    """refuses the settings of a roberta / xlm-roberta config that BertEncoder would otherwise silently compute wrong"""
+    mt = cfg.get("model_type", "")
+    pet = cfg.get("position_embedding_type", "absolute")
+    if pet != "absolute":
+        raise NotImplementedError(f"{mt}: position_embedding_type={pet!r} is not built; only 'absolute'")
+    act = cfg.get("hidden_act", "gelu")
+    if act != "gelu":
+        raise NotImplementedError(f"{mt}: hidden_act={act!r} is not built; only 'gelu' (erf)")
+    if cfg.get("is_decoder", False):
+        raise NotImplementedError(f"{mt}: is_decoder=true (causal self-attention) is not built")
+    if cfg.get("add_cross_attention", False):
+        raise NotImplementedError(f"{mt}: add_cross_attention=true is not built")
+
+
+def roberta_max_len(cfg: Dict) -> int:
+    """the longest sequence a roberta / xlm-roberta position table serves: positions run from pad_token_id + 1, so
+    max_position_embeddings - pad_token_id - 1 (512 for the 514-row tables, 8192 for bge-m3's 8194)"""
+    return int(cfg["max_position_embeddings"]) - int(cfg.get("pad_token_id", 1)) - 1
 
 
 def attention_biases(kind: str, cfg: Dict):

@@ -65,7 +65,7 @@ def load_tokenizer(name_or_path: str):
 
 def build_encoder(name_or_path: str, lora: bool, device: torch.device, state_dict: Optional[Dict] = None,
                   cfg: Optional[Dict] = None, autoregressive: bool = False, full: bool = False, bnb: bool = False):
-    """BERT-family encoder (bge-*), or — `retriever_is_autoregressive` — a Llama / Qwen2 / Qwen3 decoder used as an encoder
+    """BERT-family encoder (bge-*) or (XLM-)RoBERTa encoder (multilingual-e5, bge-m3, xlm-roberta-*), or — `retriever_is_autoregressive` — a Llama / Qwen2 / Qwen3 decoder used as an encoder
     (last hidden state, eos pooling; LoRA targets q_proj / v_proj: reference rag_e2e_base_model.py:66-70,84-90)"""
     cfg = cfg or params.load_config(name_or_path)
     kind = params.model_kind(cfg)
@@ -77,9 +77,9 @@ def build_encoder(name_or_path: str, lora: bool, device: torch.device, state_dic
         if kind not in ("llama", "qwen2", "qwen3"):
             raise NotImplementedError("autoregressive retrievers are built for Llama, Qwen2 and Qwen3 models only")
         return _named(LlamaDecoder(cfg, sd, device=device, lora=lora, lora_seed=0, full=full, nf4_storage=nf4), name_or_path)
-    if kind != "bert":
-        raise NotImplementedError("non-autoregressive retrievers must be BERT-family encoders (bge-*); pass "
-                                  "retriever_is_autoregressive=True for a causal LM")
+    if kind not in ("bert", "roberta"):
+        raise NotImplementedError("non-autoregressive retrievers must be BERT (bge-*) or (XLM-)RoBERTa (multilingual-e5, bge-m3) "
+                                  "encoders; pass retriever_is_autoregressive=True for a causal LM")
     return _named(BertEncoder(cfg, sd, device=device, lora=lora, full=full, nf4_storage=nf4), name_or_path)
 
 
@@ -91,14 +91,15 @@ def _named(engine_model, name_or_path: str):
 
 def _nf4_storage(bnb: bool, full: bool, kind: str) -> bool:
     """use_bnb + DALM_B200_NF4_STORAGE=1: keep the sub-model's Linear weights as packed NF4 codes and expand them per use
-    (engine/nf4store.py) instead of the dequantised-resident default. BERT encoders and Llama decoders."""
+    (engine/nf4store.py) instead of the dequantised-resident default. BERT / (XLM-)RoBERTa encoders and Llama decoders."""
     from ..engine.nf4store import storage_enabled
     if not bnb or not storage_enabled():
         return False
     if full:
         _maybe_bnb({}, True, True, None)                      # raises: 4-bit base weights cannot be fully fine-tuned
-    if kind not in ("bert", "llama"):
-        raise NotImplementedError(f"DALM_B200_NF4_STORAGE=1: 4-bit storage is built for BERT encoders and Llama decoders, not {kind!r}")
+    if kind not in ("bert", "roberta", "llama"):
+        raise NotImplementedError(f"DALM_B200_NF4_STORAGE=1: 4-bit storage is built for BERT / (XLM-)RoBERTa encoders and Llama "
+                                  f"decoders, not {kind!r}")
     return True
 
 

@@ -440,6 +440,27 @@ def bert_embed(ids, word, pos, type_emb, out=None):
     return z
 
 
+def roberta_embed(ids, word, pos, type_emb, pad_id: int, out=None, pos_ids=None):
+    """RoBERTa / XLM-RoBERTa embeddings: positions from the ids (HF create_position_ids_from_input_ids with padding_idx =
+    pad_id), computed on the device. Returns (z fp32 [B*L, H], position ids int64 [B*L]). Positions past the table are clamped
+    by the kernel; callers check L against the table first."""
+    B, L = ids.shape
+    V, H = word.shape
+    _rows32(out, "roberta_embed out", H, B * L)
+    _tables16(("roberta_embed word", word), ("roberta_embed pos", pos), ("roberta_embed type", type_emb))
+    if pos.shape[1] != H or type_emb.numel() != H:
+        raise _lib.DalmB200Error(f"roberta_embed: tables must be {H} wide (pos {tuple(pos.shape)}, type {tuple(type_emb.shape)})")
+    z = torch.empty(B * L, H, dtype=f32, device=ids.device) if out is None else out
+    if pos_ids is None:
+        pos_ids = torch.empty(B * L, dtype=i64, device=ids.device)
+    _chk(pos_ids, i64, "roberta_embed pos_ids")
+    if pos_ids.numel() != B * L or not pos_ids.is_contiguous():
+        raise _lib.DalmB200Error(f"roberta_embed: pos_ids must be a dense int64 [{B * L}]")
+    _lib.call("dalm_b200_roberta_embed", _p(ids.contiguous()), _p(word), _p(pos), _p(type_emb), int(pad_id), _p(z), _p(pos_ids),
+              B, L, H, V, pos.shape[0], _stream())
+    return z, pos_ids
+
+
 def embed_gather(ids, table):
     M = ids.numel()
     V, H = table.shape
@@ -743,13 +764,20 @@ def col_reduce_(dy_f32=None, dy_bf16=None, z=None, mean=None, rstd=None, out_sum
               _p(rstd), _p(out_sum), _p(out_prod), M, H, _stream())
 
 
-def embed_scatter_add_(d, ids, dword, dpos=None, L: int = 1) -> None:
+def embed_scatter_add_(d, ids, dword, dpos=None, L: int = 1, *, pos_ids=None, pad_id: int = -1) -> None:
+    """pos_ids: int64 [M] positions to scatter into dpos (roberta_embed's output; None: m % L). pad_id >= 0: that word row and
+    that position row receive no gradient (nn.Embedding padding_idx); -1: none"""
     M, H = d.shape
     _rows32(d, "embed_scatter_add d", H); _rows32(dword, "embed_scatter_add dword", H); _rows32(dpos, "embed_scatter_add dpos", H)
     _chk(ids, i64, "embed_scatter_add ids")
     if ids.numel() != M or not ids.is_contiguous():
         raise _lib.DalmB200Error(f"embed_scatter_add: need one contiguous id per row ({ids.numel()} for {M} rows)")
-    _lib.call("dalm_b200_embed_scatter_add", _p(d), _p(ids), _p(dword), _p(dpos), M, H, int(L), dword.shape[0], _stream())
+    if pos_ids is not None:
+        _chk(pos_ids, i64, "embed_scatter_add pos_ids")
+        if pos_ids.numel() != M or not pos_ids.is_contiguous():
+            raise _lib.DalmB200Error(f"embed_scatter_add: need one contiguous position per row ({pos_ids.numel()} for {M} rows)")
+    _lib.call("dalm_b200_embed_scatter_add", _p(d), _p(ids), _p(pos_ids), _p(dword), _p(dpos), M, H, int(L), dword.shape[0],
+              int(pad_id), _stream())
 
 
 def masked_add(a=None, b=None, drop: Optional[Drop] = None, out=None):

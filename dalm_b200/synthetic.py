@@ -84,6 +84,19 @@ QWEN3_SHAPES: Dict[str, Dict] = {
 }
 
 
+# XLM-RoBERTa / RoBERTa encoders: BERT's layer, positions counted from pad_token_id + 1
+ROBERTA_SHAPES: Dict[str, Dict] = {
+    "xlmr-tiny": dict(hidden_size=64, num_hidden_layers=2, num_attention_heads=2, intermediate_size=128),      # head_dim 32: mma.sync attention
+    "xlmr-hd64": dict(hidden_size=128, num_hidden_layers=2, num_attention_heads=2, intermediate_size=256),     # head_dim 64: wgmma attention
+    "roberta-tiny": dict(hidden_size=64, num_hidden_layers=2, num_attention_heads=2, intermediate_size=128, model_type="roberta"),
+    # published config.json values (written from the model cards; not re-fetched offline)
+    "multilingual-e5-base": dict(hidden_size=768, num_hidden_layers=12, num_attention_heads=12, intermediate_size=3072),
+    "xlm-roberta-base": dict(hidden_size=768, num_hidden_layers=12, num_attention_heads=12, intermediate_size=3072),
+    "bge-m3": dict(hidden_size=1024, num_hidden_layers=24, num_attention_heads=16, intermediate_size=4096,
+                   max_position_embeddings=8194),
+}
+
+
 FALCON_SHAPES: Dict[str, Dict] = {
     "falcon-tiny": dict(hidden_size=128, num_hidden_layers=2, num_attention_heads=2),
     "falcon-mini": dict(hidden_size=448, num_hidden_layers=2, num_attention_heads=7),          # 7 q heads x 64, one KV head
@@ -108,6 +121,26 @@ def bert_config(name: str, vocab_size: int = 30522) -> Dict:
         type_vocab_size=2, hidden_act="gelu", layer_norm_eps=1e-12, hidden_dropout_prob=0.1,
         attention_probs_dropout_prob=0.1, initializer_range=0.02, pad_token_id=0, position_embedding_type="absolute", **s,
     )
+
+
+def roberta_config(name: str, vocab_size: Optional[int] = None) -> Dict:
+    """XLM-RoBERTa (HF XLMRobertaModel, model_type "xlm-roberta", vocab 250002) or, for `roberta-tiny`, RoBERTa (model_type
+    "roberta", vocab 50265): BERT's layers with layer_norm_eps 1e-5, one token type, pad_token_id 1 and a position table of
+    max_position_embeddings = usable length + 2 (514; bge-m3 8194), since positions start at pad_token_id + 1. The published
+    shapes (multilingual-e5-base, xlm-roberta-base, bge-m3) were written from their config.json files and could not be re-checked
+    offline. multilingual-e5-small is not among them: it is published as a `bert` config (Multilingual-MiniLM) with an
+    XLM-R tokenizer, so it already runs as a BERT encoder."""
+    s = dict(ROBERTA_SHAPES[name])
+    mt = s.pop("model_type", "xlm-roberta")
+    arch = "RobertaModel" if mt == "roberta" else "XLMRobertaModel"
+    cfg = dict(
+        architectures=[arch], model_type=mt, vocab_size=vocab_size or (50265 if mt == "roberta" else 250002),
+        max_position_embeddings=514, type_vocab_size=1, hidden_act="gelu", layer_norm_eps=1e-5, hidden_dropout_prob=0.1,
+        attention_probs_dropout_prob=0.1, initializer_range=0.02, pad_token_id=1, bos_token_id=0, eos_token_id=2,
+        position_embedding_type="absolute", use_cache=True, classifier_dropout=None,
+    )
+    cfg.update(s)
+    return cfg
 
 
 def llama_config(name: str, vocab_size: int = 32000) -> Dict:
@@ -239,6 +272,54 @@ def build_bert_tokenizer(out_dir: str, vocab_size: int = 30522) -> str:
     return out_dir
 
 
+ROBERTA_SPECIAL = ["<s>", "<pad>", "</s>", "<unk>"]          # ids 0-3 as in XLM-R and RoBERTa; <mask> is the last id
+
+
+def build_xlmr_tokenizer(out_dir: str, vocab_size: int = 250002, model_max_length: int = 512) -> str:
+    """XLM-R-style Unigram (Metaspace) trained on the synthetic corpus, wrapped in transformers' XLMRobertaTokenizerFast:
+    <s> / <pad> / </s> / <unk> = 0-3, <mask> last, `<s> $A </s>` framing, no token_type_ids"""
+    from tokenizers import Tokenizer, models, pre_tokenizers, trainers
+    from transformers import XLMRobertaTokenizerFast
+
+    tok = Tokenizer(models.Unigram())
+    tok.pre_tokenizer = pre_tokenizers.Metaspace(replacement="▁", prepend_scheme="always")
+    trainer = trainers.UnigramTrainer(vocab_size=min(vocab_size - 1, 8000), special_tokens=ROBERTA_SPECIAL, unk_token="<unk>",
+                                      show_progress=False)
+    tok.train_from_iterator(_corpus(), trainer)
+    pieces = [tuple(v) for v in json.loads(tok.to_str())["model"]["vocab"]]
+    pieces += [(f"<extra_{i}>", -1e4) for i in range(len(pieces), vocab_size - 1)]   # ids span the real embedding table
+    pieces.append(("<mask>", 0.0))
+    xt = XLMRobertaTokenizerFast(vocab=pieces, model_max_length=model_max_length)
+    os.makedirs(out_dir, exist_ok=True)
+    xt.save_pretrained(out_dir)
+    return out_dir
+
+
+def build_roberta_tokenizer(out_dir: str, vocab_size: int = 50265, model_max_length: int = 512) -> str:
+    """RoBERTa-style byte-level BPE trained on the synthetic corpus, wrapped in transformers' RobertaTokenizer (the fast,
+    tokenizers-backed class): the same special ids and framing as build_xlmr_tokenizer"""
+    from tokenizers import Tokenizer, models, pre_tokenizers, trainers
+    from transformers import RobertaTokenizer
+
+    tok = Tokenizer(models.BPE())
+    tok.pre_tokenizer = pre_tokenizers.ByteLevel(add_prefix_space=False)
+    trainer = trainers.BpeTrainer(vocab_size=min(vocab_size - 1, 6000), special_tokens=ROBERTA_SPECIAL, show_progress=False,
+                                  initial_alphabet=pre_tokenizers.ByteLevel.alphabet())
+    tok.train_from_iterator(_corpus(), trainer)
+    vocab = tok.get_vocab()
+    model_json = json.loads(tok.to_str())["model"]
+    merges = [tuple(m) if isinstance(m, list) else tuple(m.split(" ")) for m in model_json["merges"]]
+    nxt = len(vocab)
+    while nxt < vocab_size - 1:
+        vocab[f"<extra_{nxt}>"] = nxt
+        nxt += 1
+    vocab["<mask>"] = nxt
+    rt = RobertaTokenizer(vocab=vocab, merges=merges, model_max_length=model_max_length)
+    os.makedirs(out_dir, exist_ok=True)
+    rt.save_pretrained(out_dir)
+    return out_dir
+
+
 def build_llama_tokenizer(out_dir: str, vocab_size: int = 32000) -> str:
     """Llama-style BPE (metaspace, byte fallback, <unk>/<s>/</s> = 0/1/2) wrapped in transformers' LlamaTokenizer so that
     `add_eos_token = True` (reference train_rage2e.py:304) behaves as it does for the real Llama-2 tokenizer."""
@@ -362,7 +443,8 @@ QWEN3_GENERATION = {
 def write_model_dir(out_dir: str, kind: str, name: str, vocab_size: Optional[int] = None, with_weights: bool = True,
                     seed: int = 0, generation_config: Optional[Dict] = None, bias_std: Optional[float] = None,
                     qk_norm_std: Optional[float] = None) -> str:
-    """kind: 'bert' | 'llama' | 'qwen2' | 'qwen3' | 'falcon' (a Llama 3.x shape of LLAMA3_SHAPES takes kind 'llama' and gets the
+    """kind: 'bert' | 'roberta' | 'llama' | 'qwen2' | 'qwen3' | 'falcon' ('roberta' takes a ROBERTA_SHAPES name: XLM-R shapes get
+    the XLM-R tokenizer, roberta-tiny the byte-level one; a Llama 3.x shape of LLAMA3_SHAPES takes kind 'llama' and gets the
     Llama 3 tokenizer). Writes config.json, tokenizer files and (optionally) seeded random-init
     safetensors in HF parameter naming so both transformers (oracle) and dalm_b200 (product) can load the same directory.
     generation_config: written as generation_config.json when given (e.g. QWEN2_GENERATION["base"]). bias_std: std of the
@@ -371,6 +453,12 @@ def write_model_dir(out_dir: str, kind: str, name: str, vocab_size: Optional[int
     if kind == "bert":
         cfg = bert_config(name, vocab_size or 30522)
         build_bert_tokenizer(out_dir, cfg["vocab_size"])
+    elif kind == "roberta":
+        cfg = roberta_config(name, vocab_size)
+        from .engine.params import roberta_max_len
+
+        build = build_roberta_tokenizer if cfg["model_type"] == "roberta" else build_xlmr_tokenizer
+        build(out_dir, cfg["vocab_size"], model_max_length=roberta_max_len(cfg))
     elif kind == "llama" and name in LLAMA3_SHAPES:
         cfg = llama3_config(name, vocab_size or 128256)
         build_llama3_tokenizer(out_dir, cfg["vocab_size"])

@@ -158,6 +158,11 @@ int dalm_b200_rmsnorm_bwd(const float* x, const float* g, const float* rstd, con
                           const float* dres_in, float* dres_out, void* dres16, long long ld16, int M, int H, void* stream);
 int dalm_b200_bert_embed(const int64_t* ids, const void* word, const void* pos, const void* type0, float* z, int M, int L,
                          int H, int V, void* stream);
+/* RoBERTa / XLM-RoBERTa (HF create_position_ids_from_input_ids): position = pad_id + (id != pad_id) * (count of non-pad ids in
+ * columns 0..l of the row), clamped into [0, P); z = word[id] + pos[position] + type0 (fp32, bert_embed's order of additions).
+ * ids [B,L] dense; pos_ids_out int64 [B*L] (may be NULL) receives the positions. No allocation, no host synchronisation. */
+int dalm_b200_roberta_embed(const int64_t* ids, const void* word, const void* pos, const void* type0, int pad_id, float* z,
+                            int64_t* pos_ids_out, int B, int L, int H, int V, int P, void* stream);
 int dalm_b200_embed_gather(const int64_t* ids, const void* table, float* x, int M, int H, int V, void* stream);
 int dalm_b200_rope(void* buf, long long ld, int col0, int nheads, int D, const float* cos_t, const float* sin_t, int M,
                    int L, int backward, void* stream);
@@ -198,9 +203,10 @@ int dalm_b200_adam_step(float* p, const float* g, float* m, float* v, long long 
  * (either may be NULL), mean NULL for RMSNorm. */
 int dalm_b200_col_reduce(const float* dy_f32, const void* dy_bf16, long long lddy, const float* z, const float* mean,
                          const float* rstd, float* out_sum, float* out_prod, int M, int H, void* stream);
-/* dword[ids[m],:] += d[m,:]; dpos[m % L,:] += d[m,:] (dpos may be NULL) */
-int dalm_b200_embed_scatter_add(const float* d, const int64_t* ids, float* dword, float* dpos, int M, int H, int L, int V,
-                                void* stream);
+/* dword[ids[m],:] += d[m,:]; dpos[pos_ids[m],:] += d[m,:] (dpos may be NULL; pos_ids NULL: position m % L). pad_id >= 0:
+ * tokens with id == pad_id add nothing to dword and positions == pad_id nothing to dpos (nn.Embedding padding_idx); -1: none */
+int dalm_b200_embed_scatter_add(const float* d, const int64_t* ids, const int64_t* pos_ids, float* dword, float* dpos, int M,
+                                int H, int L, int V, int pad_id, void* stream);
 /* out = (a_f32 + b_bf16) * dropout_scale  (gradient through the embedding dropout; out may alias a) */
 int dalm_b200_masked_add(const float* a, const void* b, long long ldb, float* out, int M, int H, float p,
                          unsigned long long seed, unsigned long long stream_id, const void* offset, void* stream);

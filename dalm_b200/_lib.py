@@ -37,12 +37,12 @@ SIGNATURES = {
     "dalm_b200_gemm_clear_cache": [],
     "dalm_b200_gemm_set_raster": [_I],
     "dalm_b200_gemm_set_l2_hints": [_I],
-    "dalm_b200_attention_fwd": [_P, _L, _P, _L, _P, _L, _P, _P, _L, _P, _I, _I, _I, _I, _I, _F, _I, *_DROP, _P],
-    "dalm_b200_attention_tc_fwd": [_P, _L, _P, _L, _P, _L, _P, _P, _L, _P, _I, _I, _I, _I, _I, _F, _I, *_DROP, _P],
+    "dalm_b200_attention_fwd": [_P, _L, _P, _L, _P, _L, _P, _P, _L, _P, _I, _I, _I, _I, _I, _F, _I, _I, *_DROP, _P],
+    "dalm_b200_attention_tc_fwd": [_P, _L, _P, _L, _P, _L, _P, _P, _L, _P, _I, _I, _I, _I, _I, _F, _I, _I, *_DROP, _P],
     "dalm_b200_attention_tc_bwd": [_P, _L, _P, _L, _P, _L, _P, _P, _L, _P, _P, _L, _P, _P, _L, _P, _L, _P, _L,
-                                   _I, _I, _I, _I, _I, _F, _I, *_DROP, _P],
+                                   _I, _I, _I, _I, _I, _F, _I, _I, *_DROP, _P],
     "dalm_b200_attention_bwd": [_P, _L, _P, _L, _P, _L, _P, _P, _L, _P, _P, _L, _P, _P, _L, _P, _L, _P, _L,
-                                _I, _I, _I, _I, _I, _F, _I, *_DROP, _P],
+                                _I, _I, _I, _I, _I, _F, _I, _I, *_DROP, _P],
     "dalm_b200_layernorm_fwd": [_P, _P, _P, _P, _P, _L, _P, _P, _I, _I, _F, *_DROP, _P],
     "dalm_b200_layernorm_bwd": [_P, _P, _P, _P, _P, _P, _L, _P, _P, _L, _I, _I, *_DROP, _P],
     "dalm_b200_layernorm_bwd_res": [_P, _P, _P, _P, _P, _P, _L, _P, _P, _P, _L, _I, _I, _P],
@@ -80,7 +80,7 @@ SIGNATURES = {
     "dalm_b200_rope_pos": [_P, _L, _I, _I, _I, _P, _P, _P, _I, _I, _P],
     "dalm_b200_qk_norm_rope": [_P, _L, _I, _I, _P, _P, _F, _P, _P, _I, _I, _P, _I, _P, _L, _P, _L, _P],
     "dalm_b200_qk_norm_rope_bwd": [_P, _L, _I, _I, _P, _P, _P, _P, _I, _P, _L, _P, _L, _I, _P, _P, _P],
-    "dalm_b200_attention_decode": [_P, _L, _I, _I, _I, _P, _P, _L, _L, _P, _L, _P, _L, _I, _I, _I, _I, _I, _P, _I, _F, _P],
+    "dalm_b200_attention_decode": [_P, _L, _I, _I, _I, _P, _P, _L, _L, _P, _L, _P, _L, _I, _I, _I, _I, _I, _P, _I, _F, _I, _P],
     "dalm_b200_greedy_step": [_P, _L, _I, _I, _P, _I, _L, _P, _P, _L, _P, _L, _I, _P, _I, _P, _P, _P, _P],
     "dalm_b200_sample_step": [_P, _L, _I, _I, _P, _I, _L, _P, _P, _L, _P, _L, _I, _P, _I, _P, _P, _P, _F, _I, _F, _U, _P, _P, _P],
 }

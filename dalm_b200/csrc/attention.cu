@@ -37,6 +37,8 @@ struct AttnParams {
   DropCfg drop;                     // attention-probability dropout (BERT attention_probs_dropout_prob); p = 0 => off.
                                     // element index of P[b,h,i,j] = ((b*Hq + h)*L + i)*Lp + j, Lp = L rounded up to 8
                                     // (rows start on a Philox group of 8, so one call covers an 8-key MMA n-tile)
+  int window;                       // sliding window (WIN instances only): query i sees key j iff i - window < j <= i;
+                                    // the host clamps it to L, so tile bounds computed from it cannot overflow
 };
 
 // ---------------------------------------------------------------- fragment helpers
@@ -92,10 +94,17 @@ __device__ __forceinline__ void load_b_frag_kn(uint32_t* b, const __nv_bfloat16*
   ldsm_x4_t(b, s + (k0 + (lane & 7) + (((lane >> 3) & 1) << 3)) * (D + 8) + n0 + ((lane >> 4) << 3));
 }
 
+// first key of the KV loop of the query tile at q0: 0 without a window, else the tile holding key q0 - window + 1 (the
+// first key any of its queries sees). A skipped tile would be fully masked for every query of the tile (corr = 1, p = 0
+// in the online softmax), so starting later changes no bit of the result.
+template <bool WIN, int BKV> __device__ __forceinline__ int win_begin(int q0, int window) {
+  return WIN ? (max(0, q0 - window + 1) / BKV) * BKV : 0;
+}
+
 // ============================================================================================================
 // forward
 // ============================================================================================================
-template <int D, bool DROP>
+template <int D, bool DROP, bool WIN>
 __global__ void __launch_bounds__(128) attn_fwd_kernel(AttnParams p) {
   constexpr int BQ = 64, BKV = 64, LDS = D + 8;
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -120,7 +129,7 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(AttnParams p) {
   const int row_a = q0 + warp * 16 + g, row_b = row_a + 8;       // the two query rows this thread holds
 
   const int kv_end = p.causal ? min(L, q0 + BQ) : L;
-  for (int kv0 = 0; kv0 < kv_end; kv0 += BKV) {
+  for (int kv0 = win_begin<WIN, BKV>(q0, p.window); kv0 < kv_end; kv0 += BKV) {
     __syncthreads();                                            // previous tile fully consumed
     const int nvalid = min(BKV, L - kv0);
     load_tile<BKV, D, 128>(sK, p.k + (tok0 + kv0) * p.ldk + (size_t)hk * D, p.ldk, nvalid);
@@ -159,6 +168,7 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(AttnParams p) {
         const int qr = (e < 2) ? row_a : row_b;
         float val = s[nt][e] * sl2 + sMask[kc];
         if (p.causal && (kv0 + kc) > qr) val = -INFINITY;
+        if (WIN && (kv0 + kc) <= qr - p.window) val = -INFINITY;
         s[nt][e] = val;
         mx[e >> 1] = fmaxf(mx[e >> 1], val);
       }
@@ -282,7 +292,7 @@ __global__ void attn_delta_kernel(const __nv_bfloat16* __restrict__ o, long long
 // ============================================================================================================
 // backward: dK, dV.  Each warp owns 16 keys; queries streamed in 32-row tiles.
 // ============================================================================================================
-template <int D, bool DROP>
+template <int D, bool DROP, bool WIN>
 __global__ void __launch_bounds__(128) attn_bwd_dkv_kernel(AttnParams p) {
   constexpr int BKV = 64, BQ = 32, LDS = D + 8;
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -319,9 +329,10 @@ __global__ void __launch_bounds__(128) attn_bwd_dkv_kernel(AttnParams p) {
   }
   const int key_a = kv0 + warp * 16 + g, key_b = key_a + 8;     // the two keys (rows of S^T) this thread holds
   const int q_begin = p.causal ? (kv0 / BQ) * BQ : 0;            // queries before the key tile see none of it
+  const int q_end = WIN ? min(L, kv0 + BKV - 1 + p.window) : L;  // nor do queries past its last key's window
 
   for (int hq = hk * group; hq < (hk + 1) * group; ++hq) {
-    for (int q0 = q_begin; q0 < L; q0 += BQ) {
+    for (int q0 = q_begin; q0 < q_end; q0 += BQ) {
       __syncthreads();
       const int nq = min(BQ, L - q0);
       load_tile<BQ, D, 128>(sQ, p.q + (tok0 + q0) * p.ldq + (size_t)hq * D, p.ldq, nq);
@@ -360,6 +371,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dkv_kernel(AttnParams p) {
           const int key = (e < 2) ? key_a : key_b;
           float val = st[nt][e] * sl2 + ((e < 2) ? mk_a : mk_b);
           if (p.causal && key > (q0 + qc)) val = -INFINITY;
+          if (WIN && key <= (q0 + qc) - p.window) val = -INFINITY;
           st[nt][e] = exp2f(val - sLse[qc]);                     // -inf - x -> 0 ; x - (+inf) -> 0
         }
       }
@@ -478,7 +490,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dkv_kernel(AttnParams p) {
 // ============================================================================================================
 // backward: dQ.  Each warp owns 16 queries; keys streamed in 64-row tiles.
 // ============================================================================================================
-template <int D, bool DROP>
+template <int D, bool DROP, bool WIN>
 __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(AttnParams p) {
   constexpr int BQ = 64, BKV = 64, LDS = D + 8;
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -513,7 +525,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(AttnParams p) {
   for (int i = 0; i < D / 8; ++i) { dq_acc[i][0] = dq_acc[i][1] = dq_acc[i][2] = dq_acc[i][3] = 0.f; }
 
   const int kv_end = p.causal ? min(L, q0 + BQ) : L;
-  for (int kv0 = 0; kv0 < kv_end; kv0 += BKV) {
+  for (int kv0 = win_begin<WIN, BKV>(q0, p.window); kv0 < kv_end; kv0 += BKV) {
     __syncthreads();
     const int nvalid = min(BKV, L - kv0);
     load_tile<BKV, D, 128>(sK, p.k + (tok0 + kv0) * p.ldk + (size_t)hk * D, p.ldk, nvalid);
@@ -576,6 +588,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(AttnParams p) {
         const int qr = (e < 2) ? row_a : row_b;
         float val = s[nt][e] * sl2 + sMask[kc];
         if (p.causal && (kv0 + kc) > qr) val = -INFINITY;
+        if (WIN && (kv0 + kc) <= qr - p.window) val = -INFINITY;
         const float pv = exp2f(val - lse2[e >> 1]);
         float dpv = dp[nt][e];
         if (DROP) dpv *= msq[nt][e];
@@ -615,29 +628,29 @@ template <int D> static size_t fwd_smem() { return (size_t)(64 * 3) * (D + 8) * 
 template <int D> static size_t dkv_smem() { return (size_t)(64 * 2 + 32 * 2) * (D + 8) * 2 + (32 + 32 + 64) * 4; }
 template <int D> static size_t dq_smem()  { return (size_t)(64 * 4) * (D + 8) * 2 + 64 * 4; }
 
-template <int D, bool DROP> static int launch_fwd(const AttnParams& p, cudaStream_t st) {
+template <int D, bool DROP, bool WIN> static int launch_fwd(const AttnParams& p, cudaStream_t st) {
   static bool attr = false;
-  if (!attr) { DALM_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<D, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fwd_smem<D>())); attr = true; }
+  if (!attr) { DALM_CUDA(cudaFuncSetAttribute(attn_fwd_kernel<D, DROP, WIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fwd_smem<D>())); attr = true; }
   dim3 grid((p.L + 63) / 64, p.Hq, p.B);
-  attn_fwd_kernel<D, DROP><<<grid, 128, fwd_smem<D>(), st>>>(p);
+  attn_fwd_kernel<D, DROP, WIN><<<grid, 128, fwd_smem<D>(), st>>>(p);
   count_launch();
   return check_launch("attn_fwd_kernel");
 }
-template <int D, bool DROP> static int launch_bwd(const AttnParams& p, cudaStream_t st) {
+template <int D, bool DROP, bool WIN> static int launch_bwd(const AttnParams& p, cudaStream_t st) {
   static bool attr = false;
   if (!attr) {
-    DALM_CUDA(cudaFuncSetAttribute(attn_bwd_dkv_kernel<D, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dkv_smem<D>()));
-    DALM_CUDA(cudaFuncSetAttribute(attn_bwd_dq_kernel<D, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dq_smem<D>()));
+    DALM_CUDA(cudaFuncSetAttribute(attn_bwd_dkv_kernel<D, DROP, WIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dkv_smem<D>()));
+    DALM_CUDA(cudaFuncSetAttribute(attn_bwd_dq_kernel<D, DROP, WIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dq_smem<D>()));
     attr = true;
   }
   const int total_warps = p.B * p.L * p.Hq;
   attn_delta_kernel<<<(total_warps * 32 + 255) / 256, 256, 0, st>>>(p.o, p.ldo, p.d_o, p.lddo, p.delta, p.B, p.L, p.Hq, D);
   if (int e = check_launch("attn_delta_kernel")) return e;
   dim3 gkv((p.L + 63) / 64, p.Hkv, p.B);
-  attn_bwd_dkv_kernel<D, DROP><<<gkv, 128, dkv_smem<D>(), st>>>(p);
+  attn_bwd_dkv_kernel<D, DROP, WIN><<<gkv, 128, dkv_smem<D>(), st>>>(p);
   if (int e = check_launch("attn_bwd_dkv_kernel")) return e;
   dim3 gq((p.L + 63) / 64, p.Hq, p.B);
-  attn_bwd_dq_kernel<D, DROP><<<gq, 128, dq_smem<D>(), st>>>(p);
+  attn_bwd_dq_kernel<D, DROP, WIN><<<gq, 128, dq_smem<D>(), st>>>(p);
   count_launch(3);
   return check_launch("attn_bwd_dq_kernel");
 }
@@ -676,7 +689,7 @@ template <int D> constexpr int wg_fwd_smem() { return 5 * wg_tile<D>() + 64 * 4 
 template <int D> constexpr int wg_dq_smem() { return 6 * wg_tile<D>() + 64 * 4 + 64 + 1024; }
 template <int D> constexpr int wg_dkv_smem() { return 2 * wg_tile<D>() + 4 * (wg_tile<D>() / 2) + (64 + 32 + 32) * 4 + 64 + 1024; }
 
-template <int D, bool DROP>
+template <int D, bool DROP, bool WIN>
 __global__ void __launch_bounds__(128) attn_fwd_wg_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
                                                           const __grid_constant__ CUtensorMap tv, AttnParams p) {
   using namespace wg;
@@ -693,7 +706,8 @@ __global__ void __launch_bounds__(128) attn_fwd_wg_kernel(const __grid_constant_
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   const size_t tok0 = (size_t)b * L;
   const int kv_end = p.causal ? min(L, q0 + BQ) : L;
-  const int ntile = (kv_end + BKV - 1) / BKV;
+  const int kv_begin = win_begin<WIN, BKV>(q0, p.window);       // tile `it` starts at kv_begin + it * BKV
+  const int ntile = (kv_end - kv_begin + BKV - 1) / BKV;
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < 3; ++i) mbar_init(&bar[i], 1);
@@ -701,8 +715,8 @@ __global__ void __launch_bounds__(128) attn_fwd_wg_kernel(const __grid_constant_
     mbar_arrive_expect_tx(&bar[0], TILE);
     load_tile<64, D>(sQ, &tq, &bar[0], h * D, (int)(tok0 + q0));
     mbar_arrive_expect_tx(&bar[1], 2 * TILE);
-    load_tile<64, D>(sKV, &tk, &bar[1], hk * D, (int)tok0);
-    load_tile<64, D>(sKV + TILE, &tv, &bar[1], hk * D, (int)tok0);
+    load_tile<64, D>(sKV, &tk, &bar[1], hk * D, (int)(tok0 + kv_begin));
+    load_tile<64, D>(sKV + TILE, &tv, &bar[1], hk * D, (int)(tok0 + kv_begin));
   }
   __syncthreads();
 
@@ -716,7 +730,7 @@ __global__ void __launch_bounds__(128) attn_fwd_wg_kernel(const __grid_constant_
   mbar_wait(&bar[0], 0);
 
   for (int it = 0; it < ntile; ++it) {
-    const int kv0 = it * BKV, cb = it & 1;
+    const int kv0 = kv_begin + it * BKV, cb = it & 1;
     if (threadIdx.x == 0 && it + 1 < ntile) {                   // buffer cb^1 was released by the barrier closing it - 1
       unsigned char* nb = sKV + (cb ^ 1) * 2 * TILE;
       mbar_arrive_expect_tx(&bar[1 + (cb ^ 1)], 2 * TILE);
@@ -752,6 +766,7 @@ __global__ void __launch_bounds__(128) attn_fwd_wg_kernel(const __grid_constant_
         const int qr = (e < 2) ? row_a : row_b;
         float val = s[nt][e] * sl2 + sMask[kc];
         if (p.causal && (kv0 + kc) > qr) val = -INFINITY;
+        if (WIN && (kv0 + kc) <= qr - p.window) val = -INFINITY;
         s[nt][e] = val;
         mx[e >> 1] = fmaxf(mx[e >> 1], val);
       }
@@ -844,7 +859,7 @@ __global__ void __launch_bounds__(128) attn_fwd_wg_kernel(const __grid_constant_
 
 // dK, dV: grid (ceil(L/64), Hkv, B); the warpgroup owns 64 keys (K, V resident), query tiles of 32 rows streamed over
 // the q heads of the group
-template <int D, bool DROP>
+template <int D, bool DROP, bool WIN>
 __global__ void __launch_bounds__(128) attn_bwd_dkv_wg_kernel(const __grid_constant__ CUtensorMap tk, const __grid_constant__ CUtensorMap tv,
                                                               const __grid_constant__ CUtensorMap tq32, const __grid_constant__ CUtensorMap tdo32,
                                                               AttnParams p) {
@@ -866,7 +881,8 @@ __global__ void __launch_bounds__(128) attn_bwd_dkv_wg_kernel(const __grid_const
   const size_t tok0 = (size_t)b * L;
   const float sl2 = p.scale * 1.4426950408889634f;
   const int q_begin = p.causal ? (kv0 / BQ) * BQ : 0;
-  const int nqt = (L - q_begin + BQ - 1) / BQ;
+  const int q_end = WIN ? min(L, kv0 + BKV - 1 + p.window) : L;
+  const int nqt = (q_end - q_begin + BQ - 1) / BQ;
   const int nit = group * nqt;                                   // (q head, query tile) pairs, head-major
 
   if (threadIdx.x == 0) {
@@ -942,6 +958,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dkv_wg_kernel(const __grid_const
         const int key = (e < 2) ? key_a : key_b;
         float val = st[nt][e] * sl2 + ((e < 2) ? mk_a : mk_b);
         if (p.causal && key > (q0 + qc)) val = -INFINITY;
+        if (WIN && key <= (q0 + qc) - p.window) val = -INFINITY;
         st[nt][e] = exp2f(val - sLse[qc]);
       }
     }
@@ -1013,7 +1030,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dkv_wg_kernel(const __grid_const
 }
 
 // dQ: grid (ceil(L/64), Hq, B); the warpgroup owns 64 queries (Q, dO resident), key tiles of 64 streamed
-template <int D, bool DROP>
+template <int D, bool DROP, bool WIN>
 __global__ void __launch_bounds__(128) attn_bwd_dq_wg_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tdo,
                                                              const __grid_constant__ CUtensorMap tk, const __grid_constant__ CUtensorMap tv,
                                                              AttnParams p) {
@@ -1033,7 +1050,8 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_wg_kernel(const __grid_consta
   const size_t tok0 = (size_t)b * L;
   const float sl2 = p.scale * 1.4426950408889634f;
   const int kv_end = p.causal ? min(L, q0 + BQ) : L;
-  const int ntile = (kv_end + BKV - 1) / BKV;
+  const int kv_begin = win_begin<WIN, BKV>(q0, p.window);       // tile `it` starts at kv_begin + it * BKV
+  const int ntile = (kv_end - kv_begin + BKV - 1) / BKV;
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < 3; ++i) mbar_init(&bar[i], 1);
@@ -1042,8 +1060,8 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_wg_kernel(const __grid_consta
     load_tile<64, D>(sQ, &tq, &bar[0], h * D, (int)(tok0 + q0));
     load_tile<64, D>(sdO, &tdo, &bar[0], h * D, (int)(tok0 + q0));
     mbar_arrive_expect_tx(&bar[1], 2 * TILE);
-    load_tile<64, D>(sKV, &tk, &bar[1], hk * D, (int)tok0);
-    load_tile<64, D>(sKV + TILE, &tv, &bar[1], hk * D, (int)tok0);
+    load_tile<64, D>(sKV, &tk, &bar[1], hk * D, (int)(tok0 + kv_begin));
+    load_tile<64, D>(sKV + TILE, &tv, &bar[1], hk * D, (int)(tok0 + kv_begin));
   }
   __syncthreads();
 
@@ -1063,7 +1081,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_wg_kernel(const __grid_consta
   mbar_wait(&bar[0], 0);
 
   for (int it = 0; it < ntile; ++it) {
-    const int kv0 = it * BKV, cb = it & 1;
+    const int kv0 = kv_begin + it * BKV, cb = it & 1;
     if (threadIdx.x == 0 && it + 1 < ntile) {
       unsigned char* nb = sKV + (cb ^ 1) * 2 * TILE;
       mbar_arrive_expect_tx(&bar[1 + (cb ^ 1)], 2 * TILE);
@@ -1120,6 +1138,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_wg_kernel(const __grid_consta
         const int qr = (e < 2) ? row_a : row_b;
         float val = s[nt][e] * sl2 + sMask[kc];
         if (p.causal && (kv0 + kc) > qr) val = -INFINITY;
+        if (WIN && (kv0 + kc) <= qr - p.window) val = -INFINITY;
         const float pv = exp2f(val - lse2[e >> 1]);
         float dpv = dp[nt][e];
         if (DROP) dpv *= msq[nt][e];
@@ -1154,24 +1173,24 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_wg_kernel(const __grid_consta
   }
 }
 
-template <int D, bool DROP> static int launch_fwd_wg(const AttnParams& p, int qcols, int kvcols, cudaStream_t st) {
+template <int D, bool DROP, bool WIN> static int launch_fwd_wg(const AttnParams& p, int qcols, int kvcols, cudaStream_t st) {
   static bool attr = false;
-  if (!attr) { DALM_CUDA(cudaFuncSetAttribute(attn_fwd_wg_kernel<D, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_fwd_smem<D>())); attr = true; }
+  if (!attr) { DALM_CUDA(cudaFuncSetAttribute(attn_fwd_wg_kernel<D, DROP, WIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_fwd_smem<D>())); attr = true; }
   const long long rows = (long long)p.B * p.L;
   CUtensorMap tq, tk, tv;
   if (int e = get_tmap(p.q, rows, qcols, p.ldq, 64, &tq)) return e;
   if (int e = get_tmap(p.k, rows, kvcols, p.ldk, 64, &tk)) return e;
   if (int e = get_tmap(p.v, rows, kvcols, p.ldv, 64, &tv)) return e;
   dim3 grid((p.L + 63) / 64, p.Hq, p.B);
-  attn_fwd_wg_kernel<D, DROP><<<grid, 128, wg_fwd_smem<D>(), st>>>(tq, tk, tv, p);
+  attn_fwd_wg_kernel<D, DROP, WIN><<<grid, 128, wg_fwd_smem<D>(), st>>>(tq, tk, tv, p);
   count_launch();
   return check_launch("attn_fwd_wg_kernel");
 }
-template <int D, bool DROP> static int launch_bwd_wg(const AttnParams& p, int qcols, int kvcols, cudaStream_t st) {
+template <int D, bool DROP, bool WIN> static int launch_bwd_wg(const AttnParams& p, int qcols, int kvcols, cudaStream_t st) {
   static bool attr = false;
   if (!attr) {
-    DALM_CUDA(cudaFuncSetAttribute(attn_bwd_dkv_wg_kernel<D, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_dkv_smem<D>()));
-    DALM_CUDA(cudaFuncSetAttribute(attn_bwd_dq_wg_kernel<D, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_dq_smem<D>()));
+    DALM_CUDA(cudaFuncSetAttribute(attn_bwd_dkv_wg_kernel<D, DROP, WIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_dkv_smem<D>()));
+    DALM_CUDA(cudaFuncSetAttribute(attn_bwd_dq_wg_kernel<D, DROP, WIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_dq_smem<D>()));
     attr = true;
   }
   const long long rows = (long long)p.B * p.L;
@@ -1186,10 +1205,10 @@ template <int D, bool DROP> static int launch_bwd_wg(const AttnParams& p, int qc
   attn_delta_kernel<<<(total_warps * 32 + 255) / 256, 256, 0, st>>>(p.o, p.ldo, p.d_o, p.lddo, p.delta, p.B, p.L, p.Hq, D);
   if (int e = check_launch("attn_delta_kernel")) return e;
   dim3 gkv((p.L + 63) / 64, p.Hkv, p.B);
-  attn_bwd_dkv_wg_kernel<D, DROP><<<gkv, 128, wg_dkv_smem<D>(), st>>>(tk, tv, tq32, tdo32, p);
+  attn_bwd_dkv_wg_kernel<D, DROP, WIN><<<gkv, 128, wg_dkv_smem<D>(), st>>>(tk, tv, tq32, tdo32, p);
   if (int e = check_launch("attn_bwd_dkv_wg_kernel")) return e;
   dim3 gq((p.L + 63) / 64, p.Hq, p.B);
-  attn_bwd_dq_wg_kernel<D, DROP><<<gq, 128, wg_dq_smem<D>(), st>>>(tq, tdo, tk, tv, p);
+  attn_bwd_dq_wg_kernel<D, DROP, WIN><<<gq, 128, wg_dq_smem<D>(), st>>>(tq, tdo, tk, tv, p);
   count_launch(3);
   return check_launch("attn_bwd_dq_wg_kernel");
 }
@@ -1199,7 +1218,16 @@ static int check_common(const AttnParams& p, int D) {
   DALM_REQUIRE(p.B > 0 && p.L > 0 && p.Hq > 0 && p.Hkv > 0 && p.Hq % p.Hkv == 0, "attention: bad shape B=%d L=%d Hq=%d Hkv=%d", p.B, p.L, p.Hq, p.Hkv);
   DALM_REQUIRE(p.ldq % 8 == 0 && p.ldk % 8 == 0 && p.ldv % 8 == 0 && p.ldo % 2 == 0, "attention: strides must keep 16-byte row alignment");
   DALM_REQUIRE(((uintptr_t)p.q & 15) == 0 && ((uintptr_t)p.k & 15) == 0 && ((uintptr_t)p.v & 15) == 0, "attention: q/k/v must be 16-byte aligned");
+  DALM_REQUIRE(p.window >= 0 && (p.window == 0 || p.causal), "attention: window %d must be >= 0, and > 0 only with causal", p.window);
+  DALM_REQUIRE(p.window == 0 || p.drop.p == 0.f, "attention: probability dropout with a sliding window is not built");
   return 0;
+}
+
+// window > 0 runs the WIN instances (window clamped to L: a wider window masks nothing more); window 0 runs the
+// instances that were built before the window existed, unchanged
+static bool set_window(AttnParams& p, int window) {
+  p.window = window > 0 ? min(window, p.L) : window;        // a negative window stays negative: check_common refuses it
+  return window > 0;
 }
 }  // namespace dalm
 
@@ -1208,7 +1236,7 @@ using namespace dalm;
 // q/k/v: bf16 token-major views (row b*L+l, head h at column h*D); mask: int64 [B,L] or NULL; out: bf16; lse: fp32 [B,Hq,L]
 extern "C" int dalm_b200_attention_fwd(const void* q, long long ldq, const void* k, long long ldk, const void* v,
                                        long long ldv, const int64_t* mask, void* out, long long ldo, float* lse, int B,
-                                       int L, int Hq, int Hkv, int D, float scale, int causal, float drop_p,
+                                       int L, int Hq, int Hkv, int D, float scale, int causal, int window, float drop_p,
                                        unsigned long long drop_seed, unsigned long long drop_stream_id,
                                        const void* drop_offset, void* stream) {
   AttnParams p{};
@@ -1216,14 +1244,16 @@ extern "C" int dalm_b200_attention_fwd(const void* q, long long ldq, const void*
   p.ldq = ldq; p.ldk = ldk; p.ldv = ldv; p.mask = mask; p.o = (__nv_bfloat16*)out; p.ldo = ldo; p.lse = lse;
   p.B = B; p.L = L; p.Hq = Hq; p.Hkv = Hkv; p.scale = scale; p.causal = causal;
   p.drop = make_drop(drop_p, drop_seed, drop_stream_id, drop_offset);
+  const bool win = set_window(p, window);
   if (int e = check_common(p, D)) return e;
   DALM_REQUIRE(drop_p >= 0.f && drop_p < 1.f, "attention: dropout p must be in [0,1)");
   DALM_REQUIRE(drop_p == 0.f || D <= 64, "attention: probability dropout is built for head_dim <= 64 (encoder); Llama has attention_dropout = 0");
   cudaStream_t st = (cudaStream_t)stream;
-  if (drop_p > 0.f) return D == 32 ? launch_fwd<32, true>(p, st) : launch_fwd<64, true>(p, st);
-  if (D == 32) return launch_fwd<32, false>(p, st);
-  if (D == 64) return launch_fwd<64, false>(p, st);
-  return launch_fwd<128, false>(p, st);
+  if (drop_p > 0.f) return D == 32 ? launch_fwd<32, true, false>(p, st) : launch_fwd<64, true, false>(p, st);
+  if (win) return D == 32 ? launch_fwd<32, false, true>(p, st) : D == 64 ? launch_fwd<64, false, true>(p, st) : launch_fwd<128, false, true>(p, st);
+  if (D == 32) return launch_fwd<32, false, false>(p, st);
+  if (D == 64) return launch_fwd<64, false, false>(p, st);
+  return launch_fwd<128, false, false>(p, st);
 }
 
 // delta: fp32 workspace [B,Hq,L]; dq/dk/dv: bf16 token-major outputs (dk/dv have Hkv heads)
@@ -1231,7 +1261,7 @@ extern "C" int dalm_b200_attention_bwd(const void* q, long long ldq, const void*
                                        long long ldv, const int64_t* mask, const void* out, long long ldo,
                                        const float* lse, const void* d_out, long long lddo, float* delta, void* dq,
                                        long long lddq, void* dk, long long lddk, void* dv, long long lddv, int B, int L,
-                                       int Hq, int Hkv, int D, float scale, int causal, float drop_p,
+                                       int Hq, int Hkv, int D, float scale, int causal, int window, float drop_p,
                                        unsigned long long drop_seed, unsigned long long drop_stream_id,
                                        const void* drop_offset, void* stream) {
   AttnParams p{};
@@ -1241,21 +1271,23 @@ extern "C" int dalm_b200_attention_bwd(const void* q, long long ldq, const void*
   p.dq = (__nv_bfloat16*)dq; p.dk = (__nv_bfloat16*)dk; p.dv = (__nv_bfloat16*)dv;
   p.lddq = lddq; p.lddk = lddk; p.lddv = lddv;
   p.B = B; p.L = L; p.Hq = Hq; p.Hkv = Hkv; p.scale = scale; p.causal = causal;
+  p.drop = make_drop(drop_p, drop_seed, drop_stream_id, drop_offset);
+  const bool win = set_window(p, window);
   if (int e = check_common(p, D)) return e;
   DALM_REQUIRE(lddo % 8 == 0 && ((uintptr_t)d_out & 15) == 0, "attention_bwd: d_out alignment");
   DALM_REQUIRE(drop_p >= 0.f && drop_p < 1.f && (drop_p == 0.f || D <= 64), "attention_bwd: dropout needs p in [0,1) and head_dim <= 64");
-  p.drop = make_drop(drop_p, drop_seed, drop_stream_id, drop_offset);
   cudaStream_t st = (cudaStream_t)stream;
-  if (drop_p > 0.f) return D == 32 ? launch_bwd<32, true>(p, st) : launch_bwd<64, true>(p, st);
-  if (D == 32) return launch_bwd<32, false>(p, st);
-  if (D == 64) return launch_bwd<64, false>(p, st);
-  return launch_bwd<128, false>(p, st);
+  if (drop_p > 0.f) return D == 32 ? launch_bwd<32, true, false>(p, st) : launch_bwd<64, true, false>(p, st);
+  if (win) return D == 32 ? launch_bwd<32, false, true>(p, st) : D == 64 ? launch_bwd<64, false, true>(p, st) : launch_bwd<128, false, true>(p, st);
+  if (D == 32) return launch_bwd<32, false, false>(p, st);
+  if (D == 64) return launch_bwd<64, false, false>(p, st);
+  return launch_bwd<128, false, false>(p, st);
 }
 
 // the wgmma kernels: same contract as dalm_b200_attention_fwd, head_dim 64 or 128 (dropout at 64)
 extern "C" int dalm_b200_attention_tc_fwd(const void* q, long long ldq, const void* k, long long ldk, const void* v,
                                           long long ldv, const int64_t* mask, void* out, long long ldo, float* lse, int B,
-                                          int L, int Hq, int Hkv, int D, float scale, int causal, float drop_p,
+                                          int L, int Hq, int Hkv, int D, float scale, int causal, int window, float drop_p,
                                           unsigned long long drop_seed, unsigned long long drop_stream_id,
                                           const void* drop_offset, void* stream) {
   AttnParams p{};
@@ -1263,13 +1295,15 @@ extern "C" int dalm_b200_attention_tc_fwd(const void* q, long long ldq, const vo
   p.ldq = ldq; p.ldk = ldk; p.ldv = ldv; p.mask = mask; p.o = (__nv_bfloat16*)out; p.ldo = ldo; p.lse = lse;
   p.B = B; p.L = L; p.Hq = Hq; p.Hkv = Hkv; p.scale = scale; p.causal = causal;
   p.drop = make_drop(drop_p, drop_seed, drop_stream_id, drop_offset);
+  const bool win = set_window(p, window);
   if (int e = check_common(p, D)) return e;
   DALM_REQUIRE(D == 64 || D == 128, "attention_tc: head_dim %d unsupported (64/128)", D);
   DALM_REQUIRE(drop_p >= 0.f && drop_p < 1.f && (drop_p == 0.f || D == 64), "attention_tc: dropout needs p in [0,1) and head_dim 64");
   cudaStream_t st = (cudaStream_t)stream;
-  if (drop_p > 0.f) return launch_fwd_wg<64, true>(p, Hq * D, Hkv * D, st);
-  if (D == 64) return launch_fwd_wg<64, false>(p, Hq * D, Hkv * D, st);
-  return launch_fwd_wg<128, false>(p, Hq * D, Hkv * D, st);
+  if (drop_p > 0.f) return launch_fwd_wg<64, true, false>(p, Hq * D, Hkv * D, st);
+  if (win) return D == 64 ? launch_fwd_wg<64, false, true>(p, Hq * D, Hkv * D, st) : launch_fwd_wg<128, false, true>(p, Hq * D, Hkv * D, st);
+  if (D == 64) return launch_fwd_wg<64, false, false>(p, Hq * D, Hkv * D, st);
+  return launch_fwd_wg<128, false, false>(p, Hq * D, Hkv * D, st);
 }
 
 // the wgmma kernels: same contract as dalm_b200_attention_bwd, head_dim 64 or 128 (dropout at 64)
@@ -1277,7 +1311,7 @@ extern "C" int dalm_b200_attention_tc_bwd(const void* q, long long ldq, const vo
                                           long long ldv, const int64_t* mask, const void* out, long long ldo,
                                           const float* lse, const void* d_out, long long lddo, float* delta, void* dq,
                                           long long lddq, void* dk, long long lddk, void* dv, long long lddv, int B, int L,
-                                          int Hq, int Hkv, int D, float scale, int causal, float drop_p,
+                                          int Hq, int Hkv, int D, float scale, int causal, int window, float drop_p,
                                           unsigned long long drop_seed, unsigned long long drop_stream_id,
                                           const void* drop_offset, void* stream) {
   AttnParams p{};
@@ -1287,13 +1321,15 @@ extern "C" int dalm_b200_attention_tc_bwd(const void* q, long long ldq, const vo
   p.dq = (__nv_bfloat16*)dq; p.dk = (__nv_bfloat16*)dk; p.dv = (__nv_bfloat16*)dv;
   p.lddq = lddq; p.lddk = lddk; p.lddv = lddv;
   p.B = B; p.L = L; p.Hq = Hq; p.Hkv = Hkv; p.scale = scale; p.causal = causal;
+  p.drop = make_drop(drop_p, drop_seed, drop_stream_id, drop_offset);
+  const bool win = set_window(p, window);
   if (int e = check_common(p, D)) return e;
   DALM_REQUIRE(D == 64 || D == 128, "attention_tc: head_dim %d unsupported (64/128)", D);
   DALM_REQUIRE(lddo % 8 == 0 && ((uintptr_t)d_out & 15) == 0, "attention_tc_bwd: d_out alignment");
   DALM_REQUIRE(drop_p >= 0.f && drop_p < 1.f && (drop_p == 0.f || D == 64), "attention_tc_bwd: dropout needs p in [0,1) and head_dim 64");
-  p.drop = make_drop(drop_p, drop_seed, drop_stream_id, drop_offset);
   cudaStream_t st = (cudaStream_t)stream;
-  if (drop_p > 0.f) return launch_bwd_wg<64, true>(p, Hq * D, Hkv * D, st);
-  if (D == 64) return launch_bwd_wg<64, false>(p, Hq * D, Hkv * D, st);
-  return launch_bwd_wg<128, false>(p, Hq * D, Hkv * D, st);
+  if (drop_p > 0.f) return launch_bwd_wg<64, true, false>(p, Hq * D, Hkv * D, st);
+  if (win) return D == 64 ? launch_bwd_wg<64, false, true>(p, Hq * D, Hkv * D, st) : launch_bwd_wg<128, false, true>(p, Hq * D, Hkv * D, st);
+  if (D == 64) return launch_bwd_wg<64, false, false>(p, Hq * D, Hkv * D, st);
+  return launch_bwd_wg<128, false, false>(p, Hq * D, Hkv * D, st);
 }

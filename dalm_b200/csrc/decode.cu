@@ -55,6 +55,8 @@ __device__ __forceinline__ void load8_nc(const __nv_bfloat16* p, float* f) {
 //   pass 2: block max / exp / sum
 //   pass 3: PV with 128 threads = KG key groups x D/8 lanes; every lane loads 16 bytes of V unconditionally (masked keys
 //           carry p = 0; their cache rows are initialised memory) and the KG partial rows meet in shared memory
+// With a sliding window (window > 0) all three passes run over columns max(0, cur - window + 1) .. cur only; while
+// cur < window that is every column, in the same order, so the result is bit-identical to window = 0.
 template <int D>
 __global__ void __launch_bounds__(128) attn_decode_kernel(const __nv_bfloat16* __restrict__ qkv, long long ldq, int q_col,
                                                           int k_col, int v_col, __nv_bfloat16* __restrict__ cache_k,
@@ -62,7 +64,7 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const __nv_bfloat16* _
                                                           long long cache_st, const int64_t* __restrict__ mask,
                                                           long long ldm, __nv_bfloat16* __restrict__ out, long long ldo,
                                                           int Hq, int Hkv, int cur_host, const int* __restrict__ cur_dev,
-                                                          int sp_cap, float scale) {
+                                                          int sp_cap, float scale, int window) {
   extern __shared__ float sm[];
   float* sq = sm;
   float* sp = sm + D;
@@ -71,6 +73,7 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const __nv_bfloat16* _
                                                  // part = [KG][D] = 1024 floats for every supported D
   const int h = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
   const int cur = cur_dev ? min(cur_dev[b], sp_cap - 1) : cur_host;
+  const int t0 = window > 0 ? max(0, cur - window + 1) : 0;   // first visible column
   const int group = Hq / Hkv, kvh = h / group;
   const __nv_bfloat16* qrow = qkv + (size_t)b * ldq + q_col + h * D;
   const __nv_bfloat16* krow = qkv + (size_t)b * ldq + k_col + kvh * D;
@@ -87,7 +90,7 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const __nv_bfloat16* _
   __syncthreads();
 
   float lmax = -INFINITY;
-  for (int t = tid; t <= cur; t += 128) {
+  for (int t = t0 + tid; t <= cur; t += 128) {
     // column `cur` is the token being decoded: always visible, read from the qkv row (its cache slot is written above
     // by ANOTHER CTA of this launch, so nobody reads it back here)
     const bool valid = (t == cur) || mask[(size_t)b * ldm + t] != 0;
@@ -106,7 +109,7 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const __nv_bfloat16* _
   }
   const float m = block_max(lmax, red);         // finite: column `cur` is always valid
   float lsum = 0.f;
-  for (int t = tid; t <= cur; t += 128) {
+  for (int t = t0 + tid; t <= cur; t += 128) {
     const float s = sp[t];
     const float p = (s == -INFINITY) ? 0.f : __expf(s - m);
     sp[t] = p;
@@ -121,7 +124,7 @@ __global__ void __launch_bounds__(128) attn_decode_kernel(const __nv_bfloat16* _
 #pragma unroll
   for (int e = 0; e < 8; ++e) acc[e] = 0.f;
 #pragma unroll 4
-  for (int t = kg; t <= cur; t += KG) {
+  for (int t = t0 + kg; t <= cur; t += KG) {
     const __nv_bfloat16* vp = (t == cur) ? vrow : cv + (size_t)t * cache_st;
     float f[8];
     load8_nc(vp + 8 * dl, f);
@@ -628,7 +631,7 @@ extern "C" int dalm_b200_rope_pos(void* buf, long long ld, int col0, int nheads,
 extern "C" int dalm_b200_attention_decode(const void* qkv, long long ldq, int q_col, int k_col, int v_col, void* cache_k,
                                           void* cache_v, long long cache_sb, long long cache_st, const int64_t* mask,
                                           long long ldm, void* out, long long ldo, int B, int Hq, int Hkv, int D, int cur,
-                                          const int* cur_dev, int T, float scale, void* stream) {
+                                          const int* cur_dev, int T, float scale, int window, void* stream) {
   DALM_REQUIRE(B > 0 && Hq > 0 && Hkv > 0 && (Hq % Hkv) == 0, "attention_decode: bad heads B=%d Hq=%d Hkv=%d", B, Hq, Hkv);
   DALM_REQUIRE(D == 32 || D == 64 || D == 128, "attention_decode: head_dim %d unsupported (32/64/128)", D);
   DALM_REQUIRE(T > 0 && T <= 8192 && (cur_dev != nullptr || (cur >= 0 && cur < T)),
@@ -638,6 +641,7 @@ extern "C" int dalm_b200_attention_decode(const void* qkv, long long ldq, int q_
   DALM_REQUIRE(((uintptr_t)qkv & 15) == 0 && ((uintptr_t)cache_k & 15) == 0 && ((uintptr_t)cache_v & 15) == 0,
                "attention_decode: pointers must be 16-byte aligned");
   DALM_REQUIRE(mask != nullptr && cache_st >= (long long)Hkv * D && cache_sb >= cache_st * T, "attention_decode: cache layout");
+  DALM_REQUIRE(window >= 0, "attention_decode: window %d must be >= 0 (0 = no window)", window);
   const int sp_cap = ((cur_dev ? T : cur + 1) + 3) & ~3;
   const size_t smem = (size_t)(D + sp_cap + 32 + 1024) * sizeof(float);
   dim3 grid(Hq, B);
@@ -645,7 +649,7 @@ extern "C" int dalm_b200_attention_decode(const void* qkv, long long ldq, int q_
   attn_decode_kernel<DD><<<grid, 128, smem, ST(stream)>>>((const __nv_bfloat16*)qkv, ldq, q_col, k_col, v_col,           \
                                                           (__nv_bfloat16*)cache_k, (__nv_bfloat16*)cache_v, cache_sb,    \
                                                           cache_st, mask, ldm, (__nv_bfloat16*)out, ldo, Hq, Hkv, cur,     \
-                                                          cur_dev, sp_cap, scale)
+                                                          cur_dev, sp_cap, scale, window)
   if (D == 128) DALM_DECODE(128); else if (D == 64) DALM_DECODE(64); else DALM_DECODE(32);
 #undef DALM_DECODE
   count_launch();

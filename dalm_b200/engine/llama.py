@@ -1,4 +1,4 @@
-"""Llama / Qwen2 / Qwen3 decoder (Llama-2-7B / Qwen2.5-7B / Qwen3-8B shape and smaller) forward + backward as a launch sequence over the C-ABI kernels.
+"""Llama / Qwen2 / Qwen3 / Mistral decoder (Llama-2-7B / Qwen2.5-7B / Qwen3-8B / Mistral-7B shape and smaller) forward + backward as a launch sequence over the C-ABI kernels.
 
 Mirrors `self.generator_model(input_ids=..., attention_mask=...).logits` of the reference
 (dalm/models/rag_e2e_base_model.py:104-106) through HF LlamaForCausalLM: embed -> N x [RMSNorm -> QKV(+LoRA on q,v)
@@ -17,6 +17,10 @@ fused into the QKV GEMM's RoPE epilogue (training shapes) or applied by the qk_n
 widths); the backward saves the pre-norm q|k columns and their rstd. Configs are checked by params.check_llama_family.
 Llama 3.x is this architecture with GQA and frequency-scaled RoPE: params.rope_inv_freq builds the default, `linear` and
 `llama3` frequencies, and every RoPE kernel reads the cos / sin tables `_rope` makes from them.
+Mistral (HF MistralForCausalLM) is Llama with sliding-window causal attention: params.sliding_windows gives each layer's key
+window (0 = none; also Qwen2 / Qwen3 with use_sliding_window), and every attention launch of that layer (training forward and
+backward, prefill, decode) takes it. Headless checkpoints (HF MistralModel / LlamaModel saved by AutoModel, e.g.
+e5-mistral-7b-instruct: `layers.*` with no `model.` prefix and no lm_head) load too; hf_state_dict writes their layout back.
 """
 from __future__ import annotations
 
@@ -27,7 +31,7 @@ import torch
 from .. import ops
 from .dense import DenseBank
 from .lora import LoraBank
-from .params import attention_biases, check_llama_family, rope_inv_freq
+from .params import attention_biases, check_llama_family, rope_inv_freq, sliding_windows
 
 bf16, f32 = torch.bfloat16, torch.float32
 
@@ -42,6 +46,11 @@ def _aug_buf(rows: int, cols: int, ra: int, device, zero: bool = False) -> torch
 
 class _Ctx:
     pass
+
+
+def _with_prefix(sd: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
+    """a headless (AutoModel) state dict under LlamaForCausalLM names: every key gains `model.` (it has no lm_head)"""
+    return {"model." + k: v for k, v in sd.items()}
 
 
 class LlamaDecoder(torch.nn.Module):
@@ -64,7 +73,7 @@ class LlamaDecoder(torch.nn.Module):
             self.nf4 = Nf4Store(device)
         check_llama_family(cfg)
         self.cfg = cfg
-        self.kind = cfg.get("model_type") if cfg.get("model_type") in ("qwen2", "qwen3") else "llama"
+        self.kind = cfg.get("model_type") if cfg.get("model_type") in ("qwen2", "qwen3", "mistral") else "llama"
         self.qkv_bias, self.o_bias = attention_biases(self.kind, cfg)
         self.qk_norm = self.kind == "qwen3"
         self.H = H = cfg["hidden_size"]
@@ -79,11 +88,14 @@ class LlamaDecoder(torch.nn.Module):
         if self.hd not in (32, 64, 128):
             raise NotImplementedError(f"head_dim {self.hd} not supported by the attention kernels")
         self.inv_freq = rope_inv_freq(cfg, self.hd)           # default, linear or llama3 frequencies (fp32, CPU)
+        self.windows = sliding_windows(cfg)                   # key window of each layer, 0 = full causal attention
         self.Nq, self.Nkv = self.nh * self.hd, self.nkv * self.hd
         self.Nqkv = self.Nq + 2 * self.Nkv
         self.r = 8
         self.Ra = 2 * self.r if lora else 0
-        sd = state_dict
+        # headless checkpoints (AutoModel: embed_tokens.*, layers.*, norm.*) are read under the model.-prefixed names
+        self.headless = not any(k.startswith("model.") for k in state_dict)
+        sd = _with_prefix(state_dict) if self.headless else state_dict
         if self.nf4 is not None:
             g = lambda k, dt: sd[k].to(device=self.dev, dtype=torch.float16).to(dt).contiguous()
         else:
@@ -193,18 +205,21 @@ class LlamaDecoder(torch.nn.Module):
                                 "kn": bank.w32(k("kn")) if self.qk_norm else None})
 
     def hf_state_dict(self) -> Dict[str, torch.Tensor]:
-        """fp32 CPU tensors under HF LlamaForCausalLM names (save_pretrained of a fully fine-tuned decoder)"""
+        """fp32 CPU tensors under HF LlamaForCausalLM names (save_pretrained of a fully fine-tuned decoder), or under the
+        unprefixed names of a headless checkpoint when the decoder was loaded from one"""
         if self.full is None:
             raise RuntimeError("hf_state_dict: only fully fine-tuned models own their weights (PEFT mode saves adapters)")
         out = {}
         for key, parts in self._rows.items():
             w, r = self.full.w32(key), 0
             for name, rows in parts:
-                out[name] = w[r:r + rows].detach().cpu().clone()
+                out[name[len("model."):] if self.headless else name] = w[r:r + rows].detach().cpu().clone()
                 r += rows
         return out
 
     def load_hf_state_dict(self, sd: Dict[str, torch.Tensor]) -> None:
+        if not any(k.startswith("model.") for k in sd):
+            sd = _with_prefix(sd)
         for key, parts in self._rows.items():
             w, r = self.full.w32(key), 0
             for name, rows in parts:
@@ -456,7 +471,8 @@ class LlamaDecoder(torch.nn.Module):
             if kv_sink is not None:
                 kv_sink(li, a.qkv)
             a.att, a.lse = ops.attention_auto_fwd(a.qkv[:, :self.Nq], a.qkv[:, self.Nq:self.Nq + self.Nkv],
-                                                  a.qkv[:, self.Nq + self.Nkv:], ctx.mask, B, L, self.nh, self.nkv, self.hd, causal=True)
+                                                  a.qkv[:, self.Nq + self.Nkv:], ctx.mask, B, L, self.nh, self.nkv, self.hd, causal=True,
+                                                  window=self.windows[li])
             a.x_mid = ops.gemm(a.att, W["Wo"], out_dtype=f32, resid=x, bias=W["bo"])
             a.h2, a.rstd2 = ops.rmsnorm_fwd(a.x_mid, W["g2"], self.eps)
             if self.gu_il:
@@ -491,7 +507,7 @@ class LlamaDecoder(torch.nn.Module):
             else:
                 ops.rope_pos_(qkv, 0, self.nh + self.nkv, self.hd, cos_t, sin_t, pos)
             att = ops.attention_decode(qkv, 0, self.Nq, self.Nq + self.Nkv, caches[li][0], caches[li][1], kmask, cur,
-                                       self.nh, self.nkv, self.hd)
+                                       self.nh, self.nkv, self.hd, window=self.windows[li])
             x_mid = ops.gemm_rows(att, W["Wo"], out_dtype=f32, resid=x, bias=W["bo"])
             h2, _ = ops.rmsnorm_fwd(x_mid, W["g2"], self.eps)
             act = ops.swiglu_fwd(ops.gemm_rows(h2, W["Wgu"]), F, interleave=self.gu_il)
@@ -572,7 +588,7 @@ class LlamaDecoder(torch.nn.Module):
             ops.attention_auto_bwd(a.qkv[:, :self.Nq], a.qkv[:, self.Nq:self.Nq + self.Nkv], a.qkv[:, self.Nq + self.Nkv:],
                      ctx.mask, a.att, a.lse, datt, B, L, self.nh, self.nkv, self.hd, causal=True,
                      dq=dqkv[:, :self.Nq], dk=dqkv[:, self.Nq:self.Nq + self.Nkv],
-                     dv=dqkv[:, self.Nq + self.Nkv:self.Nqkv])
+                     dv=dqkv[:, self.Nq + self.Nkv:self.Nqkv], window=self.windows[l])
             if self.qk_norm:                                                       # un-rotate, then the q/k RMSNorm backward
                 ops.qk_norm_rope_bwd_(dqkv, self.nh + self.nkv, self.nh, W["qn"], W["kn"], cos_t, sin_t, L, a.pre, a.qk_rstd,
                                       dw_q=G(l, "qn") if bank is not None else None, dw_k=G(l, "kn") if bank is not None else None)

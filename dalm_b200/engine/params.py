@@ -4,7 +4,7 @@ from __future__ import annotations
 import json
 import math
 import os
-from typing import Dict, Optional
+from typing import Dict, List, Optional
 
 import torch
 
@@ -22,7 +22,7 @@ def _normal(gen: torch.Generator, shape, std: float, dtype, device) -> torch.Ten
 def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, device="cpu",
                       bias_std: Optional[float] = None, qk_norm_std: Optional[float] = None) -> Dict[str, torch.Tensor]:
     """HF parameter names for BertModel / XLMRobertaModel / RobertaModel (no prefix) / LlamaForCausalLM / Qwen2ForCausalLM /
-    Qwen3ForCausalLM / FalconForCausalLM, init N(0, initializer_range), LN = (1, 0). Decoder attention biases (Qwen2's q/k/v, Llama's and Qwen3's
+    Qwen3ForCausalLM / MistralForCausalLM / FalconForCausalLM, init N(0, initializer_range), LN = (1, 0). Decoder attention biases (Qwen2's q/k/v, Llama's and Qwen3's
     `attention_bias`) are drawn from N(0, bias_std) (default: initializer_range) rather than HF's zeros, so that a dropped bias
     changes the outputs. Qwen3's q_norm / k_norm weights are 1 + N(0, qk_norm_std) (default: initializer_range), so that a
     dropped or swapped norm shows."""
@@ -58,7 +58,7 @@ def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, 
             sd[p + "output.LayerNorm.bias"] = _normal(gen, (H,), std, dtype, device)
         sd["pooler.dense.weight"] = _normal(gen, (H, H), std, dtype, device)   # loaded by AutoModel, unused by the path
         sd["pooler.dense.bias"] = zeros(H)
-    elif kind in ("llama", "qwen2", "qwen3"):
+    elif kind in ("llama", "qwen2", "qwen3", "mistral"):
         F, V = cfg["intermediate_size"], cfg["vocab_size"]
         nh, nkv = cfg["num_attention_heads"], cfg.get("num_key_value_heads", cfg["num_attention_heads"])
         hd = cfg.get("head_dim") or H // nh
@@ -155,14 +155,14 @@ def model_kind(cfg: Dict) -> str:
     if mt in ("roberta", "xlm-roberta"):
         check_roberta(cfg)
         return "roberta"
-    if mt in ("llama", "qwen2", "qwen3"):
+    if mt in ("llama", "qwen2", "qwen3", "mistral"):
         check_llama_family(cfg)
         return mt
     if mt == "falcon":
         check_rope_type(cfg)
         return "falcon"
     raise NotImplementedError(
-        f"model_type {mt!r} is not built in dalm_b200 (supported: bert, roberta and xlm-roberta encoders; llama, qwen2, qwen3 and falcon decoders)")
+        f"model_type {mt!r} is not built in dalm_b200 (supported: bert, roberta and xlm-roberta encoders; llama, qwen2, qwen3, mistral and falcon decoders)")
 
 
 def _rope_type(cfg: Dict) -> str:
@@ -228,22 +228,66 @@ def rope_inv_freq(cfg: Dict, head_dim: int) -> torch.Tensor:
 
 
 def check_llama_family(cfg: Dict) -> None:
-    """refuses the settings of a llama / qwen2 / qwen3 config that LlamaDecoder would otherwise silently compute wrong"""
+    """refuses the settings of a llama / qwen2 / qwen3 / mistral config that LlamaDecoder would otherwise silently compute wrong"""
     mt = cfg.get("model_type", "")
-    if mt == "llama":
+    if mt == "mistral":
+        missing = [k for k in MISTRAL_SHAPE_KEYS if k not in cfg]
+        if missing:
+            raise NotImplementedError(f"mistral: a config without {', '.join(missing)} is not built (transformers would fill "
+                                      "in MistralConfig's defaults, the 7B shape; the shape is read from config.json only)")
+    if mt in ("llama", "mistral"):
         check_rope_type(cfg)
-    if cfg.get("mlp_bias", False):
+    if mt != "mistral" and cfg.get("mlp_bias", False):        # MistralMLP has no bias whatever the key says
         raise NotImplementedError(f"{mt}: mlp_bias=true is not built (the fused SwiGLU MLP has no bias)")
     if mt == "qwen3":
         hd = cfg.get("head_dim") or cfg["hidden_size"] // cfg["num_attention_heads"]
         if hd != 128:
             raise NotImplementedError(f"qwen3: head_dim={hd} is not built (the q/k norm kernels take head_dim 128)")
     if mt in ("qwen2", "qwen3"):
-        if cfg.get("use_sliding_window", False) or "sliding_attention" in (cfg.get("layer_types") or ()):
-            raise NotImplementedError(f"{mt}: sliding-window attention (use_sliding_window=true) is not built")
+        if not cfg.get("use_sliding_window", False) and "sliding_attention" in (cfg.get("layer_types") or ()):
+            # transformers then sets sliding_window to None but still builds sliding-window masks for those layers
+            raise NotImplementedError(f"{mt}: layer_types marks sliding_attention layers while use_sliding_window is false")
+        if cfg.get("use_sliding_window", False) and not any(sliding_windows(cfg)):
+            # transformers then runs full attention on every layer, while the Qwen documentation of max_window_layers reads
+            # the other way round (the first max_window_layers layers windowed): the config does not say which it means
+            raise NotImplementedError(
+                f"{mt}: use_sliding_window=true selects no sliding-window layer (sliding_window="
+                f"{cfg.get('sliding_window', 4096)}, max_window_layers={cfg.get('max_window_layers', 28)} of "
+                f"{cfg.get('num_hidden_layers')} layers, layer_types={cfg.get('layer_types')}); set use_sliding_window=false "
+                "or list the sliding_attention layers in layer_types")
         rt = _rope_type(cfg)
         if rt != "default":
             raise NotImplementedError(f"{mt}: RoPE type {rt!r} (rope_scaling / rope_parameters) is not built; only 'default'")
+
+
+MISTRAL_DEFAULT_WINDOW = 4096                                    # MistralConfig's sliding_window when the key is absent
+MISTRAL_SHAPE_KEYS = ("hidden_size", "intermediate_size", "num_hidden_layers", "num_attention_heads", "vocab_size")
+
+
+def sliding_windows(cfg: Dict) -> List[int]:
+    """the key window of every layer (0 = full causal attention), resolved as transformers' config classes resolve it:
+    - mistral: `sliding_window` for every layer; an absent key means 4096, null means none. MistralConfig ignores
+      `layer_types` (alternating layers are Ministral, another model type), and so does this.
+    - qwen2 / qwen3: `sliding_window` only with `use_sliding_window`, on the layers `layer_types` marks "sliding_attention",
+      or when that list is absent on layers i >= `max_window_layers` (default 28).
+    - llama: none.
+    A layer with window w lets query i see key j iff i - w < j <= i, in the indices of the padded row."""
+    mt, n = cfg.get("model_type", ""), int(cfg["num_hidden_layers"])
+    if mt == "mistral":
+        w = cfg.get("sliding_window", MISTRAL_DEFAULT_WINDOW)
+        return [int(w) if w else 0] * n
+    if mt in ("qwen2", "qwen3"):
+        w = cfg.get("sliding_window", 4096)
+        if not cfg.get("use_sliding_window", False) or not w:
+            return [0] * n
+        types = cfg.get("layer_types")
+        if types is None:
+            first = int(cfg.get("max_window_layers", 28))
+            types = ["sliding_attention" if i >= first else "full_attention" for i in range(n)]
+        if len(types) != n:
+            raise ValueError(f"{mt}: layer_types lists {len(types)} layers, num_hidden_layers is {n}")
+        return [int(w) if t == "sliding_attention" else 0 for t in types]
+    return [0] * n
 
 
 def check_roberta(cfg: Dict) -> None:
@@ -269,9 +313,11 @@ def roberta_max_len(cfg: Dict) -> int:
 
 def attention_biases(kind: str, cfg: Dict):
     """(q/k/v projections carry a bias, o_proj carries a bias) for a llama-family config: Qwen2 has q/k/v biases only, Llama
-    and Qwen3 have all four when `attention_bias` is set"""
+    and Qwen3 have all four when `attention_bias` is set, Mistral has none (MistralAttention ignores the key)"""
     if kind == "qwen2":
         return True, False
+    if kind == "mistral":
+        return False, False
     ab = bool(cfg.get("attention_bias", False))
     return ab, ab
 

@@ -65,7 +65,8 @@ def load_tokenizer(name_or_path: str):
 
 def build_encoder(name_or_path: str, lora: bool, device: torch.device, state_dict: Optional[Dict] = None,
                   cfg: Optional[Dict] = None, autoregressive: bool = False, full: bool = False, bnb: bool = False):
-    """BERT-family encoder (bge-*) or (XLM-)RoBERTa encoder (multilingual-e5, bge-m3, xlm-roberta-*), or — `retriever_is_autoregressive` — a Llama / Qwen2 / Qwen3 decoder used as an encoder
+    """BERT-family encoder (bge-*) or (XLM-)RoBERTa encoder (multilingual-e5, bge-m3, xlm-roberta-*), or — `retriever_is_autoregressive` — a Llama / Qwen2 / Qwen3 /
+    Mistral decoder (e5-mistral-7b-instruct, SFR-Embedding-Mistral) used as an encoder
     (last hidden state, eos pooling; LoRA targets q_proj / v_proj: reference rag_e2e_base_model.py:66-70,84-90)"""
     cfg = cfg or params.load_config(name_or_path)
     kind = params.model_kind(cfg)
@@ -74,8 +75,9 @@ def build_encoder(name_or_path: str, lora: bool, device: torch.device, state_dic
     if not nf4:
         sd = _maybe_bnb(sd, bnb, full, device)
     if autoregressive:
-        if kind not in ("llama", "qwen2", "qwen3"):
-            raise NotImplementedError("autoregressive retrievers are built for Llama, Qwen2 and Qwen3 models only")
+        if kind not in ("llama", "qwen2", "qwen3", "mistral"):
+            raise NotImplementedError("autoregressive retrievers are built for Llama, Qwen2 and Qwen3 models only; Mistral "
+                                      "runs as Llama with a sliding window")
         return _named(LlamaDecoder(cfg, sd, device=device, lora=lora, lora_seed=0, full=full, nf4_storage=nf4), name_or_path)
     if kind not in ("bert", "roberta"):
         raise NotImplementedError("non-autoregressive retrievers must be BERT (bge-*) or (XLM-)RoBERTa (multilingual-e5, bge-m3) "
@@ -132,7 +134,7 @@ def build_decoder(name_or_path: str, lora: bool, device: torch.device, state_dic
         sd = _maybe_bnb(sd, bnb, full, device)
     if kind == "falcon":
         dec = FalconDecoder(cfg, sd, device=device, lora=lora, full=full)      # raises for lora=True, like peft would
-    elif kind not in ("llama", "qwen2", "qwen3"):
+    elif kind not in ("llama", "qwen2", "qwen3", "mistral"):
         raise NotImplementedError(f"generator of kind {kind!r} is not a causal decoder")
     else:
         dec = LlamaDecoder(cfg, sd, device=device, lora=lora, full=full, nf4_storage=nf4)

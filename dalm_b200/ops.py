@@ -296,7 +296,7 @@ GEMM_MAX_CTAS = 0
 # ----------------------------------------------------------------------------------------------------------------
 # attention
 # ----------------------------------------------------------------------------------------------------------------
-def _attention_fwd(sym, q, k, v, mask, B, L, Hq, Hkv, D, causal, out, scale, drop):
+def _attention_fwd(sym, q, k, v, mask, B, L, Hq, Hkv, D, causal, out, scale, drop, window):
     for t, n in ((q, "q"), (k, "k"), (v, "v")):
         _chk(t, bf16, n)
     if out is None:
@@ -306,11 +306,11 @@ def _attention_fwd(sym, q, k, v, mask, B, L, Hq, Hkv, D, causal, out, scale, dro
         raise _lib.DalmB200Error("attention: mask must be int64")
     scale = 1.0 / math.sqrt(D) if scale is None else scale
     _lib.call(sym, _p(q), _ld(q), _p(k), _ld(k), _p(v), _ld(v), _p(mask), _p(out), _ld(out),
-              _p(lse), B, L, Hq, Hkv, D, float(scale), 1 if causal else 0, *_d(drop), _stream())
+              _p(lse), B, L, Hq, Hkv, D, float(scale), 1 if causal else 0, int(window), *_d(drop), _stream())
     return out, lse
 
 
-def _attention_bwd(sym, q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq, dk, dv, scale, drop):
+def _attention_bwd(sym, q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq, dk, dv, scale, drop, window):
     dev = q.device
     if dq is None: dq = torch.empty(B * L, Hq * D, dtype=bf16, device=dev)
     if dk is None: dk = torch.empty(B * L, Hkv * D, dtype=bf16, device=dev)
@@ -319,46 +319,52 @@ def _attention_bwd(sym, q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal
     scale = 1.0 / math.sqrt(D) if scale is None else scale
     _lib.call(sym, _p(q), _ld(q), _p(k), _ld(k), _p(v), _ld(v), _p(mask), _p(out), _ld(out),
               _p(lse), _p(d_out), _ld(d_out), _p(delta), _p(dq), _ld(dq), _p(dk), _ld(dk), _p(dv), _ld(dv),
-              B, L, Hq, Hkv, D, float(scale), 1 if causal else 0, *_d(drop), _stream())
+              B, L, Hq, Hkv, D, float(scale), 1 if causal else 0, int(window), *_d(drop), _stream())
     return dq, dk, dv
 
 
 def attention_fwd(q, k, v, mask, B: int, L: int, Hq: int, Hkv: int, D: int, causal: bool, out=None,
-                  scale: Optional[float] = None, drop: Optional[Drop] = None):
+                  scale: Optional[float] = None, drop: Optional[Drop] = None, window: int = 0):
     """mma.sync attention forward (head_dim 32/64/128). q/k/v: bf16 token-major 2-D views [B*L, H*D] (may be column slices
-    of one qkv buffer). -> (out, lse)"""
-    return _attention_fwd("dalm_b200_attention_fwd", q, k, v, mask, B, L, Hq, Hkv, D, causal, out, scale, drop)
+    of one qkv buffer). window > 0 (causal only): query i sees key j iff i - window < j <= i (Mistral's sliding window,
+    counted in the padded row); 0 = no window. -> (out, lse)"""
+    return _attention_fwd("dalm_b200_attention_fwd", q, k, v, mask, B, L, Hq, Hkv, D, causal, out, scale, drop, window)
 
 
 def attention_bwd(q, k, v, mask, out, lse, d_out, B: int, L: int, Hq: int, Hkv: int, D: int, causal: bool,
-                  dq=None, dk=None, dv=None, scale: Optional[float] = None, drop: Optional[Drop] = None):
-    """mma.sync attention backward. -> (dq, dk, dv)"""
-    return _attention_bwd("dalm_b200_attention_bwd", q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq, dk, dv, scale, drop)
+                  dq=None, dk=None, dv=None, scale: Optional[float] = None, drop: Optional[Drop] = None, window: int = 0):
+    """mma.sync attention backward (the window must be the forward's). -> (dq, dk, dv)"""
+    return _attention_bwd("dalm_b200_attention_bwd", q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq, dk, dv, scale, drop,
+                          window)
 
 
 def attention_tc_fwd(q, k, v, mask, B: int, L: int, Hq: int, Hkv: int, D: int, causal: bool, out=None,
-                     scale: Optional[float] = None, drop: Optional[Drop] = None):
+                     scale: Optional[float] = None, drop: Optional[Drop] = None, window: int = 0):
     """wgmma/TMA attention forward (head_dim 128 or 64; probability dropout at 64). Same contract as attention_fwd."""
-    return _attention_fwd("dalm_b200_attention_tc_fwd", q, k, v, mask, B, L, Hq, Hkv, D, causal, out, scale, drop)
+    return _attention_fwd("dalm_b200_attention_tc_fwd", q, k, v, mask, B, L, Hq, Hkv, D, causal, out, scale, drop, window)
 
 
 def attention_tc_bwd(q, k, v, mask, out, lse, d_out, B: int, L: int, Hq: int, Hkv: int, D: int, causal: bool,
-                     dq=None, dk=None, dv=None, scale: Optional[float] = None, drop: Optional[Drop] = None):
+                     dq=None, dk=None, dv=None, scale: Optional[float] = None, drop: Optional[Drop] = None, window: int = 0):
     """wgmma/TMA attention backward (head_dim 128 or 64). Same contract as attention_bwd."""
-    return _attention_bwd("dalm_b200_attention_tc_bwd", q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq, dk, dv, scale, drop)
+    return _attention_bwd("dalm_b200_attention_tc_bwd", q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq, dk, dv, scale, drop,
+                          window)
 
 
-def attention_auto_fwd(q, k, v, mask, B, L, Hq, Hkv, D, causal, out=None, scale=None, drop=None):
+def attention_auto_fwd(q, k, v, mask, B, L, Hq, Hkv, D, causal, out=None, scale=None, drop=None, window: int = 0):
     """head_dim 64 / 128 -> wgmma kernels; head_dim 32 (bge-small) -> mma.sync kernels."""
     if D in (64, 128):
-        return attention_tc_fwd(q, k, v, mask, B, L, Hq, Hkv, D, causal, out=out, scale=scale, drop=drop)
-    return attention_fwd(q, k, v, mask, B, L, Hq, Hkv, D, causal, out=out, scale=scale, drop=drop)
+        return attention_tc_fwd(q, k, v, mask, B, L, Hq, Hkv, D, causal, out=out, scale=scale, drop=drop, window=window)
+    return attention_fwd(q, k, v, mask, B, L, Hq, Hkv, D, causal, out=out, scale=scale, drop=drop, window=window)
 
 
-def attention_auto_bwd(q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq=None, dk=None, dv=None, scale=None, drop=None):
+def attention_auto_bwd(q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq=None, dk=None, dv=None, scale=None, drop=None,
+                       window: int = 0):
     if D in (64, 128):
-        return attention_tc_bwd(q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq=dq, dk=dk, dv=dv, scale=scale, drop=drop)
-    return attention_bwd(q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq=dq, dk=dk, dv=dv, scale=scale, drop=drop)
+        return attention_tc_bwd(q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq=dq, dk=dk, dv=dv, scale=scale, drop=drop,
+                                window=window)
+    return attention_bwd(q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq=dq, dk=dk, dv=dv, scale=scale, drop=drop,
+                         window=window)
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -915,9 +921,10 @@ def _cur_arg(cur, B: int, what: str):
 
 
 def attention_decode(qkv, q_col: int, k_col: int, v_col: int, cache_k, cache_v, mask, cur, Hq: int, Hkv: int, D: int,
-                     out=None, scale: Optional[float] = None):
+                     out=None, scale: Optional[float] = None, window: int = 0):
     """qkv bf16 [B, >=v_col+Hkv*D] (current token of every sequence); cache_k / cache_v bf16 [B, T, Hkv*D]; mask int64 [B, T].
-    Appends the token's K / V at column `cur` (int, or int32 [B] device tensor) and returns the attention output bf16 [B, Hq*D]."""
+    Appends the token's K / V at column `cur` (int, or int32 [B] device tensor) and returns the attention output bf16 [B, Hq*D].
+    window > 0: only columns t > cur - window are visible (0 = no window)."""
     _chk(qkv, bf16, "attention_decode qkv"); _chk(cache_k, bf16, "cache_k"); _chk(cache_v, bf16, "cache_v"); _chk(mask, i64, "mask")
     B, T = cache_k.shape[0], cache_k.shape[1]
     if cache_k.shape != cache_v.shape or cache_k.stride() != cache_v.stride() or cache_k.dim() != 3 or mask.shape[0] != B or mask.shape[1] < T:
@@ -930,7 +937,7 @@ def attention_decode(qkv, q_col: int, k_col: int, v_col: int, cache_k, cache_v, 
     cur_host, cur_dev = _cur_arg(cur, B, "attention_decode")
     _lib.call("dalm_b200_attention_decode", _p(qkv), _ld(qkv), q_col, k_col, v_col, _p(cache_k), _p(cache_v),
               cache_k.stride(0), cache_k.stride(1), _p(mask), mask.stride(0), _p(out), _ld(out), B, Hq, Hkv, D, cur_host, cur_dev,
-              T, float(scale), _stream())
+              T, float(scale), int(window), _stream())
     return out
 
 

@@ -97,6 +97,29 @@ ROBERTA_SHAPES: Dict[str, Dict] = {
 }
 
 
+# Mistral (model_type "mistral"): Llama's layer with GQA and sliding-window causal attention. The tiny shapes cover the fused
+# RoPE epilogue (head_dim 128) and the RoPE row kernel (head_dim 64, an odd window below one 64-key tile), and a config
+# without a window. The published shapes were written from memory of their config.json files and could not be re-checked
+# offline. `headless`: saved as MistralModel (AutoModel: no `model.` prefix, no lm_head), like e5-mistral-7b-instruct and
+# SFR-Embedding-Mistral.
+MISTRAL_SHAPES: Dict[str, Dict] = {
+    "mistral-tiny": dict(hidden_size=512, num_hidden_layers=2, num_attention_heads=4, num_key_value_heads=2, head_dim=128,
+                         intermediate_size=1024, sliding_window=48),            # 6 q|k heads x 128: RoPE in the QKV epilogue
+    "mistral-hd64": dict(hidden_size=256, num_hidden_layers=2, num_attention_heads=4, num_key_value_heads=2, head_dim=64,
+                         intermediate_size=512, sliding_window=37),
+    "mistral-nowin": dict(hidden_size=256, num_hidden_layers=2, num_attention_heads=4, num_key_value_heads=2, head_dim=64,
+                          intermediate_size=512, sliding_window=None),
+    "Mistral-7B-v0.1": dict(hidden_size=4096, num_hidden_layers=32, num_attention_heads=32, num_key_value_heads=8, head_dim=128,
+                            intermediate_size=14336, sliding_window=4096, rope_theta=10000.0, vocab_size=32000),
+    "Mistral-7B-v0.3": dict(hidden_size=4096, num_hidden_layers=32, num_attention_heads=32, num_key_value_heads=8, head_dim=128,
+                            intermediate_size=14336, sliding_window=None, rope_theta=1000000.0, vocab_size=32768),
+    "e5-mistral-7b-instruct": dict(hidden_size=4096, num_hidden_layers=32, num_attention_heads=32, num_key_value_heads=8,
+                                   head_dim=128, intermediate_size=14336, sliding_window=4096, rope_theta=10000.0,
+                                   vocab_size=32000, headless=True),
+    "Mistral-Nemo-Base-2407": dict(hidden_size=5120, num_hidden_layers=40, num_attention_heads=32, num_key_value_heads=8,
+                                   head_dim=128, intermediate_size=14336, sliding_window=None, rope_theta=1000000.0,
+                                   vocab_size=131072, max_position_embeddings=1024000),
+}
 FALCON_SHAPES: Dict[str, Dict] = {
     "falcon-tiny": dict(hidden_size=128, num_hidden_layers=2, num_attention_heads=2),
     "falcon-mini": dict(hidden_size=448, num_hidden_layers=2, num_attention_heads=7),          # 7 q heads x 64, one KV head
@@ -164,6 +187,24 @@ def llama3_config(name: str, vocab_size: int = 128256) -> Dict:
         hidden_act="silu", rms_norm_eps=1e-5, rope_theta=500000.0, rope_scaling=rs, initializer_range=0.02, bos_token_id=0,
         eos_token_id=1, attention_bias=False, mlp_bias=False, attention_dropout=0.0, pretraining_tp=1, **s,
     )
+
+
+def mistral_config(name: str, vocab_size: Optional[int] = None) -> Dict:
+    """Mistral (HF MistralForCausalLM, or MistralModel for a headless shape): Llama-2's layer with GQA, rms_norm_eps 1e-5, no
+    biases and a `sliding_window` (null = none). Token ids follow the Llama SentencePiece layout (<unk> = 0, <s> = 1,
+    </s> = 2), which the published tokenizers share."""
+    s = dict(MISTRAL_SHAPES[name])
+    headless = s.pop("headless", False)
+    cfg = dict(
+        architectures=["MistralModel" if headless else "MistralForCausalLM"], model_type="mistral",
+        vocab_size=s.pop("vocab_size", 32000), max_position_embeddings=32768, hidden_act="silu", rms_norm_eps=1e-5,
+        rope_theta=s.pop("rope_theta", 10000.0), initializer_range=0.02, bos_token_id=1, eos_token_id=2,
+        tie_word_embeddings=False, attention_dropout=0.0,
+    )
+    cfg.update(s)
+    if vocab_size:
+        cfg["vocab_size"] = vocab_size
+    return cfg
 
 
 def qwen2_config(name: str, vocab_size: int = 152064) -> Dict:
@@ -442,10 +483,11 @@ QWEN3_GENERATION = {
 # ---------------------------------------------------------------------------------------------------------------
 def write_model_dir(out_dir: str, kind: str, name: str, vocab_size: Optional[int] = None, with_weights: bool = True,
                     seed: int = 0, generation_config: Optional[Dict] = None, bias_std: Optional[float] = None,
-                    qk_norm_std: Optional[float] = None) -> str:
-    """kind: 'bert' | 'roberta' | 'llama' | 'qwen2' | 'qwen3' | 'falcon' ('roberta' takes a ROBERTA_SHAPES name: XLM-R shapes get
-    the XLM-R tokenizer, roberta-tiny the byte-level one; a Llama 3.x shape of LLAMA3_SHAPES takes kind 'llama' and gets the
-    Llama 3 tokenizer). Writes config.json, tokenizer files and (optionally) seeded random-init
+                    qk_norm_std: Optional[float] = None, headless: Optional[bool] = None) -> str:
+    """kind: 'bert' | 'roberta' | 'llama' | 'qwen2' | 'qwen3' | 'mistral' | 'falcon' ('roberta' takes a ROBERTA_SHAPES name: XLM-R
+    shapes get the XLM-R tokenizer, roberta-tiny the byte-level one; a Llama 3.x shape of LLAMA3_SHAPES takes kind 'llama' and
+    gets the Llama 3 tokenizer; 'mistral' gets the Llama SentencePiece tokenizer). headless (mistral; default: the shape's own
+    setting): a MistralModel directory, weights without the `model.` prefix and without lm_head. Writes config.json, tokenizer files and (optionally) seeded random-init
     safetensors in HF parameter naming so both transformers (oracle) and dalm_b200 (product) can load the same directory.
     generation_config: written as generation_config.json when given (e.g. QWEN2_GENERATION["base"]). bias_std: std of the
     random attention biases, qk_norm_std the spread of Qwen3's q / k norm weights around 1 (engine/params.random_state_dict)."""
@@ -471,6 +513,11 @@ def write_model_dir(out_dir: str, kind: str, name: str, vocab_size: Optional[int
     elif kind == "qwen3":
         cfg = qwen3_config(name, vocab_size or 151936)
         build_qwen2_tokenizer(out_dir, cfg["vocab_size"])          # Qwen3 keeps Qwen2's byte-level BPE and Qwen2Tokenizer
+    elif kind == "mistral":
+        cfg = mistral_config(name, vocab_size)
+        if headless is not None:
+            cfg["architectures"] = ["MistralModel" if headless else "MistralForCausalLM"]
+        build_llama_tokenizer(out_dir, cfg["vocab_size"])
     elif kind == "falcon":
         cfg = falcon_config(name, vocab_size or 65024)
         build_llama_tokenizer(out_dir, cfg["vocab_size"])       # any causal-LM tokenizer works for the synthetic fixture
@@ -491,5 +538,12 @@ def write_model_dir(out_dir: str, kind: str, name: str, vocab_size: Optional[int
         from .engine.params import random_state_dict
 
         sd = random_state_dict(kind, cfg, seed=seed, dtype=torch.float32, device="cpu", bias_std=bias_std, qk_norm_std=qk_norm_std)
+        if cfg.get("architectures") == ["MistralModel"]:
+            sd = headless_state_dict(sd)
         save_file({k: v.contiguous() for k, v in sd.items()}, os.path.join(out_dir, "model.safetensors"))
     return out_dir
+
+
+def headless_state_dict(sd: Dict) -> Dict:
+    """a CausalLM state dict as its base model saves it (AutoModel / MistralModel): `model.` stripped, lm_head dropped"""
+    return {k[len("model."):]: v for k, v in sd.items() if k.startswith("model.")}

@@ -116,14 +116,16 @@ void dalm_b200_gemm_set_raster(int group_m);
 void dalm_b200_gemm_set_l2_hints(int mask);
 
 /* ---- attention (same call sites; HF eager/SDPA attention) ---- */
+/* window: 0 = no window; > 0 (causal only) = sliding window, query i sees key j iff i - window < j <= i, counted in the
+ * padded row (Mistral; Qwen2 / Qwen3 with use_sliding_window). Probability dropout is not built with a window. */
 int dalm_b200_attention_fwd(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv,
                             const int64_t* mask, void* out, long long ldo, float* lse, int B, int L, int Hq, int Hkv,
-                            int D, float scale, int causal, float drop_p, unsigned long long drop_seed,
+                            int D, float scale, int causal, int window, float drop_p, unsigned long long drop_seed,
     unsigned long long drop_stream_id, const void* drop_offset, void* stream);
 int dalm_b200_attention_bwd(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv,
                             const int64_t* mask, const void* out, long long ldo, const float* lse, const void* d_out,
                             long long lddo, float* delta, void* dq, long long lddq, void* dk, long long lddk, void* dv,
-                            long long lddv, int B, int L, int Hq, int Hkv, int D, float scale, int causal, float drop_p, unsigned long long drop_seed,
+                            long long lddv, int B, int L, int Hq, int Hkv, int D, float scale, int causal, int window, float drop_p, unsigned long long drop_seed,
     unsigned long long drop_stream_id, const void* drop_offset, void* stream);
 
 /* wgmma / TMA attention (Hopper tensor cores): head_dim 128 (Llama decoder) or 64 (bge-large encoder incl.
@@ -131,12 +133,12 @@ int dalm_b200_attention_bwd(const void* q, long long ldq, const void* k, long lo
  * as dalm_b200_attention_fwd / _bwd (the mma.sync kernels, kept for head_dim 32 and as a cross-check). */
 int dalm_b200_attention_tc_fwd(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv,
                                const int64_t* mask, void* out, long long ldo, float* lse, int B, int L, int Hq, int Hkv,
-                               int D, float scale, int causal, float drop_p, unsigned long long drop_seed,
+                               int D, float scale, int causal, int window, float drop_p, unsigned long long drop_seed,
                                unsigned long long drop_stream_id, const void* drop_offset, void* stream);
 int dalm_b200_attention_tc_bwd(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv,
                                const int64_t* mask, const void* out, long long ldo, const float* lse, const void* d_out,
                                long long lddo, float* delta, void* dq, long long lddq, void* dk, long long lddk, void* dv,
-                               long long lddv, int B, int L, int Hq, int Hkv, int D, float scale, int causal, float drop_p,
+                               long long lddv, int B, int L, int Hq, int Hkv, int D, float scale, int causal, int window, float drop_p,
                                unsigned long long drop_seed, unsigned long long drop_stream_id, const void* drop_offset,
                                void* stream);
 
@@ -242,6 +244,7 @@ int dalm_b200_nf4_dequant_bf16(const void* packed, const float* absmax, long lon
  * attention_decode: one query token per sequence (row b of qkv: q | k | v at the given columns, already rotated) against
  *   the bf16 KV cache [B][T][Hkv*D] (batch stride cache_sb, token stride cache_st, in elements); keys t < cur are visible
  *   iff mask[b*ldm + t] != 0, the token itself (column cur) always; its K / V rows are appended to the cache at column cur.
+ *   window > 0: only columns t > cur - window are visible (the sliding window of the training kernels).
  * greedy_step: next token = argmax(logits[b, 0..V)) for unfinished rows, pad_id for finished ones; writes tokens[b, col],
  *   mask[b, col] = 1, next_ids[b], pos[b] += 1; a row finishes when it emits one of eos_ids; alive[col] += #unfinished
  *   rows after this step (alive: int32 [T], zeroed by the caller).
@@ -272,7 +275,7 @@ int dalm_b200_qk_norm_rope_bwd(void* dbuf, long long ld, int nheads, int nq_head
 int dalm_b200_attention_decode(const void* qkv, long long ldq, int q_col, int k_col, int v_col, void* cache_k, void* cache_v,
                                long long cache_sb, long long cache_st, const int64_t* mask, long long ldm, void* out,
                                long long ldo, int B, int Hq, int Hkv, int D, int cur, const int* cur_dev, int T, float scale,
-                               void* stream);
+                               int window, void* stream);
 int dalm_b200_greedy_step(const void* logits, long long ld, int B, int V, const int64_t* eos_ids, int n_eos,
                           long long pad_id, int* unfinished, int64_t* tokens, long long ldt, int64_t* mask, long long ldm,
                           int col, int* cur_dev, int T, int64_t* next_ids, int64_t* pos, int* alive, void* stream);

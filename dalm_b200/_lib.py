@@ -54,6 +54,8 @@ SIGNATURES = {
     "dalm_b200_rope": [_P, _L, _I, _I, _I, _P, _P, _I, _I, _I, _P],
     "dalm_b200_swiglu_fwd": [_P, _L, _P, _L, _I, _I, _I, _P],
     "dalm_b200_swiglu_bwd": [_P, _L, _P, _L, _I, _I, _I, _P],
+    "dalm_b200_geglu_fwd": [_P, _L, _P, _L, _I, _I, _P],
+    "dalm_b200_geglu_bwd": [_P, _L, _P, _L, _I, _I, _P],
     "dalm_b200_gemm_bf16_swiglu": [_P, _L, _P, _L, _P, _L, _P, _L, _I, _I, _I, _P],
     "dalm_b200_gemm_bf16_rope": [_P, _L, _P, _L, _P, _L, _I, _I, _I, _P, _P, _P, _I, _I, _P, _P, _I, _F, _P, _L, _P, _L, _P],
     "dalm_b200_gemm_bf16_gelu": [_P, _L, _P, _L, _P, _L, _P, _L, _I, _I, _I, _P, _P],

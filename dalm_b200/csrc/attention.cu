@@ -37,8 +37,9 @@ struct AttnParams {
   DropCfg drop;                     // attention-probability dropout (BERT attention_probs_dropout_prob); p = 0 => off.
                                     // element index of P[b,h,i,j] = ((b*Hq + h)*L + i)*Lp + j, Lp = L rounded up to 8
                                     // (rows start on a Philox group of 8, so one call covers an 8-key MMA n-tile)
-  int window;                       // sliding window (WIN instances only): query i sees key j iff i - window < j <= i;
-                                    // the host clamps it to L, so tile bounds computed from it cannot overflow
+  int window;                       // sliding window (WIN instances only): query i sees key j iff i - window < j <= i
+                                    // (causal) or |i - j| < window (bidirectional); the host clamps it to L, so tile
+                                    // bounds computed from it cannot overflow
 };
 
 // ---------------------------------------------------------------- fragment helpers
@@ -95,12 +96,13 @@ __device__ __forceinline__ void load_b_frag_kn(uint32_t* b, const __nv_bfloat16*
 }
 
 // first key of the KV loop of the query tile at q0: 0 without a window, else the tile holding key q0 - window + 1 (the
-// first key any of its queries sees). A skipped tile would be fully masked for every query of the tile (corr = 1, p = 0
+// first key any of its queries sees, causal or not). Mirrored, it is also the first query tile a bidirectional window lets
+// see the key tile at kv0. The loops end at the last key (query) the tile's last query (key) sees: q0 + BQ - 1 + window - 1
+// without causal. Every range holds the tile's own diagonal, so it is never empty. A skipped tile would be fully masked for every query of the tile (corr = 1, p = 0
 // in the online softmax), so starting later changes no bit of the result.
 template <bool WIN, int BKV> __device__ __forceinline__ int win_begin(int q0, int window) {
   return WIN ? (max(0, q0 - window + 1) / BKV) * BKV : 0;
 }
-
 // ============================================================================================================
 // forward
 // ============================================================================================================
@@ -128,7 +130,7 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(AttnParams p) {
   const float sl2 = p.scale * 1.4426950408889634f;               // scores are exponentiated in base 2
   const int row_a = q0 + warp * 16 + g, row_b = row_a + 8;       // the two query rows this thread holds
 
-  const int kv_end = p.causal ? min(L, q0 + BQ) : L;
+  const int kv_end = p.causal ? min(L, q0 + BQ) : WIN ? min(L, q0 + BQ - 1 + p.window) : L;
   for (int kv0 = win_begin<WIN, BKV>(q0, p.window); kv0 < kv_end; kv0 += BKV) {
     __syncthreads();                                            // previous tile fully consumed
     const int nvalid = min(BKV, L - kv0);
@@ -169,6 +171,7 @@ __global__ void __launch_bounds__(128) attn_fwd_kernel(AttnParams p) {
         float val = s[nt][e] * sl2 + sMask[kc];
         if (p.causal && (kv0 + kc) > qr) val = -INFINITY;
         if (WIN && (kv0 + kc) <= qr - p.window) val = -INFINITY;
+        if (WIN && (kv0 + kc) >= qr + p.window) val = -INFINITY;
         s[nt][e] = val;
         mx[e >> 1] = fmaxf(mx[e >> 1], val);
       }
@@ -328,7 +331,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dkv_kernel(AttnParams p) {
     dv_acc[i][0] = dv_acc[i][1] = dv_acc[i][2] = dv_acc[i][3] = 0.f;
   }
   const int key_a = kv0 + warp * 16 + g, key_b = key_a + 8;     // the two keys (rows of S^T) this thread holds
-  const int q_begin = p.causal ? (kv0 / BQ) * BQ : 0;            // queries before the key tile see none of it
+  const int q_begin = p.causal ? (kv0 / BQ) * BQ : win_begin<WIN, BQ>(kv0, p.window);  // queries before it see none of it
   const int q_end = WIN ? min(L, kv0 + BKV - 1 + p.window) : L;  // nor do queries past its last key's window
 
   for (int hq = hk * group; hq < (hk + 1) * group; ++hq) {
@@ -372,6 +375,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dkv_kernel(AttnParams p) {
           float val = st[nt][e] * sl2 + ((e < 2) ? mk_a : mk_b);
           if (p.causal && key > (q0 + qc)) val = -INFINITY;
           if (WIN && key <= (q0 + qc) - p.window) val = -INFINITY;
+          if (WIN && key >= (q0 + qc) + p.window) val = -INFINITY;
           st[nt][e] = exp2f(val - sLse[qc]);                     // -inf - x -> 0 ; x - (+inf) -> 0
         }
       }
@@ -524,7 +528,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(AttnParams p) {
 #pragma unroll
   for (int i = 0; i < D / 8; ++i) { dq_acc[i][0] = dq_acc[i][1] = dq_acc[i][2] = dq_acc[i][3] = 0.f; }
 
-  const int kv_end = p.causal ? min(L, q0 + BQ) : L;
+  const int kv_end = p.causal ? min(L, q0 + BQ) : WIN ? min(L, q0 + BQ - 1 + p.window) : L;
   for (int kv0 = win_begin<WIN, BKV>(q0, p.window); kv0 < kv_end; kv0 += BKV) {
     __syncthreads();
     const int nvalid = min(BKV, L - kv0);
@@ -589,6 +593,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_kernel(AttnParams p) {
         float val = s[nt][e] * sl2 + sMask[kc];
         if (p.causal && (kv0 + kc) > qr) val = -INFINITY;
         if (WIN && (kv0 + kc) <= qr - p.window) val = -INFINITY;
+        if (WIN && (kv0 + kc) >= qr + p.window) val = -INFINITY;
         const float pv = exp2f(val - lse2[e >> 1]);
         float dpv = dp[nt][e];
         if (DROP) dpv *= msq[nt][e];
@@ -705,7 +710,7 @@ __global__ void __launch_bounds__(128) attn_fwd_wg_kernel(const __grid_constant_
   const int L = p.L, q0 = qb * BQ;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   const size_t tok0 = (size_t)b * L;
-  const int kv_end = p.causal ? min(L, q0 + BQ) : L;
+  const int kv_end = p.causal ? min(L, q0 + BQ) : WIN ? min(L, q0 + BQ - 1 + p.window) : L;
   const int kv_begin = win_begin<WIN, BKV>(q0, p.window);       // tile `it` starts at kv_begin + it * BKV
   const int ntile = (kv_end - kv_begin + BKV - 1) / BKV;
 
@@ -767,6 +772,7 @@ __global__ void __launch_bounds__(128) attn_fwd_wg_kernel(const __grid_constant_
         float val = s[nt][e] * sl2 + sMask[kc];
         if (p.causal && (kv0 + kc) > qr) val = -INFINITY;
         if (WIN && (kv0 + kc) <= qr - p.window) val = -INFINITY;
+        if (WIN && (kv0 + kc) >= qr + p.window) val = -INFINITY;
         s[nt][e] = val;
         mx[e >> 1] = fmaxf(mx[e >> 1], val);
       }
@@ -880,7 +886,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dkv_wg_kernel(const __grid_const
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   const size_t tok0 = (size_t)b * L;
   const float sl2 = p.scale * 1.4426950408889634f;
-  const int q_begin = p.causal ? (kv0 / BQ) * BQ : 0;
+  const int q_begin = p.causal ? (kv0 / BQ) * BQ : win_begin<WIN, BQ>(kv0, p.window);
   const int q_end = WIN ? min(L, kv0 + BKV - 1 + p.window) : L;
   const int nqt = (q_end - q_begin + BQ - 1) / BQ;
   const int nit = group * nqt;                                   // (q head, query tile) pairs, head-major
@@ -959,6 +965,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dkv_wg_kernel(const __grid_const
         float val = st[nt][e] * sl2 + ((e < 2) ? mk_a : mk_b);
         if (p.causal && key > (q0 + qc)) val = -INFINITY;
         if (WIN && key <= (q0 + qc) - p.window) val = -INFINITY;
+        if (WIN && key >= (q0 + qc) + p.window) val = -INFINITY;
         st[nt][e] = exp2f(val - sLse[qc]);
       }
     }
@@ -1049,7 +1056,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_wg_kernel(const __grid_consta
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
   const size_t tok0 = (size_t)b * L;
   const float sl2 = p.scale * 1.4426950408889634f;
-  const int kv_end = p.causal ? min(L, q0 + BQ) : L;
+  const int kv_end = p.causal ? min(L, q0 + BQ) : WIN ? min(L, q0 + BQ - 1 + p.window) : L;
   const int kv_begin = win_begin<WIN, BKV>(q0, p.window);       // tile `it` starts at kv_begin + it * BKV
   const int ntile = (kv_end - kv_begin + BKV - 1) / BKV;
 
@@ -1139,6 +1146,7 @@ __global__ void __launch_bounds__(128) attn_bwd_dq_wg_kernel(const __grid_consta
         float val = s[nt][e] * sl2 + sMask[kc];
         if (p.causal && (kv0 + kc) > qr) val = -INFINITY;
         if (WIN && (kv0 + kc) <= qr - p.window) val = -INFINITY;
+        if (WIN && (kv0 + kc) >= qr + p.window) val = -INFINITY;
         const float pv = exp2f(val - lse2[e >> 1]);
         float dpv = dp[nt][e];
         if (DROP) dpv *= msq[nt][e];
@@ -1218,7 +1226,7 @@ static int check_common(const AttnParams& p, int D) {
   DALM_REQUIRE(p.B > 0 && p.L > 0 && p.Hq > 0 && p.Hkv > 0 && p.Hq % p.Hkv == 0, "attention: bad shape B=%d L=%d Hq=%d Hkv=%d", p.B, p.L, p.Hq, p.Hkv);
   DALM_REQUIRE(p.ldq % 8 == 0 && p.ldk % 8 == 0 && p.ldv % 8 == 0 && p.ldo % 2 == 0, "attention: strides must keep 16-byte row alignment");
   DALM_REQUIRE(((uintptr_t)p.q & 15) == 0 && ((uintptr_t)p.k & 15) == 0 && ((uintptr_t)p.v & 15) == 0, "attention: q/k/v must be 16-byte aligned");
-  DALM_REQUIRE(p.window >= 0 && (p.window == 0 || p.causal), "attention: window %d must be >= 0, and > 0 only with causal", p.window);
+  DALM_REQUIRE(p.window >= 0, "attention: window %d must be >= 0", p.window);
   DALM_REQUIRE(p.window == 0 || p.drop.p == 0.f, "attention: probability dropout with a sliding window is not built");
   return 0;
 }

@@ -1,5 +1,5 @@
 // dalm_b200 — HBM-bound row-wise kernels of the encoder/decoder blocks (everything that is not a tensor-core tile):
-// LayerNorm / RMSNorm forward+backward, embedding gathers, RoPE, SwiGLU, GELU, masked mean-pool + L2 normalise,
+// LayerNorm / RMSNorm forward+backward, embedding gathers, RoPE, SwiGLU, GeGLU, GELU, masked mean-pool + L2 normalise,
 // LoRA weight-gradients, fused Adam. All use 16-byte vector accesses, warp-shuffle reductions and one CTA per row
 // (rows = tokens; 3204..26700 per launch => several waves over 132 SMs).
 //
@@ -371,7 +371,8 @@ __global__ void rope_kernel(__nv_bfloat16* __restrict__ buf, long long ld, int c
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// SwiGLU: gu = [gate | up] (bf16 [M,2F]);  act = silu(gate) * up
+// Gated MLP activations on a [first | second] buffer (bf16 [M,2F]): act = A(first) * second.
+//   SwiGLU (Llama): gu = [gate | up], A = silu.   GeGLU (ModernBERT): [input | gate] = Wi(x).chunk(2), A = gelu_erf.
 // ------------------------------------------------------------------------------------------------------------
 // gate / up column of feature i inside a [M, 2F] gate|up buffer: il == 0: [gate 0..F | up 0..F] (HF order); il > 0: blocks of il
 // features interleaved [gate blk | up blk | gate blk+1 | ...] - the layout that puts a feature's gate AND up accumulator in the
@@ -381,8 +382,26 @@ __device__ __forceinline__ int gate_col(int i, int F, int il, int& up_off) {
   up_off = il;
   return (i / il) * 2 * il + (i % il);
 }
-__global__ void swiglu_fwd_kernel(const __nv_bfloat16* __restrict__ gu, long long ldgu, __nv_bfloat16* __restrict__ act,
-                                  long long lda, int F, int il) {
+// A(x), and the backward of act = A(g) * u given d = d act: dg = d * u * A'(g), du = d * A(g)
+struct SiluAct {
+  static __device__ __forceinline__ float fwd(float x) { return x / (1.f + __expf(-x)); }
+  static __device__ __forceinline__ void bwd(float g, float u, float d, float& dg, float& du) {
+    const float sg = 1.f / (1.f + __expf(-g));
+    const float silu = g * sg;
+    dg = d * u * sg * (1.f + g * (1.f - sg));
+    du = d * silu;
+  }
+};
+struct GeluAct {
+  static __device__ __forceinline__ float fwd(float x) { return gelu_erf(x); }
+  static __device__ __forceinline__ void bwd(float g, float u, float d, float& dg, float& du) {
+    dg = d * u * gelu_erf_grad(g);
+    du = d * gelu_erf(g);
+  }
+};
+template <class Act>
+__global__ void glu_fwd_kernel(const __nv_bfloat16* __restrict__ gu, long long ldgu, __nv_bfloat16* __restrict__ act,
+                               long long lda, int F, int il) {
   const size_t r = blockIdx.y;
   const int i = (blockIdx.x * blockDim.x + threadIdx.x) * 8;
   if (i >= F) return;
@@ -392,12 +411,13 @@ __global__ void swiglu_fwd_kernel(const __nv_bfloat16* __restrict__ gu, long lon
   unpack8(*reinterpret_cast<const bf16x8*>(gu + r * ldgu + gc), g);
   unpack8(*reinterpret_cast<const bf16x8*>(gu + r * ldgu + gc + uo), u);
 #pragma unroll
-  for (int k = 0; k < 8; ++k) o[k] = g[k] / (1.f + __expf(-g[k])) * u[k];
+  for (int k = 0; k < 8; ++k) o[k] = Act::fwd(g[k]) * u[k];
   *reinterpret_cast<bf16x8*>(act + r * lda + i) = pack8(o);
 }
-// in place: gu <- [dgate | dup]
-__global__ void swiglu_bwd_kernel(__nv_bfloat16* __restrict__ gu, long long ldgu, const __nv_bfloat16* __restrict__ dact,
-                                  long long ldd, int F, int il) {
+// in place: gu <- [d first | d second]
+template <class Act>
+__global__ void glu_bwd_kernel(__nv_bfloat16* __restrict__ gu, long long ldgu, const __nv_bfloat16* __restrict__ dact,
+                               long long ldd, int F, int il) {
   const size_t r = blockIdx.y;
   const int i = (blockIdx.x * blockDim.x + threadIdx.x) * 8;
   if (i >= F) return;
@@ -408,12 +428,7 @@ __global__ void swiglu_bwd_kernel(__nv_bfloat16* __restrict__ gu, long long ldgu
   unpack8(*reinterpret_cast<const bf16x8*>(gu + r * ldgu + gc + uo), u);
   unpack8(*reinterpret_cast<const bf16x8*>(dact + r * ldd + i), d);
 #pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    const float sg = 1.f / (1.f + __expf(-g[k]));
-    const float silu = g[k] * sg;
-    dg[k] = d[k] * u[k] * sg * (1.f + g[k] * (1.f - sg));
-    du[k] = d[k] * silu;
-  }
+  for (int k = 0; k < 8; ++k) Act::bwd(g[k], u[k], d[k], dg[k], du[k]);
   *reinterpret_cast<bf16x8*>(gu + r * ldgu + gc) = pack8(dg);
   *reinterpret_cast<bf16x8*>(gu + r * ldgu + gc + uo) = pack8(du);
 }
@@ -974,7 +989,7 @@ extern "C" int dalm_b200_swiglu_fwd(const void* gu, long long ldgu, void* act, l
   DALM_REQUIRE((F % 8) == 0 && (ldgu % 8) == 0 && (lda % 8) == 0, "swiglu: F and strides must be multiples of 8");
   DALM_REQUIRE(interleave == 0 || ((interleave % 8) == 0 && (F % interleave) == 0), "swiglu: interleave block must divide F and be a multiple of 8");
   dim3 grid((F / 8 + 255) / 256, M);
-  swiglu_fwd_kernel<<<grid, 256, 0, ST(stream)>>>((const __nv_bfloat16*)gu, ldgu, (__nv_bfloat16*)act, lda, F, interleave);
+  glu_fwd_kernel<SiluAct><<<grid, 256, 0, ST(stream)>>>((const __nv_bfloat16*)gu, ldgu, (__nv_bfloat16*)act, lda, F, interleave);
   count_launch();
   return check_launch("swiglu_fwd_kernel");
 }
@@ -982,9 +997,33 @@ extern "C" int dalm_b200_swiglu_bwd(void* gu, long long ldgu, const void* dact, 
   DALM_REQUIRE((F % 8) == 0 && (ldgu % 8) == 0 && (ldd % 8) == 0, "swiglu: F and strides must be multiples of 8");
   DALM_REQUIRE(interleave == 0 || ((interleave % 8) == 0 && (F % interleave) == 0), "swiglu: interleave block must divide F and be a multiple of 8");
   dim3 grid((F / 8 + 255) / 256, M);
-  swiglu_bwd_kernel<<<grid, 256, 0, ST(stream)>>>((__nv_bfloat16*)gu, ldgu, (const __nv_bfloat16*)dact, ldd, F, interleave);
+  glu_bwd_kernel<SiluAct><<<grid, 256, 0, ST(stream)>>>((__nv_bfloat16*)gu, ldgu, (const __nv_bfloat16*)dact, ldd, F, interleave);
   count_launch();
   return check_launch("swiglu_bwd_kernel");
+}
+// rows go to grid.y, which holds at most 65535: longer batches (bs 8 x 8192 tokens) are launched in chunks of rows
+constexpr int GLU_ROWS = 65535;
+extern "C" int dalm_b200_geglu_fwd(const void* x, long long ldx, void* act, long long lda, int M, int F, void* stream) {
+  DALM_REQUIRE((F % 8) == 0 && (ldx % 8) == 0 && (lda % 8) == 0, "geglu: F and strides must be multiples of 8");
+  for (int r0 = 0; r0 < M; r0 += GLU_ROWS) {
+    dim3 grid((F / 8 + 255) / 256, min(GLU_ROWS, M - r0));
+    glu_fwd_kernel<GeluAct><<<grid, 256, 0, ST(stream)>>>((const __nv_bfloat16*)x + (size_t)r0 * ldx, ldx,
+                                                         (__nv_bfloat16*)act + (size_t)r0 * lda, lda, F, 0);
+    count_launch();
+    if (int e = check_launch("geglu_fwd_kernel")) return e;
+  }
+  return 0;
+}
+extern "C" int dalm_b200_geglu_bwd(void* x, long long ldx, const void* dact, long long ldd, int M, int F, void* stream) {
+  DALM_REQUIRE((F % 8) == 0 && (ldx % 8) == 0 && (ldd % 8) == 0, "geglu: F and strides must be multiples of 8");
+  for (int r0 = 0; r0 < M; r0 += GLU_ROWS) {
+    dim3 grid((F / 8 + 255) / 256, min(GLU_ROWS, M - r0));
+    glu_bwd_kernel<GeluAct><<<grid, 256, 0, ST(stream)>>>((__nv_bfloat16*)x + (size_t)r0 * ldx, ldx,
+                                                         (const __nv_bfloat16*)dact + (size_t)r0 * ldd, ldd, F, 0);
+    count_launch();
+    if (int e = check_launch("geglu_bwd_kernel")) return e;
+  }
+  return 0;
 }
 extern "C" int dalm_b200_gelu_fwd(const void* pre, long long ldp, void* act, long long lda, int M, int F, void* stream) {
   DALM_REQUIRE((F % 8) == 0 && (ldp % 8) == 0 && (lda % 8) == 0, "gelu: F and strides must be multiples of 8");

@@ -21,11 +21,11 @@ def _normal(gen: torch.Generator, shape, std: float, dtype, device) -> torch.Ten
 
 def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, device="cpu",
                       bias_std: Optional[float] = None, qk_norm_std: Optional[float] = None) -> Dict[str, torch.Tensor]:
-    """HF parameter names for BertModel / XLMRobertaModel / RobertaModel (no prefix) / LlamaForCausalLM / Qwen2ForCausalLM /
+    """HF parameter names for BertModel / XLMRobertaModel / RobertaModel / ModernBertModel (no prefix) / LlamaForCausalLM / Qwen2ForCausalLM /
     Qwen3ForCausalLM / MistralForCausalLM / FalconForCausalLM, init N(0, initializer_range), LN = (1, 0). Decoder attention biases (Qwen2's q/k/v, Llama's and Qwen3's
     `attention_bias`) are drawn from N(0, bias_std) (default: initializer_range) rather than HF's zeros, so that a dropped bias
     changes the outputs. Qwen3's q_norm / k_norm weights are 1 + N(0, qk_norm_std) (default: initializer_range), so that a
-    dropped or swapped norm shows."""
+    dropped or swapped norm shows; so are every LayerNorm weight of ModernBERT."""
     on_device = torch.device(device).type == "cuda" and cfg.get("_device_rng", False)
     gen = torch.Generator(device=device) if on_device else torch.Generator()
     gen.manual_seed(seed)
@@ -89,6 +89,20 @@ def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, 
         sd["model.norm.weight"] = ones(H) + _normal(gen, (H,), std, dtype, device)
         if not cfg.get("tie_word_embeddings", False):             # tied checkpoints store no lm_head (Qwen2 0.5B-3B)
             sd["lm_head.weight"] = _normal(gen, (V, H), std, dtype, device)
+    elif kind == "modernbert":                                   # ModernBertModel names (no prefix); no biases anywhere
+        F, V = cfg["intermediate_size"], cfg["vocab_size"]
+        sd["embeddings.tok_embeddings.weight"] = _normal(gen, (V, H), std, dtype, device)
+        sd["embeddings.norm.weight"] = ones(H) + _normal(gen, (H,), std, dtype, device)
+        for l in range(cfg["num_hidden_layers"]):
+            p = f"layers.{l}."
+            if l > 0:                                              # layer 0's attn_norm is nn.Identity
+                sd[p + "attn_norm.weight"] = ones(H) + _normal(gen, (H,), std, dtype, device)
+            sd[p + "attn.Wqkv.weight"] = _normal(gen, (3 * H, H), std, dtype, device)
+            sd[p + "attn.Wo.weight"] = _normal(gen, (H, H), std, dtype, device)
+            sd[p + "mlp_norm.weight"] = ones(H) + _normal(gen, (H,), std, dtype, device)
+            sd[p + "mlp.Wi.weight"] = _normal(gen, (2 * F, H), std, dtype, device)
+            sd[p + "mlp.Wo.weight"] = _normal(gen, (H, F), std, dtype, device)
+        sd["final_norm.weight"] = ones(H) + _normal(gen, (H,), std, dtype, device)
     elif kind == "falcon":
         V = cfg["vocab_size"]
         nh = cfg["num_attention_heads"]
@@ -158,11 +172,15 @@ def model_kind(cfg: Dict) -> str:
     if mt in ("llama", "qwen2", "qwen3", "mistral"):
         check_llama_family(cfg)
         return mt
+    if mt == "modernbert":
+        check_modernbert(cfg)
+        return "modernbert"
     if mt == "falcon":
         check_rope_type(cfg)
         return "falcon"
     raise NotImplementedError(
-        f"model_type {mt!r} is not built in dalm_b200 (supported: bert, roberta and xlm-roberta encoders; llama, qwen2, qwen3, mistral and falcon decoders)")
+        f"model_type {mt!r} is not built in dalm_b200 (supported: bert, roberta, xlm-roberta and modernbert encoders; llama, "
+        "qwen2, qwen3, mistral and falcon decoders)")
 
 
 def _rope_type(cfg: Dict) -> str:
@@ -303,6 +321,71 @@ def check_roberta(cfg: Dict) -> None:
         raise NotImplementedError(f"{mt}: is_decoder=true (causal self-attention) is not built")
     if cfg.get("add_cross_attention", False):
         raise NotImplementedError(f"{mt}: add_cross_attention=true is not built")
+
+
+MODERNBERT_THETA = {"full_attention": ("global_rope_theta", 160000.0), "sliding_attention": ("local_rope_theta", 10000.0)}
+
+
+def modernbert_rope_parameters(cfg: Dict) -> Dict[str, Dict]:
+    """{"full_attention": {...}, "sliding_attention": {...}} as ModernBertConfig resolves them: `rope_parameters` when given,
+    `rope_scaling` merged into both, and a missing rope_theta taken from the hub spelling `global_rope_theta` /
+    `local_rope_theta` (defaults 160000 / 10000)"""
+    rp = cfg.get("rope_parameters")
+    rp = {k: dict(v) if isinstance(v, dict) else v for k, v in rp.items()} if isinstance(rp, dict) else {}
+    rs = cfg.get("rope_scaling")
+    out = {}
+    for lt, (key, theta) in MODERNBERT_THETA.items():
+        d = rp.get(lt) or {"rope_type": "default"}
+        if rs is not None:
+            d.update(rs)
+        d.setdefault("rope_theta", cfg.get(key, theta))
+        d["rope_type"] = d.get("rope_type", d.get("type")) or "default"
+        out[lt] = d
+    return out
+
+
+def modernbert_layer_types(cfg: Dict) -> List[str]:
+    """`layer_types`, or else layer i is full attention iff i % global_attn_every_n_layers == 0 (default 3)"""
+    n = int(cfg["num_hidden_layers"])
+    types = cfg.get("layer_types")
+    if types is None:
+        every = int(cfg.get("global_attn_every_n_layers", 3))
+        types = ["sliding_attention" if i % every else "full_attention" for i in range(n)]
+    if len(types) != n:
+        raise ValueError(f"modernbert: layer_types lists {len(types)} layers, num_hidden_layers is {n}")
+    return list(types)
+
+
+def modernbert_layers(cfg: Dict) -> List[tuple]:
+    """(window, inv_freq) of every layer. window: 0 for a global layer; for a local one local_attention // 2 + 1, so that query
+    i sees key j iff |i - j| < window, i.e. |i - j| <= local_attention // 2 (transformers' sliding-window mask). inv_freq: fp32
+    [head_dim / 2], bit for bit ModernBertRotaryEmbedding's buffer of the layer's type."""
+    hd = cfg["hidden_size"] // cfg["num_attention_heads"]
+    rope = modernbert_rope_parameters(cfg)
+    freqs = {lt: rope_inv_freq({"model_type": "modernbert", "rope_parameters": dict(rp)}, hd) for lt, rp in rope.items()}
+    win = int(cfg.get("local_attention", 128)) // 2 + 1
+    return [(win if t == "sliding_attention" else 0, freqs[t]) for t in modernbert_layer_types(cfg)]
+
+
+def check_modernbert(cfg: Dict) -> None:
+    """refuses the settings of a modernbert config that ModernBertEncoder would otherwise silently compute wrong. Every
+    published ModernBERT retriever has zero dropout, no biases and the erf GELU."""
+    for k in ("attention_dropout", "mlp_dropout", "embedding_dropout"):
+        if float(cfg.get(k) or 0.0) != 0.0:
+            raise NotImplementedError(f"modernbert: {k}={cfg[k]} is not built (dropout is not built for ModernBERT)")
+    act = cfg.get("hidden_activation", "gelu")
+    if act != "gelu":
+        raise NotImplementedError(f"modernbert: hidden_activation={act!r} is not built; only 'gelu' (erf)")
+    for k in ("norm_bias", "mlp_bias", "attention_bias"):
+        if cfg.get(k, False):
+            raise NotImplementedError(f"modernbert: {k}=true is not built (biases are not built for ModernBERT)")
+    for lt, rp in modernbert_rope_parameters(cfg).items():
+        if rp["rope_type"] != "default":
+            raise NotImplementedError(f"modernbert: RoPE type {rp['rope_type']!r} ({lt}) is not built; only 'default'")
+    hd = cfg["hidden_size"] // cfg["num_attention_heads"]
+    if hd not in (32, 64, 128):
+        raise NotImplementedError(f"modernbert: head_dim {hd} is not built (the attention kernels take 32 / 64 / 128)")
+    modernbert_layer_types(cfg)
 
 
 def roberta_max_len(cfg: Dict) -> int:

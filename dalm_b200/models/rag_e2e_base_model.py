@@ -18,6 +18,8 @@ from ..engine.bridge import EncodeFn, GenerateFn, PoolFn
 from ..engine.decoding import load_generation_config
 from ..engine.falcon import FalconDecoder
 from ..engine.llama import LlamaDecoder
+from ..engine.modernbert import LORA_REFUSAL as MODERNBERT_LORA_REFUSAL
+from ..engine.modernbert import ModernBertEncoder
 
 logger = logging.getLogger(__name__)
 
@@ -65,11 +67,16 @@ def load_tokenizer(name_or_path: str):
 
 def build_encoder(name_or_path: str, lora: bool, device: torch.device, state_dict: Optional[Dict] = None,
                   cfg: Optional[Dict] = None, autoregressive: bool = False, full: bool = False, bnb: bool = False):
-    """BERT-family encoder (bge-*) or (XLM-)RoBERTa encoder (multilingual-e5, bge-m3, xlm-roberta-*), or — `retriever_is_autoregressive` — a Llama / Qwen2 / Qwen3 /
+    """BERT-family encoder (bge-*), (XLM-)RoBERTa encoder (multilingual-e5, bge-m3, xlm-roberta-*), ModernBERT encoder
+    (gte-modernbert, modernbert-embed; frozen or fully fine-tuned), or — `retriever_is_autoregressive` — a Llama / Qwen2 / Qwen3 /
     Mistral decoder (e5-mistral-7b-instruct, SFR-Embedding-Mistral) used as an encoder
     (last hidden state, eos pooling; LoRA targets q_proj / v_proj: reference rag_e2e_base_model.py:66-70,84-90)"""
     cfg = cfg or params.load_config(name_or_path)
     kind = params.model_kind(cfg)
+    if kind == "modernbert":
+        _check_modernbert_mode(lora, autoregressive, bnb)
+        sd = state_dict if state_dict is not None else params.load_state_dict(name_or_path)
+        return _named(ModernBertEncoder(cfg, sd, device=device, full=full), name_or_path)
     sd = state_dict if state_dict is not None else params.load_state_dict(name_or_path)
     nf4 = _nf4_storage(bnb, full, kind)
     if not nf4:
@@ -81,8 +88,24 @@ def build_encoder(name_or_path: str, lora: bool, device: torch.device, state_dic
         return _named(LlamaDecoder(cfg, sd, device=device, lora=lora, lora_seed=0, full=full, nf4_storage=nf4), name_or_path)
     if kind not in ("bert", "roberta"):
         raise NotImplementedError("non-autoregressive retrievers must be BERT (bge-*) or (XLM-)RoBERTa (multilingual-e5, bge-m3) "
-                                  "encoders; pass retriever_is_autoregressive=True for a causal LM")
+                                  "encoders, or ModernBERT ones; pass retriever_is_autoregressive=True for a causal LM")
     return _named(BertEncoder(cfg, sd, device=device, lora=lora, full=full, nf4_storage=nf4), name_or_path)
+
+
+def _check_modernbert_mode(lora: bool, autoregressive: bool, bnb: bool) -> None:
+    """ModernBERT retrievers run frozen or fully fine-tuned; every other mode is refused, naming why"""
+    from ..engine.nf4store import storage_enabled
+    if autoregressive:
+        raise NotImplementedError("retriever_is_autoregressive=True: ModernBERT is a bidirectional encoder (mean-pooled), "
+                                  "not a causal LM")
+    if lora:
+        raise NotImplementedError(MODERNBERT_LORA_REFUSAL)
+    if bnb and storage_enabled():
+        raise NotImplementedError("DALM_B200_NF4_STORAGE=1: 4-bit storage is not built for ModernBERT retrievers (it serves "
+                                  "LoRA-carrying BERT / (XLM-)RoBERTa encoders and Llama decoders)")
+    if bnb:
+        raise NotImplementedError("use_bnb on a ModernBERT retriever: the reference's 4-bit retriever needs LoRA on the same "
+                                  "sub-model, and LoRA is not built for ModernBERT; drop use_bnb for the retriever")
 
 
 def _named(engine_model, name_or_path: str):

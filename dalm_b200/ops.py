@@ -296,7 +296,19 @@ GEMM_MAX_CTAS = 0
 # ----------------------------------------------------------------------------------------------------------------
 # attention
 # ----------------------------------------------------------------------------------------------------------------
-def _attention_fwd(sym, q, k, v, mask, B, L, Hq, Hkv, D, causal, out, scale, drop, window):
+def _window_arg(causal, window, bidirectional) -> int:
+    """a window without causal means a bidirectional window (|i - j| < window, ModernBERT's local layers); the caller has to ask
+    for that meaning with bidirectional=True, so that dropping `causal` from a causal (Mistral) call is still refused"""
+    if bidirectional and causal:
+        raise _lib.DalmB200Error("attention: bidirectional=True and causal=True are exclusive")
+    if window > 0 and not causal and not bidirectional:
+        raise _lib.DalmB200Error(f"attention: window {window} without causal is a bidirectional window; pass bidirectional=True "
+                                 "to ask for it")
+    return int(window)
+
+
+def _attention_fwd(sym, q, k, v, mask, B, L, Hq, Hkv, D, causal, out, scale, drop, window, bidirectional=False):
+    window = _window_arg(causal, window, bidirectional)
     for t, n in ((q, "q"), (k, "k"), (v, "v")):
         _chk(t, bf16, n)
     if out is None:
@@ -310,7 +322,9 @@ def _attention_fwd(sym, q, k, v, mask, B, L, Hq, Hkv, D, causal, out, scale, dro
     return out, lse
 
 
-def _attention_bwd(sym, q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq, dk, dv, scale, drop, window):
+def _attention_bwd(sym, q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq, dk, dv, scale, drop, window,
+                   bidirectional=False):
+    window = _window_arg(causal, window, bidirectional)
     dev = q.device
     if dq is None: dq = torch.empty(B * L, Hq * D, dtype=bf16, device=dev)
     if dk is None: dk = torch.empty(B * L, Hkv * D, dtype=bf16, device=dev)
@@ -324,47 +338,50 @@ def _attention_bwd(sym, q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal
 
 
 def attention_fwd(q, k, v, mask, B: int, L: int, Hq: int, Hkv: int, D: int, causal: bool, out=None,
-                  scale: Optional[float] = None, drop: Optional[Drop] = None, window: int = 0):
+                  scale: Optional[float] = None, drop: Optional[Drop] = None, window: int = 0, bidirectional: bool = False):
     """mma.sync attention forward (head_dim 32/64/128). q/k/v: bf16 token-major 2-D views [B*L, H*D] (may be column slices
-    of one qkv buffer). window > 0 (causal only): query i sees key j iff i - window < j <= i (Mistral's sliding window,
-    counted in the padded row); 0 = no window. -> (out, lse)"""
-    return _attention_fwd("dalm_b200_attention_fwd", q, k, v, mask, B, L, Hq, Hkv, D, causal, out, scale, drop, window)
+    of one qkv buffer). window > 0 with causal: query i sees key j iff i - window < j <= i (Mistral's sliding window, counted
+    in the padded row); with bidirectional=True (causal False): iff |i - j| < window (ModernBERT's local layers); 0 = no
+    window. -> (out, lse)"""
+    return _attention_fwd("dalm_b200_attention_fwd", q, k, v, mask, B, L, Hq, Hkv, D, causal, out, scale, drop, window,
+                          bidirectional)
 
 
 def attention_bwd(q, k, v, mask, out, lse, d_out, B: int, L: int, Hq: int, Hkv: int, D: int, causal: bool,
-                  dq=None, dk=None, dv=None, scale: Optional[float] = None, drop: Optional[Drop] = None, window: int = 0):
+                  dq=None, dk=None, dv=None, scale: Optional[float] = None, drop: Optional[Drop] = None, window: int = 0,
+                  bidirectional: bool = False):
     """mma.sync attention backward (the window must be the forward's). -> (dq, dk, dv)"""
     return _attention_bwd("dalm_b200_attention_bwd", q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq, dk, dv, scale, drop,
-                          window)
+                          window, bidirectional)
 
 
 def attention_tc_fwd(q, k, v, mask, B: int, L: int, Hq: int, Hkv: int, D: int, causal: bool, out=None,
-                     scale: Optional[float] = None, drop: Optional[Drop] = None, window: int = 0):
+                     scale: Optional[float] = None, drop: Optional[Drop] = None, window: int = 0, bidirectional: bool = False):
     """wgmma/TMA attention forward (head_dim 128 or 64; probability dropout at 64). Same contract as attention_fwd."""
-    return _attention_fwd("dalm_b200_attention_tc_fwd", q, k, v, mask, B, L, Hq, Hkv, D, causal, out, scale, drop, window)
+    return _attention_fwd("dalm_b200_attention_tc_fwd", q, k, v, mask, B, L, Hq, Hkv, D, causal, out, scale, drop, window,
+                          bidirectional)
 
 
 def attention_tc_bwd(q, k, v, mask, out, lse, d_out, B: int, L: int, Hq: int, Hkv: int, D: int, causal: bool,
-                     dq=None, dk=None, dv=None, scale: Optional[float] = None, drop: Optional[Drop] = None, window: int = 0):
+                     dq=None, dk=None, dv=None, scale: Optional[float] = None, drop: Optional[Drop] = None, window: int = 0,
+                     bidirectional: bool = False):
     """wgmma/TMA attention backward (head_dim 128 or 64). Same contract as attention_bwd."""
     return _attention_bwd("dalm_b200_attention_tc_bwd", q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq, dk, dv, scale, drop,
-                          window)
+                          window, bidirectional)
 
 
-def attention_auto_fwd(q, k, v, mask, B, L, Hq, Hkv, D, causal, out=None, scale=None, drop=None, window: int = 0):
+def attention_auto_fwd(q, k, v, mask, B, L, Hq, Hkv, D, causal, out=None, scale=None, drop=None, window: int = 0,
+                       bidirectional: bool = False):
     """head_dim 64 / 128 -> wgmma kernels; head_dim 32 (bge-small) -> mma.sync kernels."""
-    if D in (64, 128):
-        return attention_tc_fwd(q, k, v, mask, B, L, Hq, Hkv, D, causal, out=out, scale=scale, drop=drop, window=window)
-    return attention_fwd(q, k, v, mask, B, L, Hq, Hkv, D, causal, out=out, scale=scale, drop=drop, window=window)
+    f = attention_tc_fwd if D in (64, 128) else attention_fwd
+    return f(q, k, v, mask, B, L, Hq, Hkv, D, causal, out=out, scale=scale, drop=drop, window=window, bidirectional=bidirectional)
 
 
 def attention_auto_bwd(q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq=None, dk=None, dv=None, scale=None, drop=None,
-                       window: int = 0):
-    if D in (64, 128):
-        return attention_tc_bwd(q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq=dq, dk=dk, dv=dv, scale=scale, drop=drop,
-                                window=window)
-    return attention_bwd(q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq=dq, dk=dk, dv=dv, scale=scale, drop=drop,
-                         window=window)
+                       window: int = 0, bidirectional: bool = False):
+    f = attention_tc_bwd if D in (64, 128) else attention_bwd
+    return f(q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq=dq, dk=dk, dv=dv, scale=scale, drop=drop, window=window,
+             bidirectional=bidirectional)
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -467,11 +484,12 @@ def roberta_embed(ids, word, pos, type_emb, pad_id: int, out=None, pos_ids=None)
     return z, pos_ids
 
 
-def embed_gather(ids, table):
+def embed_gather(ids, table, out=None):
     M = ids.numel()
     V, H = table.shape
     _tables16(("embed_gather table", table))
-    x = torch.empty(M, H, dtype=f32, device=ids.device)
+    _rows32(out, "embed_gather out", H, M)
+    x = torch.empty(M, H, dtype=f32, device=ids.device) if out is None else out
     _lib.call("dalm_b200_embed_gather", _p(ids.contiguous()), _p(table), _p(x), M, H, V, _stream())
     return x
 
@@ -493,6 +511,21 @@ def swiglu_fwd(gu, F: int, act=None, interleave: int = 0):
 def swiglu_bwd_(gu, dact, F: int, interleave: int = 0):
     _lib.call("dalm_b200_swiglu_bwd", _p(gu), _ld(gu), _p(dact), _ld(dact), gu.shape[0], F, int(interleave), _stream())
     return gu
+
+
+def geglu_fwd(x, F: int, act=None):
+    """ModernBertMLP: x = [input | gate] (bf16 [M, 2F]) -> gelu_erf(input) * gate (bf16 [M, F])"""
+    M = x.shape[0]
+    if act is None:
+        act = torch.empty(M, F, dtype=bf16, device=x.device)
+    _lib.call("dalm_b200_geglu_fwd", _p(x), _ld(x), _p(act), _ld(act), M, F, _stream())
+    return act
+
+
+def geglu_bwd_(x, dact, F: int):
+    """in place: x <- [d_input | d_gate]"""
+    _lib.call("dalm_b200_geglu_bwd", _p(x), _ld(x), _p(dact), _ld(dact), x.shape[0], F, _stream())
+    return x
 
 
 def gemm_swiglu(a: torch.Tensor, w_il: torch.Tensor, gu: Optional[torch.Tensor] = None, act: Optional[torch.Tensor] = None):

@@ -120,6 +120,20 @@ MISTRAL_SHAPES: Dict[str, Dict] = {
                                    head_dim=128, intermediate_size=14336, sliding_window=None, rope_theta=1000000.0,
                                    vocab_size=131072, max_position_embeddings=1024000),
 }
+# ModernBERT encoders (model_type "modernbert"): pre-norm layers with RoPE, GeGLU and, on two layers of three, bidirectional
+# sliding-window attention. The tiny shapes use local_attention 16 (query i sees keys |i - j| <= 8) so that several windows fit
+# in short test rows, and 4 layers: layer 0 (global, no attn_norm), two local layers and a second global one. The published
+# shapes were written from memory of their config.json files and could not be re-checked offline.
+MODERNBERT_SHAPES: Dict[str, Dict] = {
+    "modernbert-tiny": dict(hidden_size=64, num_hidden_layers=4, num_attention_heads=2, intermediate_size=96,
+                            local_attention=16),                              # head_dim 32: mma.sync attention
+    "modernbert-hd64": dict(hidden_size=128, num_hidden_layers=4, num_attention_heads=2, intermediate_size=160,
+                            local_attention=16),                              # head_dim 64: wgmma attention
+    "ModernBERT-base": dict(hidden_size=768, num_hidden_layers=22, num_attention_heads=12, intermediate_size=1152),
+    "gte-modernbert-base": dict(hidden_size=768, num_hidden_layers=22, num_attention_heads=12, intermediate_size=1152),
+    "modernbert-embed-base": dict(hidden_size=768, num_hidden_layers=22, num_attention_heads=12, intermediate_size=1152),
+    "ModernBERT-large": dict(hidden_size=1024, num_hidden_layers=28, num_attention_heads=16, intermediate_size=2624),
+}
 FALCON_SHAPES: Dict[str, Dict] = {
     "falcon-tiny": dict(hidden_size=128, num_hidden_layers=2, num_attention_heads=2),
     "falcon-mini": dict(hidden_size=448, num_hidden_layers=2, num_attention_heads=7),          # 7 q heads x 64, one KV head
@@ -163,6 +177,25 @@ def roberta_config(name: str, vocab_size: Optional[int] = None) -> Dict:
         position_embedding_type="absolute", use_cache=True, classifier_dropout=None,
     )
     cfg.update(s)
+    return cfg
+
+
+MODERNBERT_SPECIAL = {"[UNK]": 50280, "[CLS]": 50281, "[SEP]": 50282, "[PAD]": 50283, "[MASK]": 50284}
+
+
+def modernbert_config(name: str, vocab_size: int = 50368) -> Dict:
+    """ModernBERT (HF ModernBertModel): vocab 50368 with [CLS] 50281 / [SEP] 50282 / [PAD] 50283, local_attention 128 (the
+    tiny shapes: 16), a global layer every 3, RoPE theta 160000 (global) / 10000 (local) in the hub spelling, norm_eps 1e-5, no
+    biases, zero dropout and 8192 positions"""
+    cfg = dict(
+        architectures=["ModernBertModel"], model_type="modernbert", vocab_size=vocab_size, max_position_embeddings=8192,
+        hidden_activation="gelu", norm_eps=1e-5, norm_bias=False, attention_bias=False, mlp_bias=False, attention_dropout=0.0,
+        mlp_dropout=0.0, embedding_dropout=0.0, local_attention=128, global_attn_every_n_layers=3, global_rope_theta=160000.0,
+        local_rope_theta=10000.0, initializer_range=0.02, pad_token_id=MODERNBERT_SPECIAL["[PAD]"],
+        bos_token_id=MODERNBERT_SPECIAL["[CLS]"], cls_token_id=MODERNBERT_SPECIAL["[CLS]"],
+        eos_token_id=MODERNBERT_SPECIAL["[SEP]"], sep_token_id=MODERNBERT_SPECIAL["[SEP]"],
+    )
+    cfg.update(MODERNBERT_SHAPES[name])
     return cfg
 
 
@@ -361,6 +394,33 @@ def build_roberta_tokenizer(out_dir: str, vocab_size: int = 50265, model_max_len
     return out_dir
 
 
+def build_modernbert_tokenizer(out_dir: str, vocab_size: int = 50368) -> str:
+    """ModernBERT-style byte-level BPE trained on the synthetic corpus, saved as a `PreTrainedTokenizerFast` like the published
+    one: [UNK] / [CLS] / [SEP] / [PAD] / [MASK] at 50280-50284, `[CLS] $A [SEP]` framing, right padding, and only input_ids /
+    attention_mask as model inputs (no token_type_ids)"""
+    from tokenizers import AddedToken, Tokenizer, decoders, models, pre_tokenizers, processors, trainers
+    from transformers import PreTrainedTokenizerFast
+
+    tok = Tokenizer(models.BPE())
+    tok.pre_tokenizer = pre_tokenizers.ByteLevel(add_prefix_space=False)
+    tok.decoder = decoders.ByteLevel()
+    trainer = trainers.BpeTrainer(vocab_size=6000, show_progress=False, initial_alphabet=pre_tokenizers.ByteLevel.alphabet())
+    tok.train_from_iterator(_corpus(), trainer)
+    first = min(MODERNBERT_SPECIAL.values())
+    tok.add_tokens([f"<|extra_{i}|>" for i in range(tok.get_vocab_size(), first)])       # ids span the real embedding table
+    tok.add_special_tokens([AddedToken(t, special=True) for t in sorted(MODERNBERT_SPECIAL, key=MODERNBERT_SPECIAL.get)])
+    tok.add_tokens([f"[unused{i}]" for i in range(tok.get_vocab_size(), vocab_size)])
+    cls, sep = MODERNBERT_SPECIAL["[CLS]"], MODERNBERT_SPECIAL["[SEP]"]
+    tok.post_processor = processors.TemplateProcessing(single="[CLS] $A [SEP]", pair="[CLS] $A [SEP] $B:1 [SEP]:1",
+                                                       special_tokens=[("[CLS]", cls), ("[SEP]", sep)])
+    ft = PreTrainedTokenizerFast(tokenizer_object=tok, unk_token="[UNK]", cls_token="[CLS]", sep_token="[SEP]",
+                                 pad_token="[PAD]", mask_token="[MASK]", padding_side="right", model_max_length=8192,
+                                 model_input_names=["input_ids", "attention_mask"])
+    os.makedirs(out_dir, exist_ok=True)
+    ft.save_pretrained(out_dir)
+    return out_dir
+
+
 def build_llama_tokenizer(out_dir: str, vocab_size: int = 32000) -> str:
     """Llama-style BPE (metaspace, byte fallback, <unk>/<s>/</s> = 0/1/2) wrapped in transformers' LlamaTokenizer so that
     `add_eos_token = True` (reference train_rage2e.py:304) behaves as it does for the real Llama-2 tokenizer."""
@@ -484,7 +544,7 @@ QWEN3_GENERATION = {
 def write_model_dir(out_dir: str, kind: str, name: str, vocab_size: Optional[int] = None, with_weights: bool = True,
                     seed: int = 0, generation_config: Optional[Dict] = None, bias_std: Optional[float] = None,
                     qk_norm_std: Optional[float] = None, headless: Optional[bool] = None) -> str:
-    """kind: 'bert' | 'roberta' | 'llama' | 'qwen2' | 'qwen3' | 'mistral' | 'falcon' ('roberta' takes a ROBERTA_SHAPES name: XLM-R
+    """kind: 'bert' | 'roberta' | 'modernbert' | 'llama' | 'qwen2' | 'qwen3' | 'mistral' | 'falcon' ('roberta' takes a ROBERTA_SHAPES name: XLM-R
     shapes get the XLM-R tokenizer, roberta-tiny the byte-level one; a Llama 3.x shape of LLAMA3_SHAPES takes kind 'llama' and
     gets the Llama 3 tokenizer; 'mistral' gets the Llama SentencePiece tokenizer). headless (mistral; default: the shape's own
     setting): a MistralModel directory, weights without the `model.` prefix and without lm_head. Writes config.json, tokenizer files and (optionally) seeded random-init
@@ -518,6 +578,9 @@ def write_model_dir(out_dir: str, kind: str, name: str, vocab_size: Optional[int
         if headless is not None:
             cfg["architectures"] = ["MistralModel" if headless else "MistralForCausalLM"]
         build_llama_tokenizer(out_dir, cfg["vocab_size"])
+    elif kind == "modernbert":
+        cfg = modernbert_config(name, vocab_size or 50368)
+        build_modernbert_tokenizer(out_dir, cfg["vocab_size"])
     elif kind == "falcon":
         cfg = falcon_config(name, vocab_size or 65024)
         build_llama_tokenizer(out_dir, cfg["vocab_size"])       # any causal-LM tokenizer works for the synthetic fixture

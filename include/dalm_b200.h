@@ -116,8 +116,10 @@ void dalm_b200_gemm_set_raster(int group_m);
 void dalm_b200_gemm_set_l2_hints(int mask);
 
 /* ---- attention (same call sites; HF eager/SDPA attention) ---- */
-/* window: 0 = no window; > 0 (causal only) = sliding window, query i sees key j iff i - window < j <= i, counted in the
- * padded row (Mistral; Qwen2 / Qwen3 with use_sliding_window). Probability dropout is not built with a window. */
+/* window: 0 = no window; > 0 = sliding window, counted in the padded row. Causal: query i sees key j iff
+ * i - window < j <= i (Mistral; Qwen2 / Qwen3 with use_sliding_window). Bidirectional: iff |i - j| < window (ModernBERT's
+ * local layers, window = local_attention / 2 + 1). Both combine with the key-padding mask; a query row that sees no key
+ * gets output 0, lse = +inf and contributes nothing to dQ / dK / dV. Probability dropout is not built with a window. */
 int dalm_b200_attention_fwd(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv,
                             const int64_t* mask, void* out, long long ldo, float* lse, int B, int L, int Hq, int Hkv,
                             int D, float scale, int causal, int window, float drop_p, unsigned long long drop_seed,
@@ -172,6 +174,10 @@ int dalm_b200_rope(void* buf, long long ld, int col0, int nheads, int D, const f
  * alternate [gate blk | up blk | ...] (the layout dalm_b200_gemm_bf16_swiglu produces) */
 int dalm_b200_swiglu_fwd(const void* gu, long long ldgu, void* act, long long lda, int M, int F, int interleave, void* stream);
 int dalm_b200_swiglu_bwd(void* gu, long long ldgu, const void* dact, long long ldd, int M, int F, int interleave, void* stream);
+/* x = [input | gate] = Wi(h).chunk(2) of ModernBertMLP (bf16 [M, 2F], any 16-byte-aligned row stride):
+ * act = gelu_erf(input) * gate. The backward works in place, x <- [d_input | d_gate], fp32 math. */
+int dalm_b200_geglu_fwd(const void* x, long long ldx, void* act, long long lda, int M, int F, void* stream);
+int dalm_b200_geglu_bwd(void* x, long long ldx, const void* dact, long long ldd, int M, int F, void* stream);
 int dalm_b200_gelu_fwd(const void* pre, long long ldp, void* act, long long lda, int M, int F, void* stream);
 int dalm_b200_gelu_bwd(const void* pre, long long ldp, void* dact, long long ldd, int M, int F, void* stream);
 /* mean_pooling + F.normalize (rag_e2e_base_model.py:96-97,108-111; retriever_only_base_model.py:60-68) */

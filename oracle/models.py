@@ -66,13 +66,53 @@ def build_bert(cfg: Dict, state_dict: Dict[str, torch.Tensor]) -> nn.Module:
     return m.float().eval()
 
 
-def build_llama(cfg: Dict, state_dict: Dict[str, torch.Tensor]) -> nn.Module:
-    from transformers import LlamaConfig, LlamaForCausalLM
+def build_roberta(cfg: Dict, state_dict: Dict[str, torch.Tensor]) -> nn.Module:
+    """transformers' XLMRobertaModel / RobertaModel (by model_type), eager attention"""
+    import transformers
 
-    c = LlamaConfig(**{k: v for k, v in cfg.items() if k not in ("architectures", "model_type")})
-    m = LlamaForCausalLM(c)
-    m.load_state_dict({k: v.float() for k, v in state_dict.items()}, strict=True)
+    prefix = "Roberta" if cfg["model_type"] == "roberta" else "XLMRoberta"
+    c = getattr(transformers, prefix + "Config")(**{k: v for k, v in cfg.items() if k not in ("architectures", "model_type")},
+                                                  _attn_implementation="eager")
+    m = getattr(transformers, prefix + "Model")(c)
+    missing, unexpected = m.load_state_dict({k: v.float() for k, v in state_dict.items()}, strict=False)
+    assert not [k for k in missing if "position_ids" not in k and "token_type_ids" not in k], missing
+    assert not unexpected, unexpected
     return m.float().eval()
+
+
+def build_modernbert(cfg: Dict, state_dict: Dict[str, torch.Tensor]) -> nn.Module:
+    """transformers' ModernBertModel, eager attention"""
+    from transformers import ModernBertConfig, ModernBertModel
+
+    c = ModernBertConfig(**{k: v for k, v in cfg.items() if k not in ("architectures", "model_type")},
+                         _attn_implementation="eager")
+    m = ModernBertModel(c)
+    missing, unexpected = m.load_state_dict(state_dict, strict=False)
+    assert not missing and not unexpected, (missing, unexpected)
+    return m.float().eval()
+
+
+_CAUSAL_LM = {"llama": "Llama", "qwen2": "Qwen2", "qwen3": "Qwen3", "mistral": "Mistral"}
+
+
+def build_causal_lm(cfg: Dict, state_dict: Dict[str, torch.Tensor], headless: bool = False,
+                    attn_implementation: Optional[str] = None) -> nn.Module:
+    """transformers' <Family>ForCausalLM, or <Family>Model when `headless`, for cfg["model_type"] in llama / qwen2 / qwen3 /
+    mistral. attn_implementation None keeps transformers' default. A config with tie_word_embeddings may store no lm_head."""
+    import transformers
+
+    family = _CAUSAL_LM[cfg["model_type"]]
+    c = getattr(transformers, family + "Config")(**{k: v for k, v in cfg.items() if k not in ("architectures", "model_type")})
+    cls = getattr(transformers, family + ("Model" if headless else "ForCausalLM"))
+    m = cls(c) if attn_implementation is None else cls._from_config(c, attn_implementation=attn_implementation)
+    missing, unexpected = m.load_state_dict({k: v.float() for k, v in state_dict.items()}, strict=False)
+    tied = {"lm_head.weight"} if cfg.get("tie_word_embeddings") else set()
+    assert not unexpected and set(missing) <= tied, (missing, unexpected)
+    return m.float().eval()
+
+
+def build_llama(cfg: Dict, state_dict: Dict[str, torch.Tensor]) -> nn.Module:
+    return build_causal_lm({**cfg, "model_type": "llama"}, state_dict)
 
 
 def build_falcon(cfg: Dict, state_dict: Dict[str, torch.Tensor]) -> nn.Module:

@@ -4,13 +4,10 @@ import math
 import pytest
 import torch
 
+from model_helpers import rel
+
 pytestmark = pytest.mark.gpu
 bf16 = torch.bfloat16
-
-
-def _rel(a, b):
-    a, b = a.double(), b.double()
-    return ((a - b).norm() / (b.norm() + 1e-30)).item()
 
 
 def _ref(q, k, v, mask, causal, B, L, Hq, Hkv, D):
@@ -47,10 +44,10 @@ def test_attention_tc_forward(cuda_dev, B, L, Hq, Hkv, causal, pad):
     if B * L * Hq <= 20000:
         ref = _ref(q, k, v, mask, causal, B, L, Hq, Hkv, D)
         rows = mask.bool().view(-1) if (causal and pad == "left") else torch.ones(B * L, dtype=torch.bool, device=dev)
-        assert _rel(out.float()[rows], ref[rows]) < 1.5e-2
+        assert rel(out.float()[rows], ref[rows]) < 1.5e-2
         if causal and pad == "left":
             assert out.float()[~rows].abs().max().item() == 0.0
-    assert _rel(out.float(), out2.float()) < 1.5e-2
+    assert rel(out.float(), out2.float()) < 1.5e-2
     fin = torch.isfinite(lse2)
     assert torch.equal(torch.isfinite(lse), fin)
     assert (lse[fin] - lse2[fin]).abs().max().item() < 2e-2
@@ -82,13 +79,13 @@ def test_attention_tc_backward(cuda_dev, B, L, Hq, Hkv, causal, pad):
     dqkv = torch.zeros(B * L, (Hq + 2 * Hkv) * D + 64, device=dev, dtype=bf16)          # outputs are column slices of a wider buffer
     dq, dk, dv = ops.attention_tc_bwd(q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq=dqkv[:, :Hq * D],
                                       dk=dqkv[:, Hq * D:(Hq + Hkv) * D], dv=dqkv[:, (Hq + Hkv) * D:(Hq + 2 * Hkv) * D])
-    assert _rel(dq.float(), qd.grad) < 3e-2
-    assert _rel(dk.float(), kd.grad) < 3e-2
-    assert _rel(dv.float(), vd.grad) < 3e-2
+    assert rel(dq.float(), qd.grad) < 3e-2
+    assert rel(dk.float(), kd.grad) < 3e-2
+    assert rel(dv.float(), vd.grad) < 3e-2
     assert dqkv[:, (Hq + 2 * Hkv) * D:].abs().max().item() == 0
     # and against the mma.sync kernels
     dq2, dk2, dv2 = ops.attention_bwd(q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal)
-    assert _rel(dq.float(), dq2.float()) < 2e-2 and _rel(dk.float(), dk2.float()) < 2e-2 and _rel(dv.float(), dv2.float()) < 2e-2
+    assert rel(dq.float(), dq2.float()) < 2e-2 and rel(dk.float(), dk2.float()) < 2e-2 and rel(dv.float(), dv2.float()) < 2e-2
 
 
 def test_attention_tc_speed_report(cuda_dev, capsys):
@@ -165,14 +162,14 @@ def test_attention_tc_head_dim_64(cuda_dev, B, L, Hq, Hkv, causal, pad, p_drop):
     qd, kd, vd = (t.detach().double().requires_grad_(True) for t in (q, k, v))
     ref = _ref64(qd, kd, vd, mask, causal, B, L, Hq, Hkv, D, dm)
     rows = mask.bool().view(-1) if (causal and pad == "left") else torch.ones(B * L, dtype=torch.bool, device=dev)
-    assert _rel(out.float()[rows], ref[rows]) < 1.5e-2
+    assert rel(out.float()[rows], ref[rows]) < 1.5e-2
     if causal and pad == "left":
         assert out.float()[~rows].abs().max().item() == 0.0
     # LSE against the mma.sync kernel's (same definition: natural log, +inf for fully masked rows)
     out2, lse2 = ops.attention_fwd(q, k, v, mask, B, L, Hq, Hkv, D, causal, drop=d)
     fin = torch.isfinite(lse2)
     assert torch.equal(torch.isfinite(lse), fin) and (lse[fin] - lse2[fin]).abs().max().item() < 2e-2
-    assert _rel(out.float(), out2.float()) < 1.5e-2                                      # identical dropout masks in both kernels
+    assert rel(out.float(), out2.float()) < 1.5e-2                                      # identical dropout masks in both kernels
     d_out = torch.randn(B * L, Hq * D, device=dev).to(bf16)
     d_out[~rows] = 0
     ref.backward(d_out.double())
@@ -180,9 +177,9 @@ def test_attention_tc_head_dim_64(cuda_dev, B, L, Hq, Hkv, causal, pad, p_drop):
     dq, dk, dv = ops.attention_tc_bwd(q, k, v, mask, out, lse, d_out, B, L, Hq, Hkv, D, causal, dq=dqkv[:, :Hq * D],
                                       dk=dqkv[:, Hq * D:(Hq + Hkv) * D], dv=dqkv[:, (Hq + Hkv) * D:wide], drop=d)
     tol = 3e-2 if Hq // Hkv < 8 else 4e-2                            # MQA sums 71 heads' bf16-rounded P / dS into one dK / dV
-    assert _rel(dq.float(), qd.grad) < tol
-    assert _rel(dk.float(), kd.grad) < tol
-    assert _rel(dv.float(), vd.grad) < tol
+    assert rel(dq.float(), qd.grad) < tol
+    assert rel(dk.float(), kd.grad) < tol
+    assert rel(dv.float(), vd.grad) < tol
     assert dqkv[:, wide:].abs().max().item() == 0
 
 

@@ -15,11 +15,6 @@ def _free_port():
     s = socket.socket(); s.bind(("127.0.0.1", 0)); p = s.getsockname()[1]; s.close(); return p
 
 
-def _rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return ((a - b).norm() / (b.norm() + 1e-30)).item()
-
-
 def _worker(rank, world, port, q):
     os.environ.update(RANK=str(rank), WORLD_SIZE=str(world), LOCAL_RANK=str(rank), MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     import sys
@@ -31,11 +26,11 @@ def _worker(rank, world, port, q):
         from dalm_b200.accel import Accelerator
         from dalm_b200.training.utils.train_utils import fused_rag_step
         from oracle import models as om
-        import test_step_gpu as T
+        from model_helpers import llama_rag_models, r16_2d, rag_batch, rel
         acc = Accelerator()
         dev = torch.device("cuda", rank)
-        model, enc, dec, bert, llama = T._models(dev)                       # same seeds on both ranks (DDP broadcast semantics)
-        batches = [T._batch(5, 12, 24, 40, 600, 500, seed=70 + r, pad="left") for r in range(world)]
+        model, enc, dec, bert, llama = llama_rag_models(dev, 500, r16_2d)    # same seeds on both ranks (DDP broadcast semantics)
+        batches = [rag_batch(5, 12, 24, 40, 600, 500, seed=70 + r, pad="left") for r in range(world)]
         enc.lora.zero_grad(); dec.lora.zero_grad()
         out = fused_rag_step(model, batches[rank], 100.0)
         sync = acc.gradient_sync(model.trainable_banks())
@@ -50,7 +45,7 @@ def _worker(rank, world, port, q):
                 for n, _, _ in bank.specs:
                     for g, key in ((bank.gA[n] * sync.grad_scale, pre + n + ".lora_A"), (bank.gB[n] * sync.grad_scale, pre + n + ".lora_B")):
                         mean = sum(r["grads"][key] for r in refs) / world
-                        worst = max(worst, _rel(g, mean))
+                        worst = max(worst, rel(g, mean))
             ok = ok and worst < 6e-2
             # and the exchange itself is exact: what every rank holds == the fp32 mean of the two local gradients
         local = torch.cat([b.grad.clone() for b in model.trainable_banks()])
@@ -93,18 +88,14 @@ def _neg_worker(rank, world, port, q):
         from dalm_b200.training.utils import negatives
         from dalm_b200.training.utils.train_utils import fused_retriever_step
         from oracle import models as om, losses
-        import test_step_gpu as T
+        from model_helpers import llama_rag_models, r16_2d, rag_batch, rel, retriever_batch
         acc = Accelerator()
         assert negatives.active()
         dev = torch.device("cuda", rank)
-        _, enc, _, bert, _ = T._models(dev)
+        _, enc, _, bert, _ = llama_rag_models(dev, 500, r16_2d)
         se = AutoModelForSentenceEmbedding("", use_bnb=False, get_peft=True, _model=enc, _load_tokenizer=False)
         Bs = [6, 4]                                                            # a short batch on rank 1
-        rbs = []
-        for r in range(world):
-            b = T._batch(Bs[r], 12, 24, 8, 600, 500, seed=90 + r)
-            rbs.append({"query_input_ids": b["retriever_query_input_ids"], "query_attention_mask": b["retriever_query_attention_mask"],
-                        "passage_input_ids": b["retriever_passage_input_ids"], "passage_attention_mask": b["retriever_passage_attention_mask"]})
+        rbs = [retriever_batch(rag_batch(Bs[r], 12, 24, 8, 600, 500, seed=90 + r)) for r in range(world)]
         enc.lora.zero_grad()
         out = fused_retriever_step(se, rbs[rank], 100.0)
         sync = acc.gradient_sync(se.trainable_banks() if hasattr(se, "trainable_banks") else enc.banks())
@@ -123,7 +114,7 @@ def _neg_worker(rank, world, port, q):
             for n, _, _ in enc.lora.specs:
                 for g, key in ((enc.lora.gA[n] * sync.grad_scale, n + ".lora_A"), (enc.lora.gB[n] * sync.grad_scale, n + ".lora_B")):
                     want = next(v for k, v in grads.items() if k.endswith(key + ".weight") or k.endswith(key))
-                    worst = max(worst, _rel(g, want))
+                    worst = max(worst, rel(g, want))
             ok = ok and worst < 8e-2
         q.put((rank, bool(ok), worst))
         dist.barrier()

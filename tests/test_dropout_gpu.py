@@ -7,13 +7,10 @@ import math
 import pytest
 import torch
 
+from model_helpers import rel
+
 pytestmark = pytest.mark.gpu
 bf16, f32 = torch.bfloat16, torch.float32
-
-
-def _rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return ((a - b).norm() / (b.norm() + 1e-30)).item()
 
 
 def test_generator_statistics_and_counters(cuda_dev):
@@ -48,21 +45,21 @@ def test_gemm_and_layernorm_sites_exact(cuda_dev):
     out = ops.gemm(a, b, out_dtype=f32, bias=bias, resid=res, drop=d)
     mask = ops.dropout_scale(M * N, d, dev).view(M, N)
     ref = (a.float() @ b.float().t() + bias) * mask + res          # dropout(dense) + residual (BertSelfOutput)
-    assert _rel(out, ref) < 1e-5
+    assert rel(out, ref) < 1e-5
     for bn in (64, 128, 2128):
-        assert _rel(ops.gemm(a, b, out_dtype=f32, bias=bias, resid=res, drop=d, block_n=bn), ref) < 1e-5
+        assert rel(ops.gemm(a, b, out_dtype=f32, bias=bias, resid=res, drop=d, block_n=bn), ref) < 1e-5
     # layernorm: forward output dropout, backward bf16-branch mask
     for H in (256, 1024, 384):                                     # warp-per-row kernels (256, 1024) and the CTA-per-row ones (384)
         z = torch.randn(M, H, device=dev); g = torch.randn(H, device=dev); be = torch.randn(H, device=dev)
         d0 = ops.Drop(0.1, 99, 7, None)
         y32, y16, mean, rstd = ops.layernorm_fwd(z, g, be, 1e-12, drop=d0)
         m0 = ops.dropout_scale(M * H, d0, dev).view(M, H)
-        assert _rel(y32, torch.nn.functional.layer_norm(z, (H,), g, be, 1e-12) * m0) < 1e-5
+        assert rel(y32, torch.nn.functional.layer_norm(z, (H,), g, be, 1e-12) * m0) < 1e-5
         dy = torch.randn(M, H, device=dev)
         dz32, dz16 = ops.layernorm_bwd(z, g, mean, rstd, dy_f32=dy, drop16=d0)
         dz32b, dz16b = ops.layernorm_bwd(z, g, mean, rstd, dy_f32=dy)
         assert torch.equal(dz32, dz32b)                                # residual branch unmasked
-        assert _rel(dz16.float(), dz32 * m0) < 4e-3                    # dense branch = mask * dz / (1-p)
+        assert rel(dz16.float(), dz32 * m0) < 4e-3                    # dense branch = mask * dz / (1-p)
 
 
 @pytest.mark.parametrize("B,L,H,D", [(2, 50, 4, 64), (3, 37, 2, 32)])
@@ -81,11 +78,11 @@ def test_attention_probability_dropout_exact(cuda_dev, B, L, H, D):
     qh = qd.view(B, L, H, D).transpose(1, 2); kh = kd.view(B, L, H, D).transpose(1, 2); vh = vd.view(B, L, H, D).transpose(1, 2)
     s = (qh @ kh.transpose(-1, -2) / math.sqrt(D)).masked_fill(mask.view(B, 1, 1, L) == 0, float("-inf"))
     ref = ((torch.softmax(s, -1) * dm) @ vh).transpose(1, 2).reshape(B * L, H * D)
-    assert _rel(out.float(), ref) < 1.5e-2
+    assert rel(out.float(), ref) < 1.5e-2
     do = torch.randn(B * L, H * D, device=dev).to(bf16)
     ref.backward(do.double())
     dq, dk, dv = ops.attention_bwd(q, k, v, mask, out, lse, do, B, L, H, H, D, False, drop=d)
-    assert _rel(dq.float(), qd.grad) < 3e-2 and _rel(dk.float(), kd.grad) < 3e-2 and _rel(dv.float(), vd.grad) < 3e-2
+    assert rel(dq.float(), qd.grad) < 3e-2 and rel(dk.float(), kd.grad) < 3e-2 and rel(dv.float(), vd.grad) < 3e-2
 
 
 def test_lora_input_dropout_sites_exact(cuda_dev):
@@ -99,16 +96,16 @@ def test_lora_input_dropout_sites_exact(cuda_dev):
     d = ops.Drop(0.05, 11, 2 << 8 | 3, None)
     xm = x.float() * ops.dropout_scale(M * K, d, dev).view(M, K)
     ops.skinny_gemm(x, a_stack, buf[:, K:], K=K, R=R, dropx=d)
-    assert _rel(buf[:, K:K + R].float(), xm @ a_stack[:R].float().t()) < 5e-3
+    assert rel(buf[:, K:K + R].float(), xm @ a_stack[:R].float().t()) < 5e-3
     g = (torch.randn(M, R, device=dev) * 0.2).to(bf16)
     o0 = torch.zeros(8, K, device=dev); o1 = torch.zeros(8, K, device=dev)
     ops.lora_wgrad_(x, g, o0, K, 1, K, R, 1.0, out1=o1, dropx=d)
     xm16 = xm.to(bf16).float()                                     # the kernel masks the bf16 tile before the MMA
-    assert _rel(o0, g[:, :8].float().t() @ xm16) < 1e-4 and _rel(o1, g[:, 8:].float().t() @ xm16) < 1e-4
+    assert rel(o0, g[:, :8].float().t() @ xm16) < 1e-4 and rel(o1, g[:, 8:].float().t() @ xm16) < 1e-4
     dh = (torch.randn(M, K, device=dev) * 0.1).to(bf16)
     ref = dh.float() + ops.dropout_scale(M * K, d, dev).view(M, K) * (g.float() @ a_stack[:R].float())
     ops.lora_dx_(dh, g, a_stack, K=K, R=R, drop=d)
-    assert _rel(dh.float(), ref) < 4e-3
+    assert rel(dh.float(), ref) < 4e-3
 
 
 def test_bert_encoder_train_mode_matches_hf_with_replayed_masks(cuda_dev, monkeypatch):
@@ -156,7 +153,7 @@ def test_bert_encoder_train_mode_matches_hf_with_replayed_masks(cuda_dev, monkey
     ref_hid = ref(ids, mask)[0]
     assert len(used) == len(queue)
     valid = mask.bool()
-    assert _rel(hid.cpu()[valid], ref_hid[valid]) < 1.2e-2
+    assert rel(hid.cpu()[valid], ref_hid[valid]) < 1.2e-2
     emb, norm = ops.pool_norm_fwd(hid, mask.to(cuda_dev), True)
     ref_emb = pooling.normalize(pooling.mean_pooling(ref_hid, mask))
     d_emb = torch.randn(B, H, generator=g)
@@ -166,7 +163,7 @@ def test_bert_encoder_train_mode_matches_hf_with_replayed_masks(cuda_dev, monkey
     worst = 0.0
     for n, _, _ in enc.lora.specs:
         mod = om._get_module(ref, n)
-        worst = max(worst, _rel(enc.lora.gA[n], mod.lora_A.grad), _rel(enc.lora.gB[n], mod.lora_B.grad))
+        worst = max(worst, rel(enc.lora.gA[n], mod.lora_A.grad), rel(enc.lora.gB[n], mod.lora_B.grad))
     assert worst < 6e-2, worst
     # eval() switches every site off again
     enc.eval()
@@ -189,4 +186,4 @@ def test_lora_dx_row_widths(cuda_dev, M, K, R, p):
     scale = ops.dropout_scale(M * K, d, dev).view(M, K) if d is not None else 1.0
     ref = dh.float() + scale * (g.float() @ a_stack[:R].float())
     ops.lora_dx_(dh, g, a_stack, K=K, R=R, drop=d)
-    assert _rel(dh.float(), ref) < 4e-3
+    assert rel(dh.float(), ref) < 4e-3

@@ -2,13 +2,10 @@
 import pytest
 import torch
 
+from model_helpers import rel
+
 pytestmark = pytest.mark.gpu
 bf16, f32 = torch.bfloat16, torch.float32
-
-
-def _rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return ((a - b).norm() / (b.norm() + 1e-30)).item()
 
 
 def test_single_sample_batch_losses(cuda_dev):
@@ -30,7 +27,7 @@ def test_single_sample_batch_losses(cuda_dev):
     tok_lp, dl = ops.ce_marginal(logits.to(dev), ids.to(dev), mask.to(dev), nsum)
     out = ops.finalize_loss(tok_lp, mask.to(dev), nsum, r["losses"])
     assert abs(out[2].item() - ref["loss"].item()) < 1e-5 * abs(ref["loss"].item())
-    assert _rel(dl, ref["dlogits"]) < 1e-5
+    assert rel(dl, ref["dlogits"]) < 1e-5
 
 
 def test_fully_masked_and_single_position(cuda_dev):
@@ -64,9 +61,9 @@ def test_length_one_sequences_and_single_row_gemm(cuda_dev):
     ref = om.build_bert(cfg, sd)
     ids = torch.tensor([[7]]); mask = torch.ones(1, 1, dtype=torch.int64)              # B = 1, L = 1
     hid, _ = enc.forward_hidden(ids.to(cuda_dev), mask.to(cuda_dev), save=False)
-    assert _rel(hid, ref(ids, mask)[0]) < 1e-2
+    assert rel(hid, ref(ids, mask)[0]) < 1e-2
     a = torch.randn(1, 64, device=cuda_dev).to(bf16); b = torch.randn(8, 64, device=cuda_dev).to(bf16)
-    assert _rel(ops.gemm(a, b, out_dtype=f32), a.float() @ b.float().t()) < 1e-5
+    assert rel(ops.gemm(a, b, out_dtype=f32), a.float() @ b.float().t()) < 1e-5
 
 
 @pytest.mark.parametrize("L", [1, 5, 127, 129, 257])
@@ -79,7 +76,7 @@ def test_tc_attention_ragged_lengths(cuda_dev, L):
     mask = torch.ones(B, L, dtype=torch.int64, device=cuda_dev)
     o1, l1 = ops.attention_tc_fwd(q, k, v, mask, B, L, H, H, D, True)
     o2, l2 = ops.attention_fwd(q, k, v, mask, B, L, H, H, D, True)
-    assert _rel(o1.float(), o2.float()) < 1.5e-2 and (l1 - l2).abs().max().item() < 2e-2
+    assert rel(o1.float(), o2.float()) < 1.5e-2 and (l1 - l2).abs().max().item() < 2e-2
     do = torch.randn_like(o1)
     g1 = ops.attention_tc_bwd(q, k, v, mask, o1, l1, do, B, L, H, H, D, True)
     g2 = ops.attention_bwd(q, k, v, mask, o1, l1, do, B, L, H, H, D, True)
@@ -87,7 +84,7 @@ def test_tc_attention_ragged_lengths(cuda_dev, L):
         if b.float().norm().item() < 1e-3:                    # L = 1: dq = dk = 0 analytically (softmax of one entry); compare absolutely
             assert (a.float() - b.float()).abs().max().item() < 1e-5
         else:
-            assert _rel(a.float(), b.float()) < 3e-2
+            assert rel(a.float(), b.float()) < 3e-2
 
 
 def test_empty_inputs_are_rejected(cuda_dev):

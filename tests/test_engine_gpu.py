@@ -6,17 +6,9 @@ relative L2 norm with bf16-forward budgets written at each check; LoRA gradients
 import pytest
 import torch
 
+from model_helpers import attach_lora, check_decoder, draw_lora_B, hf_grads, lora_grad_error, r16_2d, rel
+
 pytestmark = pytest.mark.gpu
-bf16, f32 = torch.bfloat16, torch.float32
-
-
-def _rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return ((a - b).norm() / (b.norm() + 1e-30)).item()
-
-
-def _bert_factors(enc):
-    return {n: {"A": enc.lora.A[n].cpu(), "B": enc.lora.B[n].cpu()} for n, _, _ in enc.lora.specs}
 
 
 @pytest.mark.parametrize("name,B,L", [("bge-tiny", 3, 20), ("bge-small-en", 2, 50)])
@@ -29,15 +21,12 @@ def test_bert_encoder_fwd_bwd(cuda_dev, name, B, L):
     sd = params.random_state_dict("bert", cfg, seed=1)
     # the engine stores matmul weights in bf16: give the oracle the same (bf16-rounded) values so the comparison
     # isolates arithmetic, not weight quantisation
-    sd = {k: (v.to(bf16).float() if v.dim() == 2 else v) for k, v in sd.items()}
+    sd = r16_2d(sd)
     enc = BertEncoder(cfg, sd, device=cuda_dev, lora=True)
-    # non-zero B so that the LoRA path is exercised in forward and dA is non-trivial
     g = torch.Generator().manual_seed(5)
-    for n, _, _ in enc.lora.specs:
-        enc.lora.B[n].copy_((torch.randn(enc.lora.B[n].shape, generator=g) * 0.02).to(cuda_dev))
-    enc.repack_lora()
+    draw_lora_B(enc, g)
     ref = om.build_bert(cfg, sd)
-    om.attach_lora(ref, _bert_factors(enc))
+    attach_lora(ref, enc)
     ids = torch.randint(5, 1000, (B, L), generator=g)
     mask = torch.ones(B, L, dtype=torch.int64)
     mask[0, L - 6:] = 0
@@ -45,20 +34,17 @@ def test_bert_encoder_fwd_bwd(cuda_dev, name, B, L):
     ref_hid = ref(ids, mask)[0]
     valid = mask.bool()
     # bf16 GEMM operands through N layers: budget 1e-2 relative on the hidden states of valid tokens
-    assert _rel(hid.cpu()[valid], ref_hid[valid]) < 1e-2
+    assert rel(hid.cpu()[valid], ref_hid[valid]) < 1e-2
     emb, norm = ops.pool_norm_fwd(hid, mask.to(cuda_dev), True)
     ref_emb = pooling.normalize(pooling.mean_pooling(ref_hid, mask))
-    assert _rel(emb, ref_emb) < 5e-3
+    assert rel(emb, ref_emb) < 5e-3
     # backward from a random embedding gradient
     d_emb = torch.randn(B, cfg["hidden_size"], generator=g)
     ref_emb.backward(d_emb)
     d_hid = ops.pool_norm_bwd(emb, norm, d_emb.to(cuda_dev), mask.to(cuda_dev), L, True)
     enc.lora.zero_grad()
     enc.backward_hidden(ctx, d_hid)
-    worst = 0.0
-    for n, _, _ in enc.lora.specs:
-        mod = om._get_module(ref, n)
-        worst = max(worst, _rel(enc.lora.gA[n], mod.lora_A.grad), _rel(enc.lora.gB[n], mod.lora_B.grad))
+    worst = lora_grad_error(enc, hf_grads(ref))
     # gradients flow through bf16 activations/gradients: budget 5e-2 relative per factor
     assert worst < 5e-2, worst
 
@@ -66,46 +52,18 @@ def test_bert_encoder_fwd_bwd(cuda_dev, name, B, L):
 @pytest.mark.parametrize("name,B,L,pad", [("llama-tiny", 3, 24, "right"), ("llama-tiny", 2, 40, "left"), ("llama-mini", 2, 64, "right"),
                                            ("llama-hd128", 2, 150, "right"), ("llama-hd128", 2, 72, "left")])
 def test_llama_decoder_fwd_bwd(cuda_dev, name, B, L, pad):
-    from dalm_b200 import ops, synthetic
+    from dalm_b200 import synthetic
     from dalm_b200.engine import params
     from dalm_b200.engine.llama import LlamaDecoder
-    from oracle import models as om, losses
+    from oracle import models as om
     cfg = synthetic.llama_config(name, vocab_size=512)
-    sd = params.random_state_dict("llama", cfg, seed=2)
-    sd = {k: (v.to(bf16).float() if v.dim() == 2 else v) for k, v in sd.items()}
+    sd = r16_2d(params.random_state_dict("llama", cfg, seed=2))
     dec = LlamaDecoder(cfg, sd, device=cuda_dev, lora=True)
     g = torch.Generator().manual_seed(9)
-    for n, _, _ in dec.lora.specs:
-        dec.lora.B[n].copy_((torch.randn(dec.lora.B[n].shape, generator=g) * 0.02).to(cuda_dev))
-    dec.repack_lora()
+    draw_lora_B(dec, g)
     ref = om.build_llama(cfg, sd)
-    om.attach_lora(ref, {n: {"A": dec.lora.A[n].cpu(), "B": dec.lora.B[n].cpu()} for n, _, _ in dec.lora.specs})
-    ids = torch.randint(3, 512, (B, L), generator=g)
-    mask = torch.ones(B, L, dtype=torch.int64)
-    if pad == "right":
-        mask[0, L - 5:] = 0
-    else:
-        mask[0, :5] = 0; mask[1, :2] = 0
-    qlen = torch.tensor([3, L // 2, L + 2][:B])
-    S = torch.randn(B, B, generator=g) * 3
-    logits, ctx = dec.forward_logits(ids.to(cuda_dev), mask.to(cuda_dev))
-    ref_logits = ref(input_ids=ids, attention_mask=mask).logits
-    valid = mask.bool()
-    assert _rel(logits.float().cpu()[valid], ref_logits[valid]) < 1.5e-2
-    # loss through the reference's own formula on both sides
-    ref_loss = losses.marginalized_loss_loopform(ref_logits, ids, mask, S, qlen)
-    ref_loss.backward()
-    cvec, nsum = ops.marginal_counts(mask.to(cuda_dev), qlen.to(cuda_dev))
-    tok_lp, dl = ops.ce_marginal(logits, ids.to(cuda_dev), mask.to(cuda_dev), nsum)
-    mine = losses.marginalized_loss_loopform(logits.float().cpu(), ids, mask, S, qlen)
-    assert abs(mine.item() - ref_loss.item()) / abs(ref_loss.item()) < 1e-3          # north_star tolerance
-    dec.lora.zero_grad()
-    dec.backward_logits(ctx, dl)
-    worst = 0.0
-    for n, _, _ in dec.lora.specs:
-        mod = om._get_module(ref, n)
-        worst = max(worst, _rel(dec.lora.gA[n], mod.lora_A.grad), _rel(dec.lora.gB[n], mod.lora_B.grad))
-    assert worst < 5e-2, worst
+    attach_lora(ref, dec)
+    check_decoder(dec, ref, g, 512, B, L, pad)                            # the ids continue the LoRA draws' generator
 
 
 @pytest.mark.parametrize("name,B,L,pad", [("falcon-tiny", 3, 40, "right"), ("falcon-mini", 2, 130, "left")])
@@ -117,8 +75,7 @@ def test_falcon_decoder_forward(cuda_dev, name, B, L, pad):
     from dalm_b200.engine.falcon import FalconDecoder
     from oracle import models as om, losses
     cfg = synthetic.falcon_config(name, vocab_size=504)
-    sd = params.random_state_dict("falcon", cfg, seed=4)
-    sd = {k: (v.to(bf16).float() if v.dim() == 2 else v) for k, v in sd.items()}
+    sd = r16_2d(params.random_state_dict("falcon", cfg, seed=4))
     dec = FalconDecoder(cfg, sd, device=cuda_dev)
     with pytest.raises(ValueError):
         FalconDecoder(cfg, sd, device=cuda_dev, lora=True)
@@ -132,7 +89,7 @@ def test_falcon_decoder_forward(cuda_dev, name, B, L, pad):
     with torch.no_grad():
         ref_logits = ref(input_ids=ids, attention_mask=mask).logits
     valid = mask.bool()
-    assert _rel(logits.float().cpu()[valid], ref_logits[valid]) < 1.5e-2
+    assert rel(logits.float().cpu()[valid], ref_logits[valid]) < 1.5e-2
     S = torch.randn(B, B, generator=g) * 3
     qlen = torch.tensor([3, L // 2, L + 2][:B])
     want = losses.marginalized_loss_loopform(ref_logits, ids, mask, S, qlen)

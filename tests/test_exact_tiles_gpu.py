@@ -18,31 +18,15 @@ import random
 import pytest
 import torch
 
-from exact_helpers import PAD_R, Guarded, _expect_close, _expect_equal, _poisoned, _ulp_bf16, _ulp_f32
+from exact_helpers import (M_EDGE, PAD_R, STAGES, Guarded, _attn_fns, _attn_ref64, _expect_close, _expect_equal,  # noqa: F401
+                           _gelu64, _ints, _pick_block_n, _poisoned, _row_mask, _ulp_bf16, _ulp_f32, dev, ops)
 
 bf16, f32, f64 = torch.bfloat16, torch.float32, torch.float64
-
-
-@pytest.fixture(scope="module")
-def dev():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from dalm_b200 import _lib
-    _lib.call("dalm_b200_probe_device")
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(scope="module")
-def ops(dev):
-    from dalm_b200 import ops as _ops
-    return _ops
 
 
 # ----------------------------------------------------------------------------------------------------------------
 # 1. GEMM: integer operands, exact comparison
 # ----------------------------------------------------------------------------------------------------------------
-STAGES = {64: 8, 128: 6, 256: 4}                 # GemmCfg<BN>::STAGES: depth of the shared-memory ring
-M_EDGE = (1, 127, 128, 129, 255, 256, 257)       # 128 = the CTA tile's rows, 256 = the cluster's
 M_EDGE_WGRAD = (8, 120, 128, 136, 248, 256, 264)  # the wgrad layout needs M % 8 == 0
 K_EDGE = (8, 56, 64, 72)                         # 64 = one k-block
 T_EDGE = (1, 7, 63, 65)                          # wgrad contraction over token rows: no multiple-of-8 requirement
@@ -61,14 +45,6 @@ VARIANTS = (
     dict(out=bf16, bias=True, act=2),
     dict(out=bf16, alpha=4.0, resid=bf16, inplace=True),
 )
-
-
-def _ints(shape, g, hi=2):
-    return torch.randint(-hi, hi + 1, shape, generator=g).to(f32)
-
-
-def _gelu64(x):
-    return 0.5 * x * (1.0 + torch.erf(x / math.sqrt(2.0)))
 
 
 def _gelu_grad64(x):
@@ -171,18 +147,6 @@ def test_gemm_exact_ring_depth(ops, dev, layout, bn):
             _run_gemm(ops, dev, layout, bn, M, N, K, VARIANTS[(i + 3 * layout) % len(VARIANTS)],
                       max_ctas=ctas * (2 if bn > 1000 else 1), seed=100 + i)
             i += 1
-
-
-def _pick_block_n(M, N, sms):
-    """the tile width gemm_gelu takes (pick_block_n in gemm_wgmma.cu)"""
-    m1, best, bn = -(-M // 128), 1e30, 64
-    for cand, pen in ((256, 1.0), (128, 1.55), (64, 2.7)):
-        if cand > 64 and N < cand:
-            continue
-        cost = -(-(m1 * -(-N // cand)) // sms) * cand * pen
-        if cost < best:
-            best, bn = cost, cand
-    return bn
 
 
 def _gelu_shapes(sms):
@@ -424,10 +388,6 @@ def test_selector_construction(kind, D, drop, L, causal, Hq, Hkv, scale):
         assert (leak.max(-1).values > best[:-1])[valid[:-1]].any(), "no attractor in the next sample's rows"
 
 
-def _attn_fns(ops, kind):
-    return (ops.attention_tc_fwd, ops.attention_tc_bwd) if kind == "wg" else (ops.attention_fwd, ops.attention_bwd)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("kind,D,drop,L,causal,Hq,Hkv,scale", SELECTOR_PARAMS)
 def test_attention_selector_exact(ops, dev, kind, D, drop, L, causal, Hq, Hkv, scale):
@@ -466,40 +426,6 @@ def test_attention_selector_exact(ops, dev, kind, D, drop, L, causal, Hq, Hkv, s
         b, h, i = torch.nonzero(valid)[err.argmax()].tolist()
         pytest.fail(f"{what}: lse off by {err.max().item():.3e} at (sample {b}, head {h}, query {i})")
     out.check(what + " out")
-
-
-def _row_mask(B, L, pattern, g):
-    mask = torch.ones(B, L, dtype=torch.int64)
-    if pattern == "right64":                              # >= 64 pad tokens: a fully masked second KV tile
-        mask[0, max(1, L - 70):] = 0
-        mask[1, 64:] = 0
-        mask[2, L - 5:] = 0
-    elif pattern == "left64":
-        mask[0, : min(L - 1, max(64, L - 10))] = 0
-        mask[1, :64] = 0
-        mask[2, :3] = 0
-    elif pattern == "holes":
-        mask = (torch.rand(B, L, generator=g) > 0.3).long()
-        mask[1, 10:min(L - 1, 74)] = 0
-        mask[:, 0] = 1
-    elif pattern == "empty":                              # sample 1: every key masked
-        mask[0, L - 7:] = 0
-        mask[1] = 0
-    return mask
-
-
-def _attn_ref64(q, k, v, vis, B, L, Hq, Hkv, D, scale):
-    """fp64 attention with an explicit safe softmax: rows without a visible key give zero output, lse -inf, zero gradient"""
-    qh = q.view(B, L, Hq, D).transpose(1, 2)
-    kh = k.view(B, L, Hkv, D).transpose(1, 2).repeat_interleave(Hq // Hkv, 1)
-    vh = v.view(B, L, Hkv, D).transpose(1, 2).repeat_interleave(Hq // Hkv, 1)
-    s = (qh @ kh.transpose(-1, -2) * scale).masked_fill(~vis, float("-inf"))
-    m = s.amax(-1, keepdim=True).detach()
-    m = torch.where(torch.isinf(m), torch.zeros_like(m), m)
-    e = torch.exp(s - m)
-    l = e.sum(-1, keepdim=True)
-    o = (e / torch.where(l > 0, l, torch.ones_like(l))) @ vh
-    return o.transpose(1, 2).reshape(B * L, Hq * D), (m + torch.log(l)).squeeze(-1).detach()
 
 
 ROW_PARAMS = [

@@ -6,14 +6,11 @@ import os
 import pytest
 import torch
 
+from model_helpers import (attach_lora, compare_full_grads, draw_lora_B, llama_rag_models, lora_grad_error, r16, rag_batch,
+                           rag_step_vs_oracle, rel, retriever_batch)
+
 pytestmark = pytest.mark.gpu
 bf16, f32 = torch.bfloat16, torch.float32
-
-
-def _rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return ((a - b).norm() / (b.norm() + 1e-30)).item()
-
 
 # ---------------------------------------------------------------------------------------------------------------
 # kernels
@@ -27,9 +24,9 @@ def test_gemm_nn_layout_is_dgrad_against_untransposed_weight(cuda_dev, M, N, K, 
     w = (torch.randn(K, N, generator=g) * 0.1).to(cuda_dev, bf16)          # W[out=K, in=N]: dx = dy W
     out = ops.gemm(a, w, layout=1, block_n=bn, max_ctas=max_ctas)
     ref = a.float() @ w.float()
-    assert _rel(out.float(), ref) < 5e-3
+    assert rel(out.float(), ref) < 5e-3
     out32 = ops.gemm(a, w, layout=1, out_dtype=f32, block_n=bn, max_ctas=max_ctas)
-    assert _rel(out32, ref) < 1e-4
+    assert rel(out32, ref) < 1e-4
 
 
 @pytest.mark.parametrize("T,M,N,bn,max_ctas", [(1000, 192, 320, 0, 0), (64, 128, 256, 256, 0), (3204, 264, 1096, 128, 4),
@@ -42,14 +39,14 @@ def test_gemm_wgrad_layout_contracts_over_token_rows(cuda_dev, T, M, N, bn, max_
     ref = dy.float().t() @ x.float()
     gw = torch.full((M, N), 7.0, dtype=f32, device=cuda_dev)
     ops.gemm(dy, x, out=gw, layout=2, block_n=bn, max_ctas=max_ctas)       # fresh gradient: written, not accumulated
-    assert _rel(gw, ref) < 1e-4
+    assert rel(gw, ref) < 1e-4
     ops.wgrad_(dy, x, gw, accumulate=True)                                # second contribution: +=
-    assert _rel(gw, 2 * ref) < 1e-4
+    assert rel(gw, 2 * ref) < 1e-4
     # strided views (column blocks of a fused activation buffer), as the engine passes them
     buf = torch.randn(T, M + 64, generator=g).to(cuda_dev, bf16)
     gw2 = torch.empty(M, N, dtype=f32, device=cuda_dev)
     ops.wgrad_(buf[:, :M], x, gw2, accumulate=False)
-    assert _rel(gw2, buf[:, :M].float().t() @ x.float()) < 1e-4
+    assert rel(gw2, buf[:, :M].float().t() @ x.float()) < 1e-4
 
 
 def test_col_reduce_bias_and_norm_gradients(cuda_dev):
@@ -65,14 +62,14 @@ def test_col_reduce_bias_and_norm_gradients(cuda_dev):
         zh = (z - mean[:, None]) * rstd[:, None]
         s, p = torch.zeros(H, device=cuda_dev), torch.ones(H, device=cuda_dev)
         ops.col_reduce_(dy_f32=dya, dy_bf16=dyb, z=z, mean=mean, rstd=rstd, out_sum=s, out_prod=p)
-        assert _rel(s, dy.sum(0)) < 1e-5 and _rel(p - 1, (dy * zh).sum(0)) < 1e-4
+        assert rel(s, dy.sum(0)) < 1e-5 and rel(p - 1, (dy * zh).sum(0)) < 1e-4
         # bias gradient: bf16 only; RMSNorm gain: no mean
         s2 = torch.zeros(H, device=cuda_dev)
         ops.col_reduce_(dy_bf16=dyb, out_sum=s2)
-        assert _rel(s2, dyb.float().sum(0)) < 1e-5
+        assert rel(s2, dyb.float().sum(0)) < 1e-5
         p2 = torch.zeros(H, device=cuda_dev)
         ops.col_reduce_(dy_bf16=dyb, z=z, rstd=rstd, out_prod=p2)
-        assert _rel(p2, (dyb.float() * z * rstd[:, None]).sum(0)) < 1e-4
+        assert rel(p2, (dyb.float() * z * rstd[:, None]).sum(0)) < 1e-4
 
 
 def test_embed_scatter_add_and_masked_add(cuda_dev):
@@ -86,7 +83,7 @@ def test_embed_scatter_add_and_masked_add(cuda_dev):
     rw = torch.zeros(V, H, device=cuda_dev).index_add_(0, ids.view(-1), d)
     rp = torch.zeros(32, H, device=cuda_dev)
     rp[:L] = d.view(B, L, H).sum(0)
-    assert _rel(dw, rw) < 1e-6 and _rel(dp, rp) < 1e-6
+    assert rel(dw, rw) < 1e-6 and rel(dp, rp) < 1e-6
     a = torch.randn(B * L, H, generator=g).to(cuda_dev)
     b = torch.randn(B * L, H, generator=g).to(cuda_dev, bf16)
     drop = ops.Drop(0.1, 1234, 99, None)
@@ -118,83 +115,24 @@ def test_adam_shadow_matches_torch_adam(cuda_dev):
 # ---------------------------------------------------------------------------------------------------------------
 # whole-step parity: every parameter's gradient
 # ---------------------------------------------------------------------------------------------------------------
-def _full_models(dev, vb=600, vl=504, lora_r=False, lora_g=False):
-    from dalm_b200 import synthetic
-    from dalm_b200.engine import params
-    from dalm_b200.engine.bert import BertEncoder
-    from dalm_b200.engine.llama import LlamaDecoder
-    from dalm_b200.models.rag_e2e_base_model import AutoModelForRagE2E, Mode
-    from oracle import models as om
-    bcfg, lcfg = synthetic.bert_config("bge-tiny", vb), synthetic.llama_config("llama-tiny", vl)
-    r16 = lambda sd: {k: v.to(bf16).float() for k, v in sd.items()}            # fp32 master == bf16 shadow at the start
-    bsd, lsd = r16(params.random_state_dict("bert", bcfg, seed=11)), r16(params.random_state_dict("llama", lcfg, seed=12))
-    enc = BertEncoder(bcfg, bsd, device=dev, lora=lora_r, full=not lora_r)
-    dec = LlamaDecoder(lcfg, lsd, device=dev, lora=lora_g, full=not lora_g)
-    mode = {(False, False): None, (True, False): Mode.RETRIEVER, (False, True): Mode.GENERATOR}[(lora_r, lora_g)]
-    model = AutoModelForRagE2E("", "", get_peft=mode, _retriever=enc, _generator=dec, _load_tokenizers=False)
-    return model, enc, dec, om.build_bert(bcfg, bsd), om.build_llama(lcfg, lsd)
-
-
-def _compare_full_grads(engine, ref_grads, prefix, skip=(), tol=6e-2, abs_floor=1e-7):
-    """every HF parameter of the fully fine-tuned engine model vs the oracle's autograd gradient"""
-    worst, checked = ("", 0.0), 0
-    got = {}
-    for key, parts in engine._rows.items():
-        gw, r = engine.full.g(key), 0
-        for name, rows in parts:
-            got[name] = gw[r:r + rows]
-            r += rows
-    for name, gt in got.items():
-        if name in skip:
-            continue
-        rg = ref_grads[prefix + name]
-        if rg.norm().item() < abs_floor:                    # a mathematically zero gradient (key bias: softmax is shift
-            assert gt.float().norm().item() < 1e-4, name    # invariant): ours is bf16 rounding noise, compare absolutely
-            continue
-        e = _rel(gt, rg)
-        checked += 1
-        if e > worst[1]:
-            worst = (name, e)
-    assert worst[1] < tol, worst
-    return checked
-
-
-def _batch(B, Lq, Lp, Lg, vb, vl, seed):
-    g = torch.Generator().manual_seed(seed)
-    mk = lambda L: torch.ones(B, L, dtype=torch.int64)
-    b = {"retriever_query_input_ids": torch.randint(5, vb, (B, Lq), generator=g), "retriever_query_attention_mask": mk(Lq),
-         "retriever_passage_input_ids": torch.randint(5, vb, (B, Lp), generator=g), "retriever_passage_attention_mask": mk(Lp),
-         "generator_input_input_ids": torch.randint(3, vl, (B, Lg), generator=g), "generator_input_attention_mask": mk(Lg),
-         "query_passage_input_len": torch.randint(1, Lg + 3, (B,), generator=g)}
-    b["retriever_query_attention_mask"][0, Lq - 3:] = 0
-    b["retriever_passage_attention_mask"][1, Lp // 2:] = 0
-    b["generator_input_attention_mask"][0, :5] = 0
-    return b
-
-
 def test_full_finetune_rag_step_gradients_match_oracle(cuda_dev):
     from dalm_b200.optim import FusedAdam
     from dalm_b200.training.utils.train_utils import fused_rag_step
-    from oracle import models as om
-    model, enc, dec, bert, llama = _full_models(cuda_dev)
-    batch = _batch(5, 12, 24, 40, 600, 504, seed=21)
-    ref = om.rag_step(bert, llama, batch)
+    model, enc, dec, bert, llama = llama_rag_models(cuda_dev, 504, r16, lora_r=False, lora_g=False)
+    batch = rag_batch(5, 12, 24, 40, 600, 504, seed=21)
     opt = FusedAdam(model.parameters(), lr=1e-3)
-    opt.zero_grad()
-    out = fused_rag_step(model, batch, 100.0)
-    got = out["losses"].cpu()
-    assert abs(got[2].item() - ref["loss"].item()) / abs(ref["loss"].item()) < 1e-3
-    n_r = _compare_full_grads(enc, ref["grads"], "retriever.")
-    n_g = _compare_full_grads(dec, ref["grads"], "generator.")
+    ref, out = rag_step_vs_oracle(model, enc, dec, bert, llama, batch)
+    n_r = compare_full_grads(enc, ref["grads"], "retriever.")
+    n_g = compare_full_grads(dec, ref["grads"], "generator.")
     assert n_r > 30 and n_g > 15
     # a second backward without zero_grad accumulates (un-fused API path / gradient accumulation)
     g1r, g1g = enc.full.g32.clone(), dec.full.g32.clone()
     fused_rag_step(model, batch, 100.0)
-    assert _rel(enc.full.g32, 2 * g1r) < 1e-3 and _rel(dec.full.g32, 2 * g1g) < 1e-3
+    assert rel(enc.full.g32, 2 * g1r) < 1e-3 and rel(dec.full.g32, 2 * g1g) < 1e-3
     # zero_grad + step again gives the single-step gradient back (fresh wgrads overwrite, atomics start from zero)
     opt.zero_grad()
     fused_rag_step(model, batch, 100.0)
-    assert _rel(enc.full.g32, g1r) < 1e-3 and _rel(dec.full.g32, g1g) < 1e-3
+    assert rel(enc.full.g32, g1r) < 1e-3 and rel(dec.full.g32, g1g) < 1e-3
     # Adam: master weights move like torch.optim.Adam on the oracle's gradients; the bf16 shadow follows the master
     w_before = dec.full.w32("L0.Wqkv").clone()
     opt.step()
@@ -219,8 +157,8 @@ def test_full_finetune_through_the_reference_style_autograd_loop(cuda_dev):
     from dalm_b200.optim import FusedAdam
     from dalm_b200.training.utils.train_utils import compute_marginalized_loss_from_logits, get_cosine_sim, get_nt_xent_loss
     from oracle import models as om
-    model, enc, dec, bert, llama = _full_models(cuda_dev, vl=500)          # vocab not a multiple of 8: padded lm_head rows
-    batch = _batch(4, 10, 20, 32, 600, 500, seed=31)
+    model, enc, dec, bert, llama = llama_rag_models(cuda_dev, 500, r16, lora_r=False, lora_g=False)   # vocab not a multiple of 8:
+    batch = rag_batch(4, 10, 20, 32, 600, 500, seed=31)                                                 # padded lm_head rows
     ref = om.rag_step(bert, llama, batch)
     d = {k: v.to(cuda_dev) for k, v in batch.items()}
     opt = FusedAdam(model.parameters(), lr=1e-3)
@@ -234,29 +172,18 @@ def test_full_finetune_through_the_reference_style_autograd_loop(cuda_dev):
                                                           S, d["query_passage_input_len"])
     loss.backward()
     assert abs(loss.item() - ref["loss"].item()) / abs(ref["loss"].item()) < 1e-3
-    _compare_full_grads(enc, ref["grads"], "retriever.")
-    _compare_full_grads(dec, ref["grads"], "generator.")
+    compare_full_grads(enc, ref["grads"], "retriever.")
+    compare_full_grads(dec, ref["grads"], "generator.")
 
 
 def test_mixed_peft_retriever_lora_generator_full(cuda_dev):
     """`--use-peft retriever`: adapters on the retriever, the generator fully fine-tuned (reference rag_e2e_base_model.py:61-80:
     only the named sub-model goes through get_peft_model)"""
-    from dalm_b200.training.utils.train_utils import fused_rag_step
-    from oracle import models as om
-    model, enc, dec, bert, llama = _full_models(cuda_dev, lora_r=True)
-    g = torch.Generator().manual_seed(13)
-    for n, _, _ in enc.lora.specs:
-        enc.lora.B[n].copy_((torch.randn(enc.lora.B[n].shape, generator=g) * 0.02).to(cuda_dev))
-    enc.repack_lora()
-    om.attach_lora(bert, {n: {"A": enc.lora.A[n].cpu(), "B": enc.lora.B[n].cpu()} for n, _, _ in enc.lora.specs})
-    batch = _batch(4, 10, 20, 32, 600, 504, seed=41)
-    ref = om.rag_step(bert, llama, batch)
-    enc.lora.zero_grad(); dec.full.zero_grad()
-    out = fused_rag_step(model, batch, 100.0)
-    assert abs(out["loss"].item() - ref["loss"].item()) / abs(ref["loss"].item()) < 1e-3
-    _compare_full_grads(dec, ref["grads"], "generator.")
-    worst = max(max(_rel(enc.lora.gA[n], ref["grads"]["retriever." + n + ".lora_A"]),
-                    _rel(enc.lora.gB[n], ref["grads"]["retriever." + n + ".lora_B"])) for n, _, _ in enc.lora.specs)
+    model, enc, dec, bert, llama = llama_rag_models(cuda_dev, 504, r16, lora_r=True, lora_g=False)
+    batch = rag_batch(4, 10, 20, 32, 600, 504, seed=41)
+    ref, out = rag_step_vs_oracle(model, enc, dec, bert, llama, batch)
+    compare_full_grads(dec, ref["grads"], "generator.")
+    worst = lora_grad_error(enc, ref["grads"], "retriever.")
     assert worst < 6e-2, worst
     assert len(model.trainable_banks()) == 2
 
@@ -273,9 +200,7 @@ def test_full_finetune_retriever_only_with_dropout_and_graph(cuda_dev):
     bcfg = synthetic.bert_config("bge-tiny", 600)
     enc = BertEncoder(bcfg, params.random_state_dict("bert", bcfg, seed=3), device=cuda_dev, full=True)
     se = AutoModelForSentenceEmbedding("", use_bnb=False, get_peft=False, _model=enc, _load_tokenizer=False)
-    b = _batch(6, 12, 24, 8, 600, 504, seed=51)
-    rb = {"query_input_ids": b["retriever_query_input_ids"], "query_attention_mask": b["retriever_query_attention_mask"],
-          "passage_input_ids": b["retriever_passage_input_ids"], "passage_attention_mask": b["retriever_passage_attention_mask"]}
+    rb = retriever_batch(rag_batch(6, 12, 24, 8, 600, 504, seed=51))
     se.train()
     opt = FusedAdam(se.parameters(), lr=2e-4)
     graphed = GraphedStep(fused_retriever_step, se, rb, 100.0, zero_grads=opt.zero_grad)
@@ -334,17 +259,13 @@ def test_falcon_full_finetune_with_recompute_matches_oracle(cuda_dev):
     from dalm_b200.training.utils.train_utils import GraphedStep, fused_rag_step
     from oracle import models as om
     bcfg, fcfg = synthetic.bert_config("bge-tiny", 600), synthetic.falcon_config("falcon-tiny", 504)
-    r16 = lambda sd: {k: v.to(bf16).float() for k, v in sd.items()}
     bsd, fsd = r16(params.random_state_dict("bert", bcfg, seed=21)), r16(params.random_state_dict("falcon", fcfg, seed=22))
     enc, dec = BertEncoder(bcfg, bsd, device=cuda_dev, lora=True), FalconDecoder(fcfg, fsd, device=cuda_dev, full=True)
-    g = torch.Generator().manual_seed(23)
-    for n, _, _ in enc.lora.specs:
-        enc.lora.B[n].copy_((torch.randn(enc.lora.B[n].shape, generator=g) * 0.02).to(cuda_dev))
-    enc.repack_lora()
+    draw_lora_B(enc, torch.Generator().manual_seed(23))
     model = AutoModelForRagE2E("", "", get_peft=Mode.RETRIEVER, _retriever=enc, _generator=dec, _load_tokenizers=False)
-    batch = _batch(4, 10, 20, 48, 600, 504, seed=24)
+    batch = rag_batch(4, 10, 20, 48, 600, 504, seed=24)
     bert, falcon = om.build_bert(bcfg, bsd), om.build_falcon(fcfg, fsd)
-    om.attach_lora(bert, {n: {"A": enc.lora.A[n].cpu(), "B": enc.lora.B[n].cpu()} for n, _, _ in enc.lora.specs})
+    attach_lora(bert, enc)
     ref = om.rag_step(bert, falcon, batch)
     opt = FusedAdam(model.parameters(), lr=1e-3)
     opt.zero_grad()
@@ -356,13 +277,12 @@ def test_falcon_full_finetune_with_recompute_matches_oracle(cuda_dev):
         extra = ref["grads"].get("generator.lm_head.weight")
         if name == "transformer.word_embeddings.weight" and extra is not None and extra.data_ptr() != rg.data_ptr():
             rg = rg + extra                                                        # untied in the oracle build: sum of both uses
-        e = _rel(dec.full.g(key), rg)
+        e = rel(dec.full.g(key), rg)
         checked += 1
         if e > worst[1]:
             worst = (name, e)
     assert worst[1] < 6e-2 and checked == 3 + 6 * fcfg["num_hidden_layers"], (worst, checked)
-    w = max(max(_rel(enc.lora.gA[n], ref["grads"]["retriever." + n + ".lora_A"]),
-                _rel(enc.lora.gB[n], ref["grads"]["retriever." + n + ".lora_B"])) for n, _, _ in enc.lora.specs)
+    w = lora_grad_error(enc, ref["grads"], "retriever.")
     assert w < 6e-2, w
     # training under a CUDA graph (recomputation inside the captured backward) decreases the loss
     graphed = GraphedStep(fused_rag_step, model, batch, 100.0, zero_grads=opt.zero_grad)

@@ -15,13 +15,10 @@ import math
 import pytest
 import torch
 
+from model_helpers import rel
+
 pytestmark = pytest.mark.gpu
 bf16, f32 = torch.bfloat16, torch.float32
-
-
-def _rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return ((a - b).norm() / (b.norm() + 1e-30)).item()
 
 
 def _r16(sd):
@@ -40,7 +37,7 @@ def _factors(bank):
 
 
 def _worst_lora(bank, grads, prefix):
-    return max(max(_rel(bank.gA[n], grads[prefix + n + ".lora_A"]), _rel(bank.gB[n], grads[prefix + n + ".lora_B"]))
+    return max(max(rel(bank.gA[n], grads[prefix + n + ".lora_A"]), rel(bank.gB[n], grads[prefix + n + ".lora_B"]))
                for n, _, _ in bank.specs)
 
 
@@ -88,9 +85,9 @@ def test_cfg3_step_at_full_width(cuda_dev):
     enc.lora.zero_grad(); dec.lora.zero_grad()
     out = fused_rag_step(model, batch, 100.0)
     got = out["losses"].cpu()
-    rel = lambda a, b: abs(a - b) / abs(b)
-    assert rel(got[2].item(), ref["loss"].item()) < 1e-3, (got, ref["loss"])                     # north_star tolerance
-    assert rel(got[1].item(), ref["Lm"].item()) < 1e-3
+    relerr = lambda a, b: abs(a - b) / abs(b)
+    assert relerr(got[2].item(), ref["loss"].item()) < 1e-3, (got, ref["loss"])                     # north_star tolerance
+    assert relerr(got[1].item(), ref["Lm"].item()) < 1e-3
     # Lc: cross-entropy is 1-Lipschitz in the sup norm of its logits (each direction), so |dLc| <= 2 max|dS| whatever the
     # kernel does; S = 100 * cos-sim of bf16-forward embeddings, so max|dS| is the number that carries the bf16 budget
     dS = (out["S"].cpu() - ref["S"]).abs().max().item()
@@ -100,7 +97,7 @@ def test_cfg3_step_at_full_width(cuda_dev):
     # looser bound above is the encoder's bf16 forward, not the loss kernel (VERDICT r1 weak 1: "justify 2e-2")
     cvec, nsum = ops.marginal_counts(batch["generator_input_attention_mask"].to(dev), batch["query_passage_input_len"].to(dev))
     r = ops.inbatch_loss(ref["q"].to(dev), ref["p"].to(dev), 100.0, cvec, nsum, need_grad=False)
-    assert rel(r["losses"][0].item(), ref["Lc"].item()) < 1e-5
+    assert relerr(r["losses"][0].item(), ref["Lc"].item()) < 1e-5
     assert (r["S"].cpu() - ref["S"]).abs().max().item() < 1e-3
     # gradients of every LoRA factor (bf16 activations and gradients: 6e-2 relative L2 per factor, as at toy widths)
     assert _worst_lora(enc.lora, ref["grads"], "retriever.") < 6e-2
@@ -108,7 +105,7 @@ def test_cfg3_step_at_full_width(cuda_dev):
     # logits of the real-width decoder on the valid positions
     logits, _ = dec.forward_logits(batch["generator_input_input_ids"].to(dev), batch["generator_input_attention_mask"].to(dev), save=False)
     valid = batch["generator_input_attention_mask"].bool()
-    assert _rel(logits.float().cpu()[valid], ref["logits"][valid]) < 1.5e-2
+    assert rel(logits.float().cpu()[valid], ref["logits"][valid]) < 1.5e-2
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -175,7 +172,7 @@ def test_cfg5_falcon_forward_at_full_width(cuda_dev):
     with torch.no_grad():
         ref_logits = ref(input_ids=ids, attention_mask=mask).logits
     valid = mask.bool()
-    assert _rel(logits.float().cpu()[valid], ref_logits[valid]) < 1.5e-2
+    assert rel(logits.float().cpu()[valid], ref_logits[valid]) < 1.5e-2
     S = torch.randn(B, B, generator=g) * 3
     qlen = torch.tensor([700, 2050])
     want = losses.marginalized_loss_loopform(ref_logits, ids, mask, S, qlen)
@@ -214,7 +211,7 @@ def test_cfg5_falcon_full_finetune_grads_at_full_width(cuda_dev):
     for name, p_ in ref.named_parameters():
         if name == "lm_head.weight" or p_.grad is None:                 # tied: accumulated into the embedding gradient
             continue
-        e = _rel(got[name], p_.grad)
+        e = rel(got[name], p_.grad)
         if e > worst:
             worst, worst_name = e, name
     assert worst < 6e-2, (worst, worst_name)
@@ -266,8 +263,8 @@ def test_attention_tc_cfg3_shape_vs_fp64(cuda_dev, pad):
     out, lse = ops.attention_tc_fwd(q, k, v, mask, B, L, H, H, D, True)
     dq, dk, dv = ops.attention_tc_bwd(q, k, v, mask, out, lse, d_out, B, L, H, H, D, True)
     ref, rq, rk, rv = _attn_ref64(q, k, v, mask, True, B, L, H, H, D, d_out)
-    assert _rel(out.float()[rows], ref[rows]) < 1e-2
+    assert rel(out.float()[rows], ref[rows]) < 1e-2
     assert out.float()[~rows].abs().max().item() == 0.0 if (~rows).any() else True
-    assert _rel(dq.float()[rows], rq[rows]) < 2e-2
-    assert _rel(dk.float(), rk) < 2e-2
-    assert _rel(dv.float(), rv) < 2e-2
+    assert rel(dq.float()[rows], rq[rows]) < 2e-2
+    assert rel(dk.float(), rk) < 2e-2
+    assert rel(dv.float(), rv) < 2e-2

@@ -9,9 +9,8 @@ not a CTA cap, is what makes the CTAs walk several tiles.
 import pytest
 import torch
 
-from exact_helpers import Guarded, _expect_close, _expect_equal, _poisoned, _ulp_bf16, _ulp_f32
-from test_exact_tiles_gpu import STAGES, _gelu64, _ints, _pick_block_n
-from test_qwen3_gpu import EPS, _norm_w, _ref_norm_rope, _tables
+from exact_helpers import (EPS, STAGES, Guarded, _expect_close, _expect_equal, _gelu64, _ints, _norm_w, _pick_block_n, _poisoned,
+                           _ref_norm_rope, _tables, _ulp_bf16, _ulp_f32)
 
 pytestmark = pytest.mark.gpu
 bf16, f32 = torch.bfloat16, torch.float32

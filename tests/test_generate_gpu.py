@@ -20,13 +20,10 @@ import math
 import pytest
 import torch
 
+from model_helpers import attach_lora, check_against_oracle, draw_lora_B, prompt, r16_2d, rel
+
 pytestmark = pytest.mark.gpu
 bf16, f32, i64 = torch.bfloat16, torch.float32, torch.int64
-
-
-def _rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return ((a - b).norm() / (b.norm() + 1e-30)).item()
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -51,13 +48,13 @@ def test_rope_pos(cuda_dev, D, heads):
     # untouched columns bit-exact; rotated ones within one bf16 rounding of the fp32 reference (fma contraction may differ)
     assert torch.equal(got[:, :col0], want[:, :col0]) and torch.equal(got[:, col0 + heads * D:], want[:, col0 + heads * D:])
     assert ((got.float() - want.float()).abs() <= want.float().abs() * 2 ** -7 + 1e-6).all()      # one bf16 ulp
-    assert _rel(got.float(), want.float()) < 2e-3
+    assert rel(got.float(), want.float()) < 2e-3
     # arange positions == the training kernel (position = row % L)
     L = 10
     b2 = torch.randn(3 * L, heads * D, generator=g).to(bf16).to(cuda_dev)
     a = ops.rope_(b2.clone(), 0, heads, D, cos_t[:L].contiguous(), sin_t[:L].contiguous(), L)
     p = ops.rope_pos_(b2.clone(), 0, heads, D, cos_t, sin_t, torch.arange(L, device=cuda_dev).repeat(3))
-    assert ((a.float() - p.float()).abs() <= a.float().abs() * 2 ** -7 + 1e-6).all() and _rel(p.float(), a.float()) < 2e-3
+    assert ((a.float() - p.float()).abs() <= a.float().abs() * 2 ** -7 + 1e-6).all() and rel(p.float(), a.float()) < 2e-3
 
 
 @pytest.mark.parametrize("D,Hq,Hkv,T,cur", [(128, 4, 4, 40, 17), (128, 4, 2, 300, 299), (64, 7, 1, 64, 0), (64, 2, 2, 130, 128),
@@ -87,7 +84,7 @@ def test_attention_decode(cuda_dev, D, Hq, Hkv, T, cur):
     vis = mask[:, :cur + 1].bool().clone(); vis[:, cur] = True
     s = s.masked_fill(~vis[:, None, :], float("-inf"))
     ref = torch.einsum("bht,bthd->bhd", torch.softmax(s, -1), V).reshape(B, Nq)
-    assert _rel(out.float(), ref) < 5e-3                        # bf16 output rounding
+    assert rel(out.float(), ref) < 5e-3                        # bf16 output rounding
     assert (out.float() - ref).abs().max().item() < 2e-2
     # device-column mode (what a CUDA-graph replay uses): same launch, the column comes from an int32 [B] device tensor
     ck2, cv2 = ck0.clone(), cv0.clone()
@@ -107,21 +104,21 @@ def test_decode_gemm(cuda_dev, M, N, K):
     a, w = a_buf[:, :K], w_buf[:, :K]                                          # row stride K + 64
     ref = a.float() @ w.float().t()
     out = ops.decode_gemm(a, w)
-    assert out.dtype == bf16 and _rel(out.float(), ref) < 4e-3                 # bf16 output rounding
+    assert out.dtype == bf16 and rel(out.float(), ref) < 4e-3                 # bf16 output rounding
     out32 = ops.decode_gemm(a, w, out_dtype=f32)
-    assert _rel(out32, ref) < 1e-4                                             # fp32 tensor-core accumulate over up to 11 008 terms
+    assert rel(out32, ref) < 1e-4                                             # fp32 tensor-core accumulate over up to 11 008 terms
     r32 = torch.randn(M, N, generator=g).to(cuda_dev)
-    assert _rel(ops.decode_gemm(a, w, out_dtype=f32, resid=r32), ref + r32) < 1e-4
+    assert rel(ops.decode_gemm(a, w, out_dtype=f32, resid=r32), ref + r32) < 1e-4
     r16 = r32.to(bf16)
-    assert _rel(ops.decode_gemm(a, w, out_dtype=bf16, resid=r16).float(), ref + r16.float()) < 4e-3
+    assert rel(ops.decode_gemm(a, w, out_dtype=bf16, resid=r16).float(), ref + r16.float()) < 4e-3
     gelu = torch.nn.functional.gelu(ref)
-    assert _rel(ops.decode_gemm(a, w, out_dtype=f32, act=1), gelu) < 1e-4
+    assert rel(ops.decode_gemm(a, w, out_dtype=f32, act=1), gelu) < 1e-4
     # the same numbers as the wgmma GEMM the rest of the engine uses (bf16 outputs agree to rounding)
     if M == 16:
-        assert _rel(ops.gemm(a, w).float(), out.float()) < 4e-3
+        assert rel(ops.gemm(a, w).float(), out.float()) < 4e-3
     wide = torch.zeros(M, N + 16, dtype=f32, device=cuda_dev)                  # output into a column slice
     ops.decode_gemm(a, w, out=wide[:, 8:8 + N])
-    assert _rel(wide[:, 8:8 + N], ref) < 1e-4 and (wide[:, :8] == 0).all() and (wide[:, 8 + N:] == 0).all()
+    assert rel(wide[:, 8:8 + N], ref) < 1e-4 and (wide[:, :8] == 0).all() and (wide[:, 8 + N:] == 0).all()
     with pytest.raises(_lib.DalmB200Error):
         ops.decode_gemm(torch.zeros(17, K, dtype=bf16, device=cuda_dev), w)   # more than one 16-row tile: use ops.gemm
 
@@ -172,80 +169,6 @@ def test_greedy_step(cuda_dev):
 # ----------------------------------------------------------------------------------------------------------------
 # whole decoders
 # ----------------------------------------------------------------------------------------------------------------
-def _prompt(B, L0, V, seed):
-    g = torch.Generator().manual_seed(seed)
-    ids = torch.randint(3, V, (B, L0), generator=g)
-    mask = torch.ones(B, L0, dtype=i64)
-    mask[1, :3] = 0          # left padding
-    mask[2, L0 - 3:] = 0     # right padding
-    return ids, mask
-
-
-def _check_against_oracle(dec, ref, ids, mask, T, eos, pad, monkeypatch):
-    """runs dec.generate with every step's logits recorded, then replays the emitted tokens through the oracle"""
-    from dalm_b200 import ops
-    from oracle import generate as og
-    rec = []
-    real = ops.greedy_step_
-
-    def recording(logits, V, *a, **k):
-        rec.append(logits[:, :V].float().cpu())
-        return real(logits, V, *a, **k)
-
-    from dalm_b200.engine import decoding
-    eos_list = [] if eos is None else list(eos)
-    gen = lambda: dec.generate(input_ids=ids.to(dec.dev), attention_mask=mask.to(dec.dev), max_length=T, early_stopping=True,
-                               eos_token_id=eos_list, pad_token_id=pad).cpu()       # [] = no EOS (None would mean the config's)
-    # pass 1: eager launches with every step's logits recorded (the recorder reads them back, which a graph capture cannot)
-    monkeypatch.setenv("DALM_B200_DECODE_GRAPH", "0")
-    monkeypatch.setattr(ops, "greedy_step_", recording)
-    out = gen()
-    monkeypatch.setattr(ops, "greedy_step_", real)
-    assert decoding.LAST_RUN["graph_replays"] == 0
-    # pass 2: the default launch mode — the decode step captured once as a CUDA graph and replayed; same kernels, same
-    # arguments, so the tokens must be IDENTICAL to the eager pass
-    monkeypatch.setenv("DALM_B200_DECODE_GRAPH", "1")
-    replayed = gen()
-    assert decoding.LAST_RUN["graph_replays"] >= min(4, out.shape[1] - ids.shape[1] - 2), decoding.LAST_RUN
-    assert torch.equal(replayed, out)
-    B, L0 = ids.shape
-    assert out.dtype == i64 and out.shape[0] == B and L0 < out.shape[1] <= T
-    assert torch.equal(out[:, :L0], ids)                                    # prompt passes through untouched
-    n_new = out.shape[1] - L0
-    assert len(rec) >= n_new
-    # oracle logits for every generated column, teacher-forced on OUR tokens (full re-run of the prefix, no cache)
-    am = torch.cat([mask, torch.ones(B, n_new, dtype=i64)], 1)
-    pos = (am.cumsum(-1) - 1).masked_fill(am == 0, 1)
-    with torch.no_grad():
-        want = ref(input_ids=out, attention_mask=am, position_ids=pos).logits.float()
-    finished = torch.zeros(B, dtype=torch.bool)
-    worst_rel, worst_margin = 0.0, 0.0
-    for j in range(n_new):
-        col = L0 + j
-        live = ~finished
-        w, g = want[:, col - 1], rec[j]
-        if live.any():
-            worst_rel = max(worst_rel, _rel(g[live], w[live]))
-            margin = w.max(-1).values - w.gather(1, out[:, col:col + 1]).squeeze(1)
-            worst_margin = max(worst_margin, float(margin[live].max()))
-        assert (out[finished, col] == pad).all()                             # finished rows emit the pad id
-        for e in eos_list:
-            finished |= live & (out[:, col] == e)
-    assert worst_rel < 3e-2, worst_rel
-    assert worst_margin < 0.05, worst_margin
-    if eos_list and out.shape[1] < T:
-        assert finished.all()                                                # stopped early only because every row hit EOS
-        # ... and not a step later than HF would: before the last column someone was still generating
-        f2 = torch.zeros(B, dtype=torch.bool)
-        for col in range(L0, out.shape[1] - 1):
-            for e in eos_list:
-                f2 |= out[:, col] == e
-        assert not f2.all()
-    # the oracle generating from the same prompt: identical wherever its own top-1 / top-2 gap exceeds the bf16 noise
-    mine = og.greedy_generate(ref, ids, mask, T, eos_token_ids=eos_list, pad_token_id=pad)
-    return out, mine
-
-
 @pytest.mark.parametrize("name,lora,rows_gemm", [("llama-tiny", True, "1"), ("llama-hd128", False, "1"), ("llama-hd128", True, "0")])
 def test_llama_generate(cuda_dev, monkeypatch, name, lora, rows_gemm):
     monkeypatch.setenv("DALM_B200_DECODE_GEMM", rows_gemm)                    # "0": decode-step GEMMs on the training tcgen05 kernel
@@ -255,25 +178,21 @@ def test_llama_generate(cuda_dev, monkeypatch, name, lora, rows_gemm):
     from oracle import models as om
     V = 512
     cfg = synthetic.llama_config(name, vocab_size=V)
-    sd = params.random_state_dict("llama", cfg, seed=2)
-    sd = {k: (v.to(bf16).float() if v.dim() == 2 else v) for k, v in sd.items()}
+    sd = r16_2d(params.random_state_dict("llama", cfg, seed=2))
     dec = LlamaDecoder(cfg, sd, device=cuda_dev, lora=lora)
     ref = om.build_llama(cfg, sd)
     if lora:
-        g = torch.Generator().manual_seed(9)
-        for n, _, _ in dec.lora.specs:
-            dec.lora.B[n].copy_((torch.randn(dec.lora.B[n].shape, generator=g) * 0.02).to(cuda_dev))
-        dec.repack_lora()
-        om.attach_lora(ref, {n: {"A": dec.lora.A[n].cpu(), "B": dec.lora.B[n].cpu()} for n, _, _ in dec.lora.specs})
+        draw_lora_B(dec, torch.Generator().manual_seed(9))
+        attach_lora(ref, dec)
         dec.train()                                                          # generate must not apply adapter dropout
-    ids, mask = _prompt(4, 12, V, seed=1)
+    ids, mask = prompt(4, 12, V, seed=1)
     T = 34
-    free, _ = _check_against_oracle(dec, ref, ids, mask, T, None, 0, monkeypatch)
+    free, _ = check_against_oracle(dec, ref, ids, mask, T, None, 0, monkeypatch)
     assert free.shape == (4, T)
     assert dec.training == bool(lora)
     # EOS ids taken from the free run so that rows finish at different steps (and all of them before max_length)
     eos = sorted({int(free[0, 14]), int(free[1, 20]), int(free[2, 17]), int(free[3, 23])})
-    out, _ = _check_against_oracle(dec, ref, ids, mask, T, eos, eos[0], monkeypatch)
+    out, _ = check_against_oracle(dec, ref, ids, mask, T, eos, eos[0], monkeypatch)
     assert out.shape[1] <= 25
     with pytest.raises(ValueError):
         dec.generate(input_ids=ids.to(cuda_dev), attention_mask=mask.to(cuda_dev), max_length=12)
@@ -286,12 +205,11 @@ def test_falcon_generate(cuda_dev, monkeypatch):
     from oracle import models as om
     V = 512
     cfg = synthetic.falcon_config("falcon-mini", vocab_size=V)               # 7 query heads x 64, one KV head
-    sd = params.random_state_dict("falcon", cfg, seed=3)
-    sd = {k: (v.to(bf16).float() if v.dim() == 2 else v) for k, v in sd.items()}
+    sd = r16_2d(params.random_state_dict("falcon", cfg, seed=3))
     dec = FalconDecoder(cfg, sd, device=cuda_dev)
     ref = om.build_falcon(cfg, sd)
-    ids, mask = _prompt(4, 12, V, seed=2)
-    free, _ = _check_against_oracle(dec, ref, ids, mask, 30, None, 0, monkeypatch)
+    ids, mask = prompt(4, 12, V, seed=2)
+    free, _ = check_against_oracle(dec, ref, ids, mask, 30, None, 0, monkeypatch)
     assert free.shape == (4, 30)
     eos = sorted({int(free[0, 15]), int(free[1, 18]), int(free[2, 13]), int(free[3, 21])})
-    _check_against_oracle(dec, ref, ids, mask, 30, eos, eos[0], monkeypatch)
+    check_against_oracle(dec, ref, ids, mask, 30, eos, eos[0], monkeypatch)

@@ -3,13 +3,10 @@ against the fp64 closed form of reference train_utils.py:113-138 (oracle/losses.
 import pytest
 import torch
 
+from model_helpers import llama_rag_models, r16_2d, rag_batch, rel
+
 pytestmark = pytest.mark.gpu
 bf16, f32 = torch.bfloat16, torch.float32
-
-
-def _rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return ((a - b).norm() / (b.norm() + 1e-30)).item()
 
 
 def _case(B, L, V, seed, left_pad=True):
@@ -99,8 +96,8 @@ def test_chunked_head_matches_materialised_logits(cuda_dev, M_rows, V, H, budget
     assert none is None
     for lp in (lp1, lp2, lp3):
         assert (lp - ref_lp).abs().max().item() < 1e-5
-    assert _rel(dhf1, ref_dhf) < 2e-3 and _rel(dhf2, ref_dhf) < 2e-3
-    assert _rel(dW, ref_dW) < 2e-3
+    assert rel(dhf1, ref_dhf) < 2e-3 and rel(dhf2, ref_dhf) < 2e-3
+    assert rel(dW, ref_dW) < 2e-3
     # fp64 closed form: lp[b,t] = log_softmax(hf W^T)[ids[b,t+1]], d hf = sum_v dlogits W
     x, w = hf.double(), W[:V].double()
     lg = (x @ w.t()).view(B, L, V)
@@ -116,17 +113,16 @@ def test_chunked_head_matches_materialised_logits(cuda_dev, M_rows, V, H, budget
     onehot = torch.zeros(B, L, V, dtype=torch.float64)
     onehot[:, :-1].scatter_(-1, ids[:, 1:].unsqueeze(-1), 1.0)
     dlg = coef * (lsm.exp() - onehot)
-    assert _rel(dhf1, (dlg.view(M, V) @ w)) < 3e-2
-    assert _rel(dW[:V], dlg.view(M, V).t() @ x) < 3e-2
+    assert rel(dhf1, (dlg.view(M, V) @ w)) < 3e-2
+    assert rel(dW[:V], dlg.view(M, V).t() @ x) < 3e-2
 
 
 def test_fused_step_chunked_head_equals_materialised(cuda_dev):
     """the whole fused RAG step with the chunked head == the same step through [B,L,V] logits (PEFT and full fine-tuning)"""
     from dalm_b200.engine import head
     from dalm_b200.training.utils import train_utils as tu
-    from test_step_gpu import _batch, _models
-    model, enc, dec, _, _ = _models(cuda_dev)
-    batch = _batch(5, 12, 24, 40, 600, 500, seed=23)
+    model, enc, dec, _, _ = llama_rag_models(cuda_dev, 500, r16_2d)
+    batch = rag_batch(5, 12, 24, 40, 600, 500, seed=23)
     old_budget, old_flag = head.L2_BUDGET, tu._CHUNKED_HEAD
     try:
         res = {}
@@ -137,6 +133,6 @@ def test_fused_step_chunked_head_equals_materialised(cuda_dev):
             out = tu.fused_rag_step(model, batch, 100.0)
             res[chunked] = (out["losses"].clone(), enc.lora.grad.clone(), dec.lora.grad.clone())
         assert (res[True][0] - res[False][0]).abs().max().item() < 1e-5
-        assert _rel(res[True][1], res[False][1]) < 1e-4 and _rel(res[True][2], res[False][2]) < 2e-3
+        assert rel(res[True][1], res[False][1]) < 1e-4 and rel(res[True][2], res[False][2]) < 2e-3
     finally:
         head.L2_BUDGET, tu._CHUNKED_HEAD = old_budget, old_flag

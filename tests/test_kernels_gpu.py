@@ -5,14 +5,11 @@ import math
 import pytest
 import torch
 
+from model_helpers import rel
+
 pytestmark = pytest.mark.gpu
 
 bf16, f32 = torch.bfloat16, torch.float32
-
-
-def _rel(a, b):
-    a, b = a.double(), b.double()
-    return ((a - b).norm() / (b.norm() + 1e-30)).item()
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -34,7 +31,7 @@ def test_gemm_plain(cuda_dev, M, N, K, bn):
     out = ops.gemm(a, b, block_n=bn)
     ref = a.float() @ b.float().t()
     # bf16 output rounding: rel 2^-9 per element; accumulate order differs only in fp32
-    assert _rel(out.float(), ref) < 4e-3
+    assert rel(out.float(), ref) < 4e-3
     assert torch.isfinite(out.float()).all()
 
 
@@ -49,7 +46,7 @@ def test_gemm_multi_tile_per_cta(cuda_dev):
     for bn in (64, 128, 256, 2128, 2256):
         for ctas in (2, 3, 7):
             out = ops.gemm(a, b, block_n=bn, max_ctas=ctas, out_dtype=f32)
-            assert _rel(out, ref) < 1e-5, (bn, ctas)
+            assert rel(out, ref) < 1e-5, (bn, ctas)
 
 
 def test_gemm_epilogues(cuda_dev):
@@ -63,21 +60,21 @@ def test_gemm_epilogues(cuda_dev):
     r16 = torch.randn(M, N, device=cuda_dev).to(bf16)
     acc = a.float() @ b.float().t()
     out = ops.gemm(a, b, out_dtype=f32, bias=bias, resid=r32, alpha=0.5)
-    assert _rel(out, 0.5 * acc + bias + r32) < 1e-5
+    assert rel(out, 0.5 * acc + bias + r32) < 1e-5
     out = ops.gemm(a, b, out_dtype=f32, bias=bias, act=1)
-    assert _rel(out, torch.nn.functional.gelu(acc + bias)) < 1e-5
+    assert rel(out, torch.nn.functional.gelu(acc + bias)) < 1e-5
     out = ops.gemm(a, b, out_dtype=bf16, resid=r16)
-    assert _rel(out.float(), acc + r16.float()) < 4e-3
+    assert rel(out.float(), acc + r16.float()) < 4e-3
     for bn in (2128, 2256):                                   # same epilogue through the CTA-pair kernel
         out = ops.gemm(a, b, out_dtype=f32, bias=bias, resid=r32, alpha=0.5, block_n=bn)
-        assert _rel(out, 0.5 * acc + bias + r32) < 1e-5
+        assert rel(out, 0.5 * acc + bias + r32) < 1e-5
         out = ops.gemm(a, b, out_dtype=f32, bias=bias, act=1, block_n=bn)
-        assert _rel(out, torch.nn.functional.gelu(acc + bias)) < 1e-5
+        assert rel(out, torch.nn.functional.gelu(acc + bias)) < 1e-5
     # strided views: A and output are column slices of wider buffers (the LoRA K-augmentation layout)
     wide_a = torch.zeros(M, K + 24, device=cuda_dev, dtype=bf16); wide_a[:, :K] = a
     wide_o = torch.zeros(M, N + 40, device=cuda_dev, dtype=bf16)
     ops.gemm(wide_a[:, :K], b, out=wide_o[:, 40:])
-    assert _rel(wide_o[:, 40:].float(), acc) < 4e-3
+    assert rel(wide_o[:, 40:].float(), acc) < 4e-3
     assert wide_o[:, :40].abs().max().item() == 0
 
 
@@ -136,7 +133,7 @@ def test_attention_fwd_bwd(cuda_dev, B, L, Hq, Hkv, D, causal, pad):
         valid = mask.bool()                   # fully-masked (left pad) query rows: compared separately below
     vrows = valid.view(-1)
     # bf16 P and bf16 output: ~1e-2 relative on the tile
-    assert _rel(out.float()[vrows], ref[vrows]) < 1.5e-2
+    assert rel(out.float()[vrows], ref[vrows]) < 1.5e-2
     if causal and pad == "left":
         assert out.float()[~vrows].abs().max().item() == 0.0      # fully masked rows produce zeros
     d_out = torch.randn(B * L, Hq * D, device=dev).to(bf16)
@@ -144,9 +141,9 @@ def test_attention_fwd_bwd(cuda_dev, B, L, Hq, Hkv, D, causal, pad):
     d_out_eff[~vrows] = 0
     ref.backward(d_out_eff.double())
     dq, dk, dv = ops.attention_bwd(q, k, v, mask, out, lse, d_out_eff, B, L, Hq, Hkv, D, causal)
-    assert _rel(dq.float(), qd.grad) < 3e-2
-    assert _rel(dk.float(), kd.grad) < 3e-2
-    assert _rel(dv.float(), vd.grad) < 3e-2
+    assert rel(dq.float(), qd.grad) < 3e-2
+    assert rel(dk.float(), kd.grad) < 3e-2
+    assert rel(dv.float(), vd.grad) < 3e-2
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -163,14 +160,14 @@ def test_layernorm_fwd_bwd(cuda_dev, M, H):
     y32, y16, mean, rstd = ops.layernorm_fwd(z, g, b, 1e-12)
     zd = z.double().requires_grad_(True)
     ref = torch.nn.functional.layer_norm(zd, (H,), g.double(), b.double(), 1e-12)
-    assert _rel(y32, ref) < 1e-5
-    assert _rel(y16.float(), ref) < 4e-3
+    assert rel(y32, ref) < 1e-5
+    assert rel(y16.float(), ref) < 4e-3
     dy_a = torch.randn(M, H, device=cuda_dev)
     dy_b = torch.randn(M, H, device=cuda_dev).to(bf16)
     ref.backward(dy_a.double() + dy_b.double())
     dz32, dz16 = ops.layernorm_bwd(z, g, mean, rstd, dy_f32=dy_a, dy_bf16=dy_b)
-    assert _rel(dz32, zd.grad) < 1e-4
-    assert _rel(dz16.float(), zd.grad) < 4e-3
+    assert rel(dz32, zd.grad) < 1e-4
+    assert rel(dz16.float(), zd.grad) < 4e-3
     # pre-LN form (Falcon): the residual's gradient is added to both outputs, in place
     dres = torch.randn(M, H, device=cuda_dev)
     want = zd.grad + dres.double()
@@ -179,8 +176,8 @@ def test_layernorm_fwd_bwd(cuda_dev, M, H):
     # (dy_bf16-only variant: recompute the reference for that input)
     zd2 = z.double().requires_grad_(True)
     torch.nn.functional.layer_norm(zd2, (H,), g.double(), b.double(), 1e-12).backward(dy_b.double())
-    assert _rel(dz32r, zd2.grad + (want - zd.grad)) < 1e-4 and dz32r.data_ptr() == dres.data_ptr()
-    assert _rel(dz16r.float(), zd2.grad + (want - zd.grad)) < 4e-3
+    assert rel(dz32r, zd2.grad + (want - zd.grad)) < 1e-4 and dz32r.data_ptr() == dres.data_ptr()
+    assert rel(dz16r.float(), zd2.grad + (want - zd.grad)) < 4e-3
 
 
 def test_rmsnorm_fwd_bwd(cuda_dev):
@@ -192,13 +189,13 @@ def test_rmsnorm_fwd_bwd(cuda_dev):
     h, rstd = ops.rmsnorm_fwd(x, g, 1e-5)
     xd = x.double().requires_grad_(True)
     ref = xd * torch.rsqrt(xd.pow(2).mean(-1, keepdim=True) + 1e-5) * g.double()
-    assert _rel(h.float(), ref) < 4e-3
+    assert rel(h.float(), ref) < 4e-3
     dh = torch.randn(M, H, device=cuda_dev).to(bf16)
     dres = torch.randn(M, H, device=cuda_dev)
     ref.backward(dh.double())
     out32, out16 = ops.rmsnorm_bwd(x, g, rstd, dh, dres_in=dres)
-    assert _rel(out32, xd.grad + dres.double()) < 1e-5
-    assert _rel(out16.float(), xd.grad + dres.double()) < 4e-3
+    assert rel(out32, xd.grad + dres.double()) < 1e-5
+    assert rel(out16.float(), xd.grad + dres.double()) < 4e-3
 
 
 def test_embeddings_rope_swiglu_gelu(cuda_dev):
@@ -227,33 +224,33 @@ def test_embeddings_rope_swiglu_gelu(cuda_dev):
     tail = buf[:, nh * D:].clone()
     work = buf.clone()
     ops.rope_(work, 0, nh, D, cos_t, sin_t, L)
-    assert _rel(work[:, :nh * D].float(), ref) < 4e-3
+    assert rel(work[:, :nh * D].float(), ref) < 4e-3
     assert torch.equal(work[:, nh * D:], tail)
     ops.rope_(work, 0, nh, D, cos_t, sin_t, L, backward=True)          # inverse rotation restores the input
-    assert _rel(work[:, :nh * D].float(), buf[:, :nh * D].float()) < 8e-3
+    assert rel(work[:, :nh * D].float(), buf[:, :nh * D].float()) < 8e-3
     # swiglu
     M, F = 50, 264
     gu = torch.randn(M, 2 * F, device=dev).to(bf16)
     act = ops.swiglu_fwd(gu, F)
     gd = gu.double().requires_grad_(True)
     ref = torch.nn.functional.silu(gd[:, :F]) * gd[:, F:]
-    assert _rel(act.float(), ref) < 4e-3
+    assert rel(act.float(), ref) < 4e-3
     dact = torch.randn(M, F, device=dev).to(bf16)
     ref.backward(dact.double())
     g2 = gu.clone()
     ops.swiglu_bwd_(g2, dact, F)
-    assert _rel(g2.float(), gd.grad) < 4e-3
+    assert rel(g2.float(), gd.grad) < 4e-3
     # gelu
     pre = torch.randn(M, F, device=dev).to(bf16)
     a = ops.gelu_fwd(pre)
     pd = pre.double().requires_grad_(True)
     ref = torch.nn.functional.gelu(pd)
-    assert _rel(a.float(), ref) < 4e-3
+    assert rel(a.float(), ref) < 4e-3
     d = torch.randn(M, F, device=dev).to(bf16)
     ref.backward(d.double())
     d2 = d.clone()
     ops.gelu_bwd_(pre, d2)
-    assert _rel(d2.float(), pd.grad) < 4e-3
+    assert rel(d2.float(), pd.grad) < 4e-3
 
 
 @pytest.mark.parametrize("B,L,H", [(5, 23, 384), (18, 128, 1024), (150, 50, 1024), (3, 7, 72), (2, 300, 4096)])
@@ -269,13 +266,13 @@ def test_pool_norm(cuda_dev, B, L, H):
     emb, norm = ops.pool_norm_fwd(hid, mask, True)
     hd = hid.double().cpu().requires_grad_(True)
     ref = pooling.normalize(pooling.mean_pooling(hd, mask.cpu()).double())
-    assert _rel(emb.cpu(), ref) < 1e-5
+    assert rel(emb.cpu(), ref) < 1e-5
     d = torch.randn(B, H, device=cuda_dev)
     ref.backward(d.double().cpu())
     dh = ops.pool_norm_bwd(emb, norm, d, mask, L, True)
-    assert _rel(dh.cpu(), hd.grad) < 1e-5
+    assert rel(dh.cpu(), hd.grad) < 1e-5
     emb2, _ = ops.pool_norm_fwd(hid, mask, False)
-    assert _rel(emb2.cpu(), pooling.mean_pooling(hid.cpu(), mask.cpu())) < 1e-5
+    assert rel(emb2.cpu(), pooling.mean_pooling(hid.cpu(), mask.cpu())) < 1e-5
 
 
 def test_lora_wgrad_pack_adam(cuda_dev):
@@ -288,16 +285,16 @@ def test_lora_wgrad_pack_adam(cuda_dev):
         out = torch.zeros(8, K, device=dev)
         ops.lora_wgrad_(x[:, :K], g[:, 16:], out, K, 1, K, 8, 2.0)
         ref = 2.0 * g[:, 16:24].double().t() @ x[:, :K].double()
-        assert _rel(out, ref) < 1e-5, (M, K)
+        assert rel(out, ref) < 1e-5, (M, K)
         outT = torch.zeros(K, 8, device=dev)
         ops.lora_wgrad_(x[:, :K], g[:, 16:], outT, 1, 8, K, 8, 2.0)
         ops.lora_wgrad_(x[:, :K], g[:, 16:], outT, 1, 8, K, 8, 2.0)          # accumulates
-        assert _rel(outT, 2 * ref.t()) < 1e-5
+        assert rel(outT, 2 * ref.t()) < 1e-5
         # two adapters sharing X: rows 0-7 -> out0, rows 8-15 -> out1
         o0 = torch.zeros(8, K, device=dev); o1 = torch.zeros(8, K, device=dev)
         ops.lora_wgrad_(x[:, :K], g[:, 8:], o0, K, 1, K, 16, 1.0, out1=o1)
-        assert _rel(o0, g[:, 8:16].double().t() @ x[:, :K].double()) < 1e-5
-        assert _rel(o1, g[:, 16:24].double().t() @ x[:, :K].double()) < 1e-5
+        assert rel(o0, g[:, 8:16].double().t() @ x[:, :K].double()) < 1e-5
+        assert rel(o1, g[:, 16:24].double().t() @ x[:, :K].double()) < 1e-5
     # skinny GEMM: out[M,R] = X W^T written into the tail columns of a wider buffer
     for (M, K, R) in ((4608, 4096, 16), (900, 1024, 24), (33, 72, 8), (300, 512, 32)):
         buf = torch.zeros(M, K + 64, device=dev, dtype=bf16)
@@ -305,7 +302,7 @@ def test_lora_wgrad_pack_adam(cuda_dev):
         w = (torch.randn(64, K, device=dev) * 0.5).to(bf16)
         ops.skinny_gemm(buf[:, :K], w, buf[:, K:], K=K, R=R)
         ref = buf[:, :K].double() @ w[:R].double().t()
-        assert _rel(buf[:, K:K + R].float(), ref) < 4e-3, (M, K, R)
+        assert rel(buf[:, K:K + R].float(), ref) < 4e-3, (M, K, R)
         assert buf[:, K + R:].abs().max().item() == 0
     K, R = 520, 8
     # pack

@@ -16,20 +16,14 @@ import math
 import pytest
 import torch
 
-from exact_helpers import Guarded, _expect_close, _poisoned
-from test_exact_tiles_gpu import _attn_fns, _attn_ref64, _row_mask, dev, ops  # noqa: F401  (module fixtures)
-from test_mistral_gpu import _attn_bwd64
+from exact_helpers import Guarded, _attn_bwd64, _attn_fns, _attn_ref64, _expect_close, _poisoned, _row_mask, dev, ops  # noqa: F401
+from model_helpers import attach_lora, draw_lora_B, lora_grad_error, r16, rel
 
 pytestmark = pytest.mark.gpu
 bf16, f32, f64, i64 = torch.bfloat16, torch.float32, torch.float64, torch.int64
 PAD = 50283
 QK_SCALE, V_SCALE = 8.0, 4.0
 TOL = 1.5e-2                    # relative error of the last hidden state on valid rows (bf16 GEMM operands, fp32 residual)
-
-
-def _rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return ((a - b).norm() / (b.norm() + 1e-30)).item()
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -134,11 +128,11 @@ def test_bidirectional_wg_agrees_with_mma(ops, dev, D, L, window):
     mask = _row_mask(3, L, "right64", torch.Generator().manual_seed(3)).to(dev)
     a = _run(ops, dev, "wg", D, 3, L, 2, mask, window, seed=5)
     b = _run(ops, dev, "mma", D, 3, L, 2, mask, window, seed=5)
-    assert _rel(a[1].view.float(), b[1].view.float()) < 1e-2
+    assert rel(a[1].view.float(), b[1].view.float()) < 1e-2
     fin = torch.isfinite(b[2])
     assert torch.equal(fin, torch.isfinite(a[2])) and (a[2][fin] - b[2][fin]).abs().max() < 1e-4
     for i in (3, 4, 5):
-        assert _rel(a[i].view.float(), b[i].view.float()) < 2e-2
+        assert rel(a[i].view.float(), b[i].view.float()) < 2e-2
 
 
 def test_bidirectional_window_argument_checks(ops, dev):
@@ -197,10 +191,6 @@ def test_geglu_fwd_bwd_vs_fp64(cuda_dev, M, F, pad):
 # ----------------------------------------------------------------------------------------------------------------
 # 3. encoder against transformers
 # ----------------------------------------------------------------------------------------------------------------
-def _r16(sd):
-    return {k: v.to(bf16).float() for k, v in sd.items()}
-
-
 def _state(cfg, seed):
     from dalm_b200.engine import params
     sd = params.random_state_dict("modernbert", cfg, seed=seed)
@@ -211,17 +201,7 @@ def _state(cfg, seed):
             sd[k][2 * H:] *= V_SCALE
         if k.endswith("attn.Wo.weight"):
             sd[k] *= V_SCALE
-    return _r16(sd)
-
-
-def _hf(cfg, sd, device="cpu"):
-    from transformers import ModernBertConfig, ModernBertModel
-    c = ModernBertConfig(**{k: v for k, v in cfg.items() if k not in ("architectures", "model_type")},
-                         _attn_implementation="eager")
-    m = ModernBertModel(c)
-    missing, unexpected = m.load_state_dict(sd, strict=False)
-    assert not missing and not unexpected, (missing, unexpected)
-    return m.float().eval().to(device)
+    return r16(sd)
 
 
 def _padded(B, L, seed, pad="right"):
@@ -250,14 +230,15 @@ def _encoder(cuda_dev, name, seed, full=False, cfg_extra=None):
                                           ("modernbert-hd64", 3, 150, "right"), ("modernbert-hd64", 3, 150, "left"),
                                           ("modernbert-hd64", 1, 8192, "right")])
 def test_encoder_forward_matches_transformers(cuda_dev, name, B, L, pad):
+    from oracle import models as om
     cfg, sd, enc = _encoder(cuda_dev, name, seed=7)
     ids, mask = _padded(B, L, seed=L, pad=pad)
     hid, _ = enc.forward_hidden(ids.to(cuda_dev), mask.to(cuda_dev), save=False)
     assert torch.isfinite(hid).all()
     with torch.no_grad():
-        ref = _hf(cfg, sd, cuda_dev)(ids.to(cuda_dev), mask.to(cuda_dev))[0]
+        ref = om.build_modernbert(cfg, sd).to(cuda_dev)(ids.to(cuda_dev), mask.to(cuda_dev))[0]
     valid = mask.bool().to(cuda_dev)
-    err = _rel(hid[valid], ref[valid])
+    err = rel(hid[valid], ref[valid])
     assert err < TOL, err
     if L > 1000:
         return
@@ -265,7 +246,7 @@ def test_encoder_forward_matches_transformers(cuda_dev, name, B, L, pad):
     _, _, ctl = _encoder(cuda_dev, name, seed=7, cfg_extra={"layer_types": ["full_attention"] * cfg["num_hidden_layers"]})
     assert ctl.windows == [0] * cfg["num_hidden_layers"]
     hc, _ = ctl.forward_hidden(ids.to(cuda_dev), mask.to(cuda_dev), save=False)
-    assert _rel(hc[valid], ref[valid]) > 10 * TOL
+    assert rel(hc[valid], ref[valid]) > 10 * TOL
 
 
 def test_full_finetune_every_gradient_pad_row_and_round_trip(cuda_dev, tmp_path):
@@ -283,7 +264,7 @@ def test_full_finetune_every_gradient_pad_row_and_round_trip(cuda_dev, tmp_path)
     q, qm = _padded(6, 20, seed=1, pad="right")
     p, pm = _padded(6, 48, seed=2, pad="left")
     rb = {"query_input_ids": q, "query_attention_mask": qm, "passage_input_ids": p, "passage_attention_mask": pm}
-    want = om.retriever_step(_hf(cfg, sd), rb)
+    want = om.retriever_step(om.build_modernbert(cfg, sd), rb)
     opt = FusedAdam(se.parameters(), lr=1e-3)
     opt.zero_grad()
     out = fused_retriever_step(se, rb, 100.0)
@@ -291,7 +272,7 @@ def test_full_finetune_every_gradient_pad_row_and_round_trip(cuda_dev, tmp_path)
     worst, n = ("", 0.0), 0
     for key, name in enc._names.items():
         rg = want["grads"]["retriever." + name]
-        worst = max(worst, (name, _rel(enc.full.g(key), rg)), key=lambda t: t[1])
+        worst = max(worst, (name, rel(enc.full.g(key), rg)), key=lambda t: t[1])
         n += 1
     assert n == len(sd) and worst[1] < 6e-2, worst
     gt = enc.full.g("tok")
@@ -310,7 +291,7 @@ def test_full_finetune_every_gradient_pad_row_and_round_trip(cuda_dev, tmp_path)
     with torch.no_grad():
         e_ref = se(p, pm)
         e_hf = pooling.normalize(pooling.mean_pooling(m(p.to(cuda_dev), pm.to(cuda_dev))[0].cpu(), pm))
-    assert _rel(e_ref, e_hf) < TOL
+    assert rel(e_ref, e_hf) < TOL
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -334,7 +315,7 @@ def test_retriever_only_step_under_cuda_graph_equals_eager(cuda_dev):
         enc.zero_grad_buffers()
         got = graphed(b)["loss"].item()
         assert abs(got - loss) <= 1e-6 * abs(loss), (got, loss)
-        assert _rel(enc.full.grad, grad) < 1e-5
+        assert rel(enc.full.grad, grad) < 1e-5
 
 
 def test_fused_rag_step_modernbert_retriever_llama_generator(cuda_dev):
@@ -347,15 +328,13 @@ def test_fused_rag_step_modernbert_retriever_llama_generator(cuda_dev):
     from oracle import models as om
     cfg, sd, enc = _encoder(cuda_dev, "modernbert-tiny", seed=11, full=True)
     lcfg = synthetic.llama_config("llama-tiny", 500)
-    lsd = _r16(params.random_state_dict("llama", lcfg, seed=12))
+    lsd = r16(params.random_state_dict("llama", lcfg, seed=12))
     dec = LlamaDecoder(lcfg, lsd, device=cuda_dev, lora=True)
     g = torch.Generator().manual_seed(13)
-    for n, _, _ in dec.lora.specs:
-        dec.lora.B[n].copy_((torch.randn(dec.lora.B[n].shape, generator=g) * 0.02).to(cuda_dev))
-    dec.repack_lora()
+    draw_lora_B(dec, g)
     model = AutoModelForRagE2E("", "", get_peft=Mode.GENERATOR, _retriever=enc, _generator=dec, _load_tokenizers=False)
-    bert, llama = _hf(cfg, sd), om.build_llama(lcfg, lsd)
-    om.attach_lora(llama, {n: {"A": dec.lora.A[n].cpu(), "B": dec.lora.B[n].cpu()} for n, _, _ in dec.lora.specs})
+    bert, llama = om.build_modernbert(cfg, sd), om.build_llama(lcfg, lsd)
+    attach_lora(llama, dec)
     q, qm = _padded(5, 20, seed=21, pad="right")
     p, pm = _padded(5, 40, seed=22, pad="left")
     Lg = 40
@@ -369,10 +348,9 @@ def test_fused_rag_step_modernbert_retriever_llama_generator(cuda_dev):
     got = fused_rag_step(model, batch, 100.0)["losses"].cpu()
     assert abs(got[2].item() - ref["loss"].item()) / abs(ref["loss"].item()) < 1e-3
     assert abs(got[0].item() - ref["Lc"].item()) / abs(ref["Lc"].item()) < 2e-2
-    worst = max(_rel(enc.full.g(key), ref["grads"]["retriever." + name]) for key, name in enc._names.items())
+    worst = max(rel(enc.full.g(key), ref["grads"]["retriever." + name]) for key, name in enc._names.items())
     assert worst < 6e-2, worst
-    worst = max(max(_rel(dec.lora.gA[n], ref["grads"]["generator." + n + ".lora_A"]),
-                    _rel(dec.lora.gB[n], ref["grads"]["generator." + n + ".lora_B"])) for n, _, _ in dec.lora.specs)
+    worst = lora_grad_error(dec, ref["grads"], "generator.")
     assert worst < 6e-2, worst
 
 

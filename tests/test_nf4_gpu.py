@@ -4,6 +4,8 @@ import numpy as np
 import pytest
 import torch
 
+from model_helpers import draw_lora_B, rag_batch
+
 pytestmark = pytest.mark.gpu
 
 
@@ -119,12 +121,11 @@ def test_nf4_storage_mode_equals_resident_mode(cuda_dev, monkeypatch):
     from dalm_b200.engine.llama import LlamaDecoder
     from dalm_b200.models.rag_e2e_base_model import AutoModelForRagE2E, Mode
     from dalm_b200.training.utils.train_utils import fused_rag_step
-    from test_step_gpu import _batch
     dev = cuda_dev
     bcfg, lcfg = synthetic.bert_config("bge-tiny", 600), synthetic.llama_config("llama-mini", 500)
     bsd = params.random_state_dict("bert", bcfg, seed=11)
     lsd = params.random_state_dict("llama", lcfg, seed=12)
-    batch = _batch(4, 12, 24, 40, 600, 500, seed=21)
+    batch = rag_batch(4, 12, 24, 40, 600, 500, seed=21)
     res = []
     for storage in (False, True):
         if storage:
@@ -135,10 +136,7 @@ def test_nf4_storage_mode_equals_resident_mode(cuda_dev, monkeypatch):
             enc = BertEncoder(bcfg, params.bnb_nf4_state_dict(bsd, dev), device=dev, lora=True)
             dec = LlamaDecoder(lcfg, params.bnb_nf4_state_dict(lsd, dev), device=dev, lora=True)
         g = torch.Generator().manual_seed(13)
-        for bank in (enc.lora, dec.lora):
-            for n, _, _ in bank.specs:
-                bank.B[n].copy_((torch.randn(bank.B[n].shape, generator=g) * 0.02).to(dev))
-        enc.repack_lora(); dec.repack_lora()
+        draw_lora_B(enc, g); draw_lora_B(dec, g)
         model = AutoModelForRagE2E("", "", get_peft=Mode.BOTH, _retriever=enc, _generator=dec, _load_tokenizers=False)
         enc.lora.zero_grad(); dec.lora.zero_grad()
         out = fused_rag_step(model, batch, 100.0)

@@ -9,35 +9,12 @@ import os
 import pytest
 import torch
 
-from exact_helpers import _expect_equal, _poisoned
+from exact_helpers import _dense_poisoned, _expect_equal, _poisoned
+from model_helpers import attach_lora, check_rag_lora_grads, compare_full_grads, draw_lora_B, hf_grads, lora_grad_error, r16, rel
 
 pytestmark = pytest.mark.gpu
 bf16, f32, f64 = torch.bfloat16, torch.float32, torch.float64
 PAD = 1                                   # pad_token_id of every published XLM-R / RoBERTa checkpoint
-
-
-def _rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return ((a - b).norm() / (b.norm() + 1e-30)).item()
-
-
-def _r16(sd):
-    """every value bf16-representable: the engine's bf16 weights and fp32 masters start equal to the oracle's fp32 weights"""
-    return {k: v.to(bf16).float() for k, v in sd.items()}
-
-
-def _hf(cfg, sd):
-    """transformers' XLMRobertaModel / RobertaModel (eager attention) holding sd"""
-    import transformers
-    conf, model = (("RobertaConfig", "RobertaModel") if cfg["model_type"] == "roberta" else
-                   ("XLMRobertaConfig", "XLMRobertaModel"))
-    c = getattr(transformers, conf)(**{k: v for k, v in cfg.items() if k not in ("architectures", "model_type")},
-                                    _attn_implementation="eager")
-    m = getattr(transformers, model)(c)
-    missing, unexpected = m.load_state_dict({k: v.float() for k, v in sd.items()}, strict=False)
-    assert not [k for k in missing if "position_ids" not in k and "token_type_ids" not in k], missing
-    assert not unexpected, unexpected
-    return m.float().eval()
 
 
 def _encoder(dev, name="xlmr-tiny", V=700, seed=1, lora_B=True, **kw):
@@ -46,18 +23,11 @@ def _encoder(dev, name="xlmr-tiny", V=700, seed=1, lora_B=True, **kw):
     from dalm_b200.engine.bert import BertEncoder
     cfg = synthetic.roberta_config(name, V)
     cfg.update(kw.pop("cfg", {}))
-    sd = _r16(params.random_state_dict("roberta", cfg, seed=seed))
+    sd = r16(params.random_state_dict("roberta", cfg, seed=seed))
     enc = BertEncoder(cfg, sd, device=dev, **kw)
-    if enc.lora is not None and lora_B:                  # non-zero B: the LoRA path shows in the forward and dA is non-trivial
-        g = torch.Generator().manual_seed(seed + 4)
-        for n, _, _ in enc.lora.specs:
-            enc.lora.B[n].copy_((torch.randn(enc.lora.B[n].shape, generator=g) * 0.02).to(dev))
-        enc.repack_lora()
+    if enc.lora is not None and lora_B:
+        draw_lora_B(enc, torch.Generator().manual_seed(seed + 4))
     return cfg, sd, enc
-
-
-def _factors(enc):
-    return {n: {"A": enc.lora.A[n].cpu(), "B": enc.lora.B[n].cpu()} for n, _, _ in enc.lora.specs}
 
 
 def _padded(B, L, V, seed, pad="right"):
@@ -120,7 +90,6 @@ def test_roberta_embed_positions_and_sum(cuda_dev, B, L, P, case):
     word = torch.randint(-100, 101, (V, H), generator=g, device=dev).to(bf16)
     pos = torch.randint(-100, 101, (P, H), generator=g, device=dev).to(bf16)
     typ = torch.randint(-100, 101, (H,), generator=g, device=dev).to(bf16)
-    from test_rowwise_exact_gpu import _dense_poisoned
     want_pos = _hf_positions(ids).clamp(0, P - 1).to(dev)
     zg, pg = _DenseGuarded(B * L * H, f32, dev), _DenseGuarded(B * L, torch.int64, dev)
     z, p = ops.roberta_embed(ids.to(dev), _dense_poisoned(word), _dense_poisoned(pos), _poisoned(typ), PAD,
@@ -145,7 +114,6 @@ def test_scatter_with_positions_and_padding_idx(cuda_dev):
     whose id is not pad (word table) and the positions that are not pad (position table); row pad of either table is left
     as it was. pos_ids=None, pad_id=-1 gives the bits of the call without them."""
     from dalm_b200 import ops
-    from test_rowwise_exact_gpu import _dense_poisoned
     dev, B, L, V, H, P = cuda_dev, 6, 24, 200, 132, 40
     ids = torch.cat([_padded(3, L, V, seed=7, pad=p)[0] for p in ("right", "left")]).to(dev)
     ids[0, 5], ids[1, 3:6] = PAD, torch.tensor([-1, V, 0], device=dev)
@@ -181,26 +149,25 @@ def _fwd_bwd_check(dev, name, B, L, pad, cfg_extra=None):
     from oracle import models as om, pooling
     V = 700
     cfg, sd, enc = _encoder(dev, name, V, lora=True, cfg=cfg_extra or {})
-    ref = _hf(cfg, sd)
-    om.attach_lora(ref, _factors(enc))
+    ref = om.build_roberta(cfg, sd)
+    attach_lora(ref, enc)
     ids, mask = _padded(B, L, V, seed=B * L, pad=pad)
     hid, ctx = enc.forward_hidden(ids.to(dev), mask.to(dev))
     ref_hid = ref(ids, mask)[0]
     valid = mask.bool()
-    e = _rel(hid.cpu()[valid], ref_hid[valid])
+    e = rel(hid.cpu()[valid], ref_hid[valid])
     assert e < 1e-2, e                                    # bf16 GEMM operands through N layers (test_engine_gpu's budget)
     with torch.no_grad():                                 # control: BERT's column positions (m % L) are far off
         col = ref(ids, mask, position_ids=torch.arange(L).expand(B, L))[0]
-    assert _rel(hid.cpu()[valid], col[valid]) > 10 * 1e-2
+    assert rel(hid.cpu()[valid], col[valid]) > 10 * 1e-2
     emb, norm = ops.pool_norm_fwd(hid, mask.to(dev), True)
     ref_emb = pooling.normalize(pooling.mean_pooling(ref_hid, mask))
-    assert _rel(emb, ref_emb) < 5e-3
+    assert rel(emb, ref_emb) < 5e-3
     d_emb = torch.randn(B, cfg["hidden_size"], generator=torch.Generator().manual_seed(9))
     ref_emb.backward(d_emb)
     enc.lora.zero_grad()
     enc.backward_hidden(ctx, ops.pool_norm_bwd(emb, norm, d_emb.to(dev), mask.to(dev), L, True))
-    worst = max(max(_rel(enc.lora.gA[n], om._get_module(ref, n).lora_A.grad), _rel(enc.lora.gB[n], om._get_module(ref, n).lora_B.grad))
-                for n, _, _ in enc.lora.specs)
+    worst = lora_grad_error(enc, hf_grads(ref))
     assert worst < 5e-2, worst                            # bf16 activations / gradients (test_engine_gpu's budget)
 
 
@@ -213,25 +180,6 @@ def test_encoder_fwd_bwd_lora(cuda_dev, name, B, L, pad):
 def test_encoder_fwd_bwd_lora_long_passages(cuda_dev):
     """Lp 2048 on a 2050-row position table: the whole usable length"""
     _fwd_bwd_check(cuda_dev, "xlmr-hd64", 2, 2048, "right", cfg_extra=dict(max_position_embeddings=2050))
-
-
-def _compare_full_grads(engine, ref_grads, prefix, tol=6e-2, abs_floor=1e-7):
-    worst, checked, got = ("", 0.0), 0, {}
-    for key, parts in engine._rows.items():
-        gw, r = engine.full.g(key), 0
-        for name, rows in parts:
-            got[name] = gw[r:r + rows]
-            r += rows
-    for name, gt in got.items():
-        rg = ref_grads[prefix + name]
-        if rg.norm().item() < abs_floor:                  # mathematically zero (key bias): ours is rounding noise
-            assert gt.float().norm().item() < 1e-4, name
-            continue
-        e = _rel(gt, rg)
-        checked += 1
-        worst = max(worst, (name, e), key=lambda t: t[1])
-    assert worst[1] < tol, worst
-    return checked
 
 
 def _rbatch(B, Lq, Lp, V, seed):
@@ -250,14 +198,14 @@ def test_full_finetune_every_gradient_padding_rows_and_round_trip(cuda_dev, tmp_
     from oracle import models as om
     cfg, sd, enc = _encoder(cuda_dev, "xlmr-tiny", 600, full=True)
     se = AutoModelForSentenceEmbedding("", use_bnb=False, get_peft=False, _model=enc, _load_tokenizer=False)
-    ref = _hf(cfg, sd)
+    ref = om.build_roberta(cfg, sd)
     rb = _rbatch(6, 12, 24, 600, seed=51)
     want = om.retriever_step(ref, rb)
     opt = FusedAdam(se.parameters(), lr=1e-3)
     opt.zero_grad()
     out = fused_retriever_step(se, rb, 100.0)
     assert abs(out["loss"].item() - want["loss"].item()) / abs(want["loss"].item()) < 2e-2
-    assert _compare_full_grads(enc, want["grads"], "retriever.") > 30
+    assert compare_full_grads(enc, want["grads"], "retriever.") > 30
     gw, gp = enc.full.g("word"), enc.full.g("pos")
     assert torch.count_nonzero(gw[PAD]) == 0 and torch.count_nonzero(gp[PAD]) == 0
     assert torch.count_nonzero(want["grads"]["retriever.embeddings.word_embeddings.weight"][PAD]) == 0
@@ -295,8 +243,8 @@ def test_encoder_train_mode_matches_hf_with_replayed_masks(cuda_dev, monkeypatch
     for l in range(enc.nl):
         lm = sc(enc.p_lora, l, 3, (B, L, H))
         queue += [lm, lm, lm, sc(enc.p_attn, l, 8, (B, nh, L, Lp))[..., :L], sc(enc.p_hidden, l, 1, (B, L, H)), sc(enc.p_hidden, l, 2, (B, L, H))]
-    ref = _hf(cfg, sd)
-    om.attach_lora(ref, _factors(enc), dropout=0.05)
+    ref = om.build_roberta(cfg, sd)
+    attach_lora(ref, enc, dropout=0.05)
     ref.train()
     used = []
 
@@ -312,15 +260,14 @@ def test_encoder_train_mode_matches_hf_with_replayed_masks(cuda_dev, monkeypatch
     ref_hid = ref(ids, mask)[0]
     assert len(used) == len(queue)
     valid = mask.bool()
-    assert _rel(hid.cpu()[valid], ref_hid[valid]) < 1.2e-2
+    assert rel(hid.cpu()[valid], ref_hid[valid]) < 1.2e-2
     emb, norm = ops.pool_norm_fwd(hid, mask.to(cuda_dev), True)
     ref_emb = pooling.normalize(pooling.mean_pooling(ref_hid, mask))
     d_emb = torch.randn(B, H, generator=torch.Generator().manual_seed(6))
     ref_emb.backward(d_emb)
     enc.lora.zero_grad()
     enc.backward_hidden(ctx, ops.pool_norm_bwd(emb, norm, d_emb.to(cuda_dev), mask.to(cuda_dev), L, True))
-    worst = max(max(_rel(enc.lora.gA[n], om._get_module(ref, n).lora_A.grad), _rel(enc.lora.gB[n], om._get_module(ref, n).lora_B.grad))
-                for n, _, _ in enc.lora.specs)
+    worst = lora_grad_error(enc, hf_grads(ref))
     assert worst < 6e-2, worst
 
 
@@ -334,19 +281,16 @@ def test_fused_rag_step_xlmr_retriever_llama_generator(cuda_dev):
     from dalm_b200.models.rag_e2e_base_model import AutoModelForRagE2E, Mode
     from dalm_b200.training.utils.train_utils import fused_rag_step
     from oracle import models as om
-    from test_step_gpu import _check_grads
     cfg, sd, enc = _encoder(cuda_dev, "xlmr-tiny", 600, seed=11, lora=True)
     lcfg = synthetic.llama_config("llama-tiny", 500)
-    lsd = _r16(params.random_state_dict("llama", lcfg, seed=12))
+    lsd = r16(params.random_state_dict("llama", lcfg, seed=12))
     dec = LlamaDecoder(lcfg, lsd, device=cuda_dev, lora=True)
     g = torch.Generator().manual_seed(13)
-    for n, _, _ in dec.lora.specs:
-        dec.lora.B[n].copy_((torch.randn(dec.lora.B[n].shape, generator=g) * 0.02).to(cuda_dev))
-    dec.repack_lora()
+    draw_lora_B(dec, g)
     model = AutoModelForRagE2E("", "", get_peft=Mode.BOTH, _retriever=enc, _generator=dec, _load_tokenizers=False)
-    bert, llama = _hf(cfg, sd), om.build_llama(lcfg, lsd)
-    om.attach_lora(bert, _factors(enc))
-    om.attach_lora(llama, _factors(dec))
+    bert, llama = om.build_roberta(cfg, sd), om.build_llama(lcfg, lsd)
+    attach_lora(bert, enc)
+    attach_lora(llama, dec)
     rb = _rbatch(5, 12, 24, 600, seed=21)
     Lg = 40
     batch = {"retriever_query_input_ids": rb["query_input_ids"], "retriever_query_attention_mask": rb["query_attention_mask"],
@@ -360,7 +304,7 @@ def test_fused_rag_step_xlmr_retriever_llama_generator(cuda_dev):
     got = fused_rag_step(model, batch, 100.0)["losses"].cpu()
     assert abs(got[2].item() - ref["loss"].item()) / abs(ref["loss"].item()) < 1e-3
     assert abs(got[0].item() - ref["Lc"].item()) / abs(ref["Lc"].item()) < 2e-2
-    _check_grads(enc, dec, ref)
+    check_rag_lora_grads(enc, dec, ref)
 
 
 def test_retriever_only_step_under_cuda_graph_equals_eager(cuda_dev):
@@ -378,8 +322,8 @@ def test_retriever_only_step_under_cuda_graph_equals_eager(cuda_dev):
         enc.lora.zero_grad()
         out = fused_retriever_step(se, b, 100.0)
         eager.append((out["loss"].item(), enc.lora.grad.clone()))
-    ref = _hf(cfg, sd)
-    om.attach_lora(ref, _factors(enc))
+    ref = om.build_roberta(cfg, sd)
+    attach_lora(ref, enc)
     want = om.retriever_step(ref, b2)
     assert abs(eager[1][0] - want["loss"].item()) / abs(want["loss"].item()) < 2e-2
     graphed = GraphedStep(fused_retriever_step, se, b1, 100.0, zero_grads=enc.lora.zero_grad)
@@ -387,7 +331,7 @@ def test_retriever_only_step_under_cuda_graph_equals_eager(cuda_dev):
         enc.lora.zero_grad()
         got = graphed(b)["loss"].item()
         assert abs(got - loss) <= 1e-6 * abs(loss), (got, loss)
-        assert _rel(enc.lora.grad, grad) < 1e-5
+        assert rel(enc.lora.grad, grad) < 1e-5
 
 
 def test_use_bnb_storage_equals_resident(cuda_dev, tmp_path, monkeypatch):
@@ -410,7 +354,7 @@ def test_use_bnb_storage_equals_resident(cuda_dev, tmp_path, monkeypatch):
     l_res = fused_retriever_step(m_res, batch, 100.0)["loss"].item()
     l_st = fused_retriever_step(m_st, batch, 100.0)["loss"].item()
     assert abs(l_res - l_st) < 1e-5 * max(1.0, abs(l_res))
-    assert _rel(m_st.model.lora.grad, m_res.model.lora.grad) < 2e-2 and m_st.model.lora.grad.abs().max().item() > 0
+    assert rel(m_st.model.lora.grad, m_res.model.lora.grad) < 2e-2 and m_st.model.lora.grad.abs().max().item() > 0
 
 
 # ----------------------------------------------------------------------------------------------------------------

@@ -19,7 +19,7 @@ import numpy as np
 import pytest
 import torch
 
-from exact_helpers import PAD_R, Guarded, _expect_close, _expect_equal, _poisoned, _ulp_bf16
+from exact_helpers import PAD_R, Guarded, _dense_poisoned, _expect_close, _expect_equal, _poisoned, _ulp_bf16
 
 pytestmark = pytest.mark.gpu
 bf16, f32, f64 = torch.bfloat16, torch.float32, torch.float64
@@ -37,14 +37,6 @@ def ops(cuda_dev):
 def Err(cuda_dev):
     from dalm_b200._lib import DalmB200Error
     return DalmB200Error
-
-
-def _dense_poisoned(x: torch.Tensor) -> torch.Tensor:
-    """x [r, c] as dense rows (row stride c, the layout the fp32 row kernels index) followed by 128 NaN rows"""
-    r, c = x.shape
-    buf = torch.full(((r + PAD_R) * c,), float("nan"), dtype=x.dtype, device=x.device)
-    buf[: r * c] = x.reshape(-1)
-    return buf[: r * c].view(r, c)
 
 
 def _v(x):

@@ -7,77 +7,21 @@ import os
 import pytest
 import torch
 
+from model_helpers import (attach_lora, check_autoregressive_retriever, check_rag_lora_grads, draw_lora_B, lora_grad_error,
+                           llama_rag_models, r16_2d, rag_batch, rag_step_vs_oracle, rel, retriever_batch)
+
 pytestmark = pytest.mark.gpu
-bf16 = torch.bfloat16
-
-
-def _rel(a, b):
-    a, b = a.double().cpu(), b.double().cpu()
-    return ((a - b).norm() / (b.norm() + 1e-30)).item()
-
-
-def _models(dev, bert_name="bge-tiny", llama_name="llama-tiny", vb=600, vl=500):
-    from dalm_b200 import synthetic
-    from dalm_b200.engine import params
-    from dalm_b200.engine.bert import BertEncoder
-    from dalm_b200.engine.llama import LlamaDecoder
-    from dalm_b200.models.rag_e2e_base_model import AutoModelForRagE2E, Mode
-    from oracle import models as om
-    bcfg, lcfg = synthetic.bert_config(bert_name, vb), synthetic.llama_config(llama_name, vl)
-    r16 = lambda sd: {k: (v.to(bf16).float() if v.dim() == 2 else v) for k, v in sd.items()}
-    bsd, lsd = r16(params.random_state_dict("bert", bcfg, seed=11)), r16(params.random_state_dict("llama", lcfg, seed=12))
-    enc, dec = BertEncoder(bcfg, bsd, device=dev, lora=True), LlamaDecoder(lcfg, lsd, device=dev, lora=True)
-    g = torch.Generator().manual_seed(13)
-    for bank in (enc.lora, dec.lora):
-        for n, _, _ in bank.specs:
-            bank.B[n].copy_((torch.randn(bank.B[n].shape, generator=g) * 0.02).to(dev))
-    enc.repack_lora(); dec.repack_lora()
-    model = AutoModelForRagE2E("", "", get_peft=Mode.BOTH, _retriever=enc, _generator=dec, _load_tokenizers=False)
-    bert, llama = om.build_bert(bcfg, bsd), om.build_llama(lcfg, lsd)
-    om.attach_lora(bert, {n: {"A": enc.lora.A[n].cpu(), "B": enc.lora.B[n].cpu()} for n, _, _ in enc.lora.specs})
-    om.attach_lora(llama, {n: {"A": dec.lora.A[n].cpu(), "B": dec.lora.B[n].cpu()} for n, _, _ in dec.lora.specs})
-    return model, enc, dec, bert, llama
-
-
-def _batch(B, Lq, Lp, Lg, vb, vl, seed, pad="left"):
-    g = torch.Generator().manual_seed(seed)
-    mk = lambda L: torch.ones(B, L, dtype=torch.int64)
-    b = {"retriever_query_input_ids": torch.randint(5, vb, (B, Lq), generator=g), "retriever_query_attention_mask": mk(Lq),
-         "retriever_passage_input_ids": torch.randint(5, vb, (B, Lp), generator=g), "retriever_passage_attention_mask": mk(Lp),
-         "generator_input_input_ids": torch.randint(3, vl, (B, Lg), generator=g), "generator_input_attention_mask": mk(Lg),
-         "query_passage_input_len": torch.randint(1, Lg + 3, (B,), generator=g)}
-    b["retriever_query_attention_mask"][0, Lq - 3:] = 0
-    b["retriever_passage_attention_mask"][1, Lp // 2:] = 0
-    if pad == "left":
-        b["generator_input_attention_mask"][0, :5] = 0
-    else:
-        b["generator_input_attention_mask"][0, Lg - 5:] = 0
-    return b
-
-
-def _check_grads(enc, dec, ref, tol=6e-2):
-    from oracle import models as om
-    worst = 0.0
-    for bank, pre in ((enc.lora, "retriever."), (dec.lora, "generator.")):
-        for n, _, _ in bank.specs:
-            worst = max(worst, _rel(bank.gA[n], ref["grads"][pre + n + ".lora_A"]), _rel(bank.gB[n], ref["grads"][pre + n + ".lora_B"]))
-    assert worst < tol, worst
 
 
 @pytest.mark.parametrize("pad", ["left", "right"])
 def test_fused_rag_step_matches_oracle(cuda_dev, pad):
-    from dalm_b200.training.utils.train_utils import fused_rag_step
-    from oracle import models as om
-    model, enc, dec, bert, llama = _models(cuda_dev)
-    batch = _batch(5, 12, 24, 40, 600, 500, seed=21, pad=pad)
-    ref = om.rag_step(bert, llama, batch)
-    enc.lora.zero_grad(); dec.lora.zero_grad()
-    out = fused_rag_step(model, batch, 100.0)
+    model, enc, dec, bert, llama = llama_rag_models(cuda_dev, 500, r16_2d)
+    batch = rag_batch(5, 12, 24, 40, 600, 500, seed=21, pad=pad)
+    ref, out = rag_step_vs_oracle(model, enc, dec, bert, llama, batch)                        # total loss: north_star 1e-3
     got = out["losses"].cpu()
-    assert abs(got[2].item() - ref["loss"].item()) / abs(ref["loss"].item()) < 1e-3          # north_star tolerance
     assert abs(got[0].item() - ref["Lc"].item()) / abs(ref["Lc"].item()) < 2e-2               # bf16 embeddings x logit_scale 100
     assert abs(got[1].item() - ref["Lm"].item()) / abs(ref["Lm"].item()) < 1e-3
-    _check_grads(enc, dec, ref)
+    check_rag_lora_grads(enc, dec, ref)
 
 
 def test_reference_style_loop_body_over_the_dropin_api(cuda_dev):
@@ -86,8 +30,8 @@ def test_reference_style_loop_body_over_the_dropin_api(cuda_dev):
     from dalm_b200.training.utils.train_utils import (compute_marginalized_loss_from_logits, fused_rag_step,
                                                       get_cosine_sim, get_nt_xent_loss)
     from oracle import models as om
-    model, enc, dec, bert, llama = _models(cuda_dev)
-    batch = _batch(4, 10, 20, 32, 600, 500, seed=31)
+    model, enc, dec, bert, llama = llama_rag_models(cuda_dev, 500, r16_2d)
+    batch = rag_batch(4, 10, 20, 32, 600, 500, seed=31)
     ref = om.rag_step(bert, llama, batch)
     dbatch = {k: v.to(cuda_dev) for k, v in batch.items()}
     optimizer = FusedAdam(model.parameters(), lr=1e-3)
@@ -103,12 +47,12 @@ def test_reference_style_loop_body_over_the_dropin_api(cuda_dev):
     loss = loss_c + loss_m
     loss.backward()
     assert abs(loss.item() - ref["loss"].item()) / abs(ref["loss"].item()) < 1e-3
-    _check_grads(enc, dec, ref)
+    check_rag_lora_grads(enc, dec, ref)
     # same gradients as the fused launch sequence
     g_auto = [enc.lora.grad.clone(), dec.lora.grad.clone()]
     optimizer.zero_grad()
     fused_rag_step(model, batch, 100.0)
-    assert _rel(enc.lora.grad, g_auto[0]) < 1e-2 and _rel(dec.lora.grad, g_auto[1]) < 1e-2
+    assert rel(enc.lora.grad, g_auto[0]) < 1e-2 and rel(dec.lora.grad, g_auto[1]) < 1e-2
     before = dec.lora.flat.clone()
     optimizer.step(); model.repack()
     assert (dec.lora.flat - before).abs().max().item() > 0
@@ -119,11 +63,9 @@ def test_retriever_only_step_and_stepwise_training(cuda_dev):
     from dalm_b200.optim import FusedAdam
     from dalm_b200.training.utils.train_utils import fused_retriever_step
     from oracle import models as om
-    model, enc, dec, bert, llama = _models(cuda_dev)
+    model, enc, dec, bert, llama = llama_rag_models(cuda_dev, 500, r16_2d)
     se = AutoModelForSentenceEmbedding("", use_bnb=False, get_peft=True, _model=enc, _load_tokenizer=False)
-    b = _batch(6, 12, 24, 8, 600, 500, seed=41)
-    rb = {"query_input_ids": b["retriever_query_input_ids"], "query_attention_mask": b["retriever_query_attention_mask"],
-          "passage_input_ids": b["retriever_passage_input_ids"], "passage_attention_mask": b["retriever_passage_attention_mask"]}
+    rb = retriever_batch(rag_batch(6, 12, 24, 8, 600, 500, seed=41))
     ref = om.retriever_step(bert, rb)
     enc.lora.zero_grad()
     out = fused_retriever_step(se, rb, 100.0)
@@ -181,27 +123,20 @@ def test_fused_step_with_frozen_falcon_generator(cuda_dev):
     from dalm_b200.training.utils.train_utils import fused_rag_step
     from oracle import models as om
     bcfg, fcfg = synthetic.bert_config("bge-tiny", 600), synthetic.falcon_config("falcon-tiny", 504)
-    r16 = lambda sd: {k: (v.to(bf16).float() if v.dim() == 2 else v) for k, v in sd.items()}
-    bsd, fsd = r16(params.random_state_dict("bert", bcfg, seed=21)), r16(params.random_state_dict("falcon", fcfg, seed=22))
+    bsd, fsd = r16_2d(params.random_state_dict("bert", bcfg, seed=21)), r16_2d(params.random_state_dict("falcon", fcfg, seed=22))
     enc, dec = BertEncoder(bcfg, bsd, device=cuda_dev, lora=True), FalconDecoder(fcfg, fsd, device=cuda_dev)
-    g = torch.Generator().manual_seed(23)
-    for n, _, _ in enc.lora.specs:
-        enc.lora.B[n].copy_((torch.randn(enc.lora.B[n].shape, generator=g) * 0.02).to(cuda_dev))
-    enc.repack_lora()
+    draw_lora_B(enc, torch.Generator().manual_seed(23))
     model = AutoModelForRagE2E("", "", get_peft=Mode.RETRIEVER, _retriever=enc, _generator=dec, _load_tokenizers=False)
-    batch = _batch(4, 10, 20, 48, 600, 504, seed=24)
+    batch = rag_batch(4, 10, 20, 48, 600, 504, seed=24)
     bert, falcon = om.build_bert(bcfg, bsd), om.build_falcon(fcfg, fsd)
-    om.attach_lora(bert, {n: {"A": enc.lora.A[n].cpu(), "B": enc.lora.B[n].cpu()} for n, _, _ in enc.lora.specs})
+    attach_lora(bert, enc)
     for p_ in falcon.parameters():
         p_.requires_grad_(False)
     ref = om.rag_step(bert, falcon, batch)
     enc.lora.zero_grad()
     out = fused_rag_step(model, batch, 100.0)
     assert abs(out["loss"].item() - ref["loss"].item()) / abs(ref["loss"].item()) < 1e-3
-    worst = 0.0
-    for n, _, _ in enc.lora.specs:
-        worst = max(worst, _rel(enc.lora.gA[n], ref["grads"]["retriever." + n + ".lora_A"]),
-                    _rel(enc.lora.gB[n], ref["grads"]["retriever." + n + ".lora_B"]))
+    worst = lora_grad_error(enc, ref["grads"], "retriever.")
     assert worst < 6e-2, worst
 
 
@@ -211,45 +146,25 @@ def test_autoregressive_retriever(cuda_dev):
     from dalm_b200 import synthetic
     from dalm_b200.engine import params
     from dalm_b200.engine.llama import LlamaDecoder
-    from dalm_b200.models.retriever_only_base_model import AutoModelForSentenceEmbedding
-    from dalm_b200.training.utils.train_utils import fused_retriever_step, get_cosine_sim, get_nt_xent_loss
-    from oracle import models as om, losses
+    from dalm_b200.training.utils.train_utils import get_cosine_sim, get_nt_xent_loss
+    from oracle import models as om
     cfg = synthetic.llama_config("llama-tiny", 400)
-    sd = {k: (v.to(bf16).float() if v.dim() == 2 else v) for k, v in params.random_state_dict("llama", cfg, seed=31).items()}
+    sd = r16_2d(params.random_state_dict("llama", cfg, seed=31))
     enc = LlamaDecoder(cfg, sd, device=cuda_dev, lora=True, lora_seed=0)
     g = torch.Generator().manual_seed(32)
-    for n, _, _ in enc.lora.specs:
-        enc.lora.B[n].copy_((torch.randn(enc.lora.B[n].shape, generator=g) * 0.02).to(cuda_dev))
-    enc.repack_lora()
-    model = AutoModelForSentenceEmbedding("", use_bnb=False, get_peft=True, is_autoregressive=True, _model=enc, _load_tokenizer=False)
+    draw_lora_B(enc, g)
     ref = om.build_llama(cfg, sd)
-    om.attach_lora(ref, {n: {"A": enc.lora.A[n].cpu(), "B": enc.lora.B[n].cpu()} for n, _, _ in enc.lora.specs})
-    B, Lq, Lp = 4, 12, 20
-    mk = lambda L: torch.ones(B, L, dtype=torch.int64)
-    rb = {"query_input_ids": torch.randint(3, 400, (B, Lq), generator=g), "query_attention_mask": mk(Lq),
-          "passage_input_ids": torch.randint(3, 400, (B, Lp), generator=g), "passage_attention_mask": mk(Lp)}
-    rb["query_attention_mask"][0, :3] = 0; rb["passage_attention_mask"][2, :6] = 0          # left padding (tokenizer default)
-    q = om.retrieval_forward_autoregressive(ref, rb["query_input_ids"], rb["query_attention_mask"])
-    p = om.retrieval_forward_autoregressive(ref, rb["passage_input_ids"], rb["passage_attention_mask"])
-    loss = losses.contrastive_loss(losses.get_cosine_sim(q, p, 100.0))
-    loss.backward()
-    enc.lora.zero_grad()
-    out = fused_retriever_step(model, rb, 100.0)
-    assert abs(out["loss"].item() - loss.item()) / abs(loss.item()) < 2e-2
-    worst = 0.0
-    for n, _, _ in enc.lora.specs:
-        mod = om._get_module(ref, n)
-        worst = max(worst, _rel(enc.lora.gA[n], mod.lora_A.grad), _rel(enc.lora.gB[n], mod.lora_B.grad))
-    assert worst < 8e-2, worst
+    attach_lora(ref, enc)
+    model, rb, q = check_autoregressive_retriever(enc, ref, g, 400, 12, 20)
     # the wrapper's own forward (autograd bridge) gives the same embeddings and gradients
     g_fused = enc.lora.grad.clone()
     enc.lora.zero_grad()
     dq = {k: v.to(cuda_dev) for k, v in rb.items()}
     qe = model(dq["query_input_ids"], dq["query_attention_mask"]); pe = model(dq["passage_input_ids"], dq["passage_attention_mask"])
-    assert _rel(qe, q.detach()) < 2e-2
+    assert rel(qe, q.detach()) < 2e-2
     S = get_cosine_sim(qe, pe, 100)
     ((get_nt_xent_loss(S) + get_nt_xent_loss(S.t())) / 2.0).backward()
-    assert _rel(enc.lora.grad, g_fused) < 2e-2
+    assert rel(enc.lora.grad, g_fused) < 2e-2
 
 
 def test_packed_loader_trains_like_the_reference_pipeline(cuda_dev, tmp_path, monkeypatch):

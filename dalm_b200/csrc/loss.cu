@@ -78,6 +78,9 @@ __global__ void __launch_bounds__(256) inbatch_loss_kernel(InbatchParams p) {
   cg::grid_group grid = cg::this_grid();
 
   // ---- phase 1: S[i,:] for the rows this CTA owns (one warp per (i,j) dot product, float4 coalesced) ----
+  // float4 loads of P need D % 4 == 0 and a 16-byte aligned P (a contiguous view may start anywhere); Q is staged through
+  // shared memory with scalar loads. Uniform over the grid.
+  const bool vec_p = (D & 3) == 0 && (reinterpret_cast<uintptr_t>(p.P) & 15) == 0;
   for (int i = blockIdx.x; i < B; i += gridDim.x) {
     __syncthreads();
     for (int d = tid; d < D; d += blockDim.x) qrow[d] = p.Q[(size_t)i * D + d];
@@ -85,7 +88,7 @@ __global__ void __launch_bounds__(256) inbatch_loss_kernel(InbatchParams p) {
     for (int j = wid; j < B; j += nwarp) {
       const float* prow = p.P + (size_t)j * D;
       float acc = 0.f;
-      if ((D & 3) == 0) {
+      if (vec_p) {
         const float4* p4 = reinterpret_cast<const float4*>(prow);
         const float4* q4 = reinterpret_cast<const float4*>(qrow);
         for (int d = lane; d < (D >> 2); d += 32) {
@@ -219,6 +222,11 @@ __global__ void __launch_bounds__(512) ce_rows_kernel(CeParams p) {
   const T* x = reinterpret_cast<const T*>(p.logits) + (size_t)blockIdx.x * p.ldl;
   T* dx = p.dlogits ? reinterpret_cast<T*>(p.dlogits) + (size_t)blockIdx.x * p.ldl : nullptr;
   const int V = p.V, tid = threadIdx.x, nt = blockDim.x;
+  // 16-byte loads / stores need whole vectors per row and 16-byte aligned rows: ldl, V and both base pointers (a view such
+  // as logits[..., 1:] keeps a padded ldl but starts mid-vector). Uniform over the grid.
+  constexpr int VEC = 16 / sizeof(T);
+  const bool vec_ok = (p.ldl % VEC) == 0 && (V % VEC) == 0 &&
+                      ((reinterpret_cast<uintptr_t>(p.logits) | reinterpret_cast<uintptr_t>(p.dlogits)) & 15) == 0;
 
   float w = 0.f;
   int64_t label = -1;
@@ -231,8 +239,7 @@ __global__ void __launch_bounds__(512) ce_rows_kernel(CeParams p) {
   if (w == 0.f) {
     if (tid == 0) p.tok_lp[row] = 0.f;
     if (dx) {
-      constexpr int VEC = 16 / sizeof(T);
-      if ((p.ldl % VEC) == 0 && (V % VEC) == 0) {
+      if (vec_ok) {
         uint4 z = make_uint4(0, 0, 0, 0);
         uint4* d4 = reinterpret_cast<uint4*>(dx);
         for (int i = tid; i < V / VEC; i += nt) d4[i] = z;
@@ -243,8 +250,6 @@ __global__ void __launch_bounds__(512) ce_rows_kernel(CeParams p) {
     return;
   }
 
-  constexpr int VEC = 16 / sizeof(T);
-  const bool vec_ok = ((p.ldl % VEC) == 0) && ((V % VEC) == 0);
   const bool cache = p.cache_in_smem != 0;
 
   // ---- pass 1: stream the row (HBM -> smem), running max ----

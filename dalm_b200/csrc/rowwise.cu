@@ -1055,6 +1055,13 @@ extern "C" int dalm_b200_pool_norm_fwd(const float* hidden, const int64_t* mask,
 extern "C" int dalm_b200_pool_norm_bwd(const float* emb, const float* norm, const float* d_emb, const int64_t* mask,
                                        float* d_hidden, int B, int L, int H, int normalize, void* stream) {
   DALM_REQUIRE(H * 4 <= 48 * 1024, "pool_norm_bwd: H too large");
+  // d_pooled takes H * 4 bytes of dynamic shared memory next to the kernel's static `red`: at H = 12288 the sum passes the
+  // 48 KB a launch gets without opting in
+  static bool attr_set = false;
+  if (!attr_set) {
+    DALM_CUDA(cudaFuncSetAttribute(pool_norm_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 48 * 1024));
+    attr_set = true;
+  }
   pool_norm_bwd_kernel<<<B, 256, H * sizeof(float), ST(stream)>>>(emb, norm, d_emb, mask, d_hidden, L, H, normalize);
   count_launch();
   return check_launch("pool_norm_bwd_kernel");

@@ -46,6 +46,27 @@ def _rows32(t: Optional[torch.Tensor], name: str, H: int, M: Optional[int] = Non
         raise _lib.DalmB200Error(f"{name}: expected dense fp32 rows {want}, got shape {tuple(t.shape)} strides {t.stride()}")
 
 
+def _vec(t: Optional[torch.Tensor], dtype, name: str, n: int) -> None:
+    """a vector the kernels index as t[0 .. n): anything shorter (or strided) would be read past its end"""
+    if t is None:
+        return
+    _chk(t, dtype, name)
+    if t.numel() != n or not t.is_contiguous():
+        raise _lib.DalmB200Error(f"{name}: expected {n} contiguous {dtype} values, got shape {tuple(t.shape)} strides {t.stride()}")
+
+
+def _bf16_rows(t: torch.Tensor, name: str, rows: int, cols: int) -> None:
+    """bf16 2-D view with contiguous rows and at least [rows, cols] elements (the kernels read rows x cols at its row stride)"""
+    _chk(t, bf16, name)
+    if t.dim() != 2 or t.shape[0] < rows or t.shape[1] < cols:
+        raise _lib.DalmB200Error(f"{name}: expected a bf16 view of at least [{rows}, {cols}], got shape {tuple(t.shape)}")
+
+
+def _reach(t: torch.Tensor) -> int:
+    """largest element offset a (non-negatively strided) view covers"""
+    return sum((s - 1) * st for s, st in zip(t.shape, t.stride()))
+
+
 def _tables16(*named) -> None:
     """bf16 embedding tables, which the gathers index as dense rows (id * H)"""
     for name, t in named:
@@ -81,6 +102,7 @@ def marginal_counts(gen_mask: torch.Tensor, qlen: torch.Tensor) -> Tuple[torch.T
     _chk(gen_mask, i64, "gen_mask"); _chk(qlen, i64, "qlen")
     gen_mask = gen_mask.contiguous(); qlen = qlen.contiguous()
     B, L = gen_mask.shape
+    _vec(qlen, i64, "marginal_counts qlen", B)
     cvec = torch.empty(B, dtype=f32, device=gen_mask.device)
     nsum = torch.empty(1, dtype=f32, device=gen_mask.device)
     _lib.call("dalm_b200_marginal_counts", _p(gen_mask), _p(qlen), B, L, _p(cvec), _p(nsum), _stream())
@@ -95,6 +117,9 @@ def inbatch_loss(q: torch.Tensor, p: torch.Tensor, logit_scale: float, cvec: Opt
     B, D = q.shape
     if p.shape != q.shape:
         raise _lib.DalmB200Error(f"inbatch_loss: q {tuple(q.shape)} and p {tuple(p.shape)} must match (in-batch negatives)")
+    if (cvec is None) != (nsum is None):
+        raise _lib.DalmB200Error("inbatch_loss: cvec and nsum go together")
+    _vec(cvec, f32, "inbatch_loss cvec", B); _vec(nsum, f32, "inbatch_loss nsum", 1)
     dev = q.device
     S = torch.empty(B, B, dtype=f32, device=dev)
     dlp = torch.empty(B, dtype=f32, device=dev)
@@ -113,6 +138,9 @@ def ce_marginal(logits: torch.Tensor, ids: torch.Tensor, mask: torch.Tensor, nsu
         raise _lib.DalmB200Error(f"ce_marginal: logits dtype {logits.dtype} unsupported")
     _chk(logits, logits.dtype, "logits"); _chk(ids, i64, "ids"); _chk(mask, i64, "mask")
     B, L, V = logits.shape
+    if ids.shape != (B, L) or mask.shape != (B, L):
+        raise _lib.DalmB200Error(f"ce_marginal: ids {tuple(ids.shape)} / mask {tuple(mask.shape)} must be [{B}, {L}] like the logits")
+    _vec(nsum, f32, "ce_marginal nsum", 1)
     # rows may be padded (row stride ld >= V, e.g. a vocabulary rounded up to the GEMM's N granularity)
     rows_ok = logits.stride(2) == 1 and logits.stride(0) == L * logits.stride(1) and logits.stride(1) >= V
     if not rows_ok:
@@ -145,6 +173,12 @@ def ce_marginal_rows_(chunk: torch.Tensor, ids: torch.Tensor, mask: torch.Tensor
     if chunk.dim() != 2 or not ids.is_contiguous() or not mask.is_contiguous() or not tok_lp.is_contiguous():
         raise _lib.DalmB200Error("ce_marginal_rows: chunk must be 2-D, ids / mask / tok_lp contiguous")
     B, L = ids.shape
+    if mask.shape != (B, L) or tok_lp.shape != (B, L):
+        raise _lib.DalmB200Error(f"ce_marginal_rows: mask {tuple(mask.shape)} / tok_lp {tuple(tok_lp.shape)} must be [{B}, {L}] "
+                                 "like ids")
+    if chunk.shape[1] < V:
+        raise _lib.DalmB200Error(f"ce_marginal_rows: chunk {tuple(chunk.shape)} narrower than the vocabulary ({V})")
+    _vec(nsum, f32, "ce_marginal_rows nsum", 1)
     _lib.call("dalm_b200_ce_marginal_rows", _p(chunk), _p(chunk) if need_grad else None, 0 if chunk.dtype == bf16 else 1, _p(ids),
               _p(mask), _p(nsum), _p(tok_lp), B, L, int(V), chunk.stride(0), float(grad_out), int(row0), chunk.shape[0], _stream())
 
@@ -182,7 +216,12 @@ def head_chunk_rows(M: int, Vp: int, budget_bytes: int, tile_n: int = 256, sms: 
 
 def finalize_loss(tok_lp: torch.Tensor, mask: torch.Tensor, nsum: torch.Tensor,
                   inbatch_losses: Optional[torch.Tensor]) -> torch.Tensor:
+    _chk(tok_lp, f32, "finalize_loss tok_lp"); _chk(mask, i64, "finalize_loss mask")
     B, L = tok_lp.shape
+    if not tok_lp.is_contiguous() or mask.shape != (B, L):
+        raise _lib.DalmB200Error(f"finalize_loss: need a dense fp32 tok_lp and a mask of its shape, got tok_lp "
+                                 f"{tuple(tok_lp.shape)} strides {tok_lp.stride()}, mask {tuple(mask.shape)}")
+    _vec(nsum, f32, "finalize_loss nsum", 1); _vec(inbatch_losses, f32, "finalize_loss inbatch_losses", 4)
     out = torch.empty(4, dtype=f32, device=tok_lp.device)
     _lib.call("dalm_b200_finalize_loss", _p(tok_lp), _p(mask.contiguous()), B, L, _p(nsum), _p(inbatch_losses), _p(out), _stream())
     return out
@@ -703,6 +742,8 @@ def gelu_bwd_(pre, dact):
 def pool_norm_fwd(hidden, mask, normalize: bool = True):
     B, L, H = hidden.shape
     _chk(hidden, f32, "hidden"); _chk(mask, i64, "mask")
+    if mask.shape != (B, L):
+        raise _lib.DalmB200Error(f"pool_norm_fwd: mask {tuple(mask.shape)} must be [{B}, {L}] like hidden")
     pooled = torch.empty(B, H, dtype=f32, device=hidden.device)
     emb = torch.empty_like(pooled)
     norm = torch.empty(B, dtype=f32, device=hidden.device)
@@ -713,6 +754,11 @@ def pool_norm_fwd(hidden, mask, normalize: bool = True):
 
 def pool_norm_bwd(emb, norm, d_emb, mask, L: int, normalize: bool = True):
     B, H = emb.shape
+    _rows32(emb, "pool_norm_bwd emb", H, B); _vec(norm, f32, "pool_norm_bwd norm", B)
+    _chk(d_emb, f32, "pool_norm_bwd d_emb", inner_contig=False); _chk(mask, i64, "pool_norm_bwd mask", inner_contig=False)
+    if d_emb.shape != (B, H) or mask.shape != (B, L):
+        raise _lib.DalmB200Error(f"pool_norm_bwd: d_emb {tuple(d_emb.shape)} / mask {tuple(mask.shape)} must be [{B}, {H}] / "
+                                 f"[{B}, {L}]")
     d_hidden = torch.empty(B, L, H, dtype=f32, device=emb.device)
     _lib.call("dalm_b200_pool_norm_bwd", _p(emb), _p(norm), _p(d_emb.contiguous()), _p(mask.contiguous()), _p(d_hidden), B, L, H,
               1 if normalize else 0, _stream())
@@ -722,19 +768,34 @@ def pool_norm_bwd(emb, norm, d_emb, mask, L: int, normalize: bool = True):
 def lora_wgrad_(x, g, out, so_r: int, so_k: int, K: int, R: int, scale: float = 1.0, out1=None, dropx: Optional[Drop] = None):
     """out[r*so_r + k*so_k] += scale * sum_m g[m,r] x[m,k]; with R == 16 rows 8..15 accumulate into out1 (same strides)"""
     M = x.shape[0]
+    _bf16_rows(x, "lora_wgrad x", M, K); _bf16_rows(g, "lora_wgrad g", M, R)
+    need = (min(R, 8) - 1) * so_r + (K - 1) * so_k                      # farthest element written in each output
+    for t, n in ((out, "out"), (out1, "out1")):
+        if t is None:
+            continue
+        _chk(t, f32, f"lora_wgrad {n}", inner_contig=False)
+        if so_r < 0 or so_k < 0 or min(t.stride()) < 0 or _reach(t) < need:
+            raise _lib.DalmB200Error(f"lora_wgrad: {n} {tuple(t.shape)} strides {t.stride()} does not cover "
+                                     f"[{min(R, 8)}, {K}] at strides ({so_r}, {so_k})")
     _lib.call("dalm_b200_lora_wgrad", _p(x), _ld(x), _p(g), _ld(g), _p(out), _p(out1), so_r, so_k, M, K, R, float(scale),
               *_d(dropx), _stream())
     return out
 
 
 def skinny_gemm(x, w, out, K: int, R: int, dropx: Optional[Drop] = None):
-    """out[M,R] (bf16 view) = x[M,K] @ w[R,K]^T   (R in {8,16})"""
+    """out[M,R] (bf16 view) = x[M,K] @ w[R,K]^T   (R in {8,16,24,32})"""
+    M = x.shape[0]
+    _bf16_rows(x, "skinny_gemm x", M, K); _bf16_rows(w, "skinny_gemm w", R, K); _bf16_rows(out, "skinny_gemm out", M, R)
+    if out.shape[0] != M:
+        raise _lib.DalmB200Error(f"skinny_gemm: out {tuple(out.shape)} must have one row per row of x ({M})")
     _lib.call("dalm_b200_skinny_gemm", _p(x), _ld(x), _p(w), _ld(w), _p(out), _ld(out), x.shape[0], K, R, *_d(dropx), _stream())
     return out
 
 
 def lora_dx_(dh, g, a_stack, K: int, R: int, drop: Drop):
     """dh[m,k] += mask(m,k)/(1-p) * sum_r g[m,r] a_stack[r,k]"""
+    M = dh.shape[0]
+    _bf16_rows(dh, "lora_dx dh", M, K); _bf16_rows(g, "lora_dx g", M, R); _bf16_rows(a_stack, "lora_dx a_stack", R, K)
     p, seed, stream, off = _d(drop)
     _lib.call("dalm_b200_lora_dx", _p(dh), _ld(dh), _p(g), _ld(g), _p(a_stack), _ld(a_stack), dh.shape[0], K, R, p, seed, stream, off, _stream())
     return dh
@@ -853,7 +914,9 @@ def topk_ip(q: torch.Tensor, p: torch.Tensor, k: int) -> Tuple[torch.Tensor, tor
         q = q.contiguous()
     nq, D = q.shape
     N = p.shape[0]
-    scores = torch.empty(nq, k, dtype=f32, device=q.device)
+    if p.dim() != 2 or p.shape[1] != D:
+        raise _lib.DalmB200Error(f"topk_ip: passages {tuple(p.shape)} must be [N, {D}] like the queries")
+    scores =torch.empty(nq, k, dtype=f32, device=q.device)
     idx = torch.empty(nq, k, dtype=torch.int32, device=q.device)
     ws = torch.empty(int(_lib.load().dalm_b200_topk_ip_workspace(nq, k)), dtype=torch.uint8, device=q.device)
     _lib.call("dalm_b200_topk_ip", _p(q), _p(p), _ld(p), nq, N, D, int(k), _p(scores), _p(idx), _p(ws), _stream())
@@ -940,6 +1003,12 @@ def rope_pos_(buf, col0: int, nheads: int, D: int, cos_t, sin_t, pos):
     M = buf.shape[0]
     if pos.numel() != M or not pos.is_contiguous():
         raise _lib.DalmB200Error(f"rope_pos: need one contiguous position id per row ({pos.numel()} for {M} rows)")
+    if buf.dim() != 2 or col0 < 0 or col0 + nheads * D > buf.shape[1]:
+        raise _lib.DalmB200Error(f"rope_pos: heads [{col0}, {col0} + {nheads} x {D}) outside buf {tuple(buf.shape)}")
+    if cos_t.dim() != 2 or cos_t.shape[1] != D // 2 or sin_t.shape != cos_t.shape or not cos_t.is_contiguous() \
+            or not sin_t.is_contiguous():
+        raise _lib.DalmB200Error(f"rope_pos: cos / sin must be dense fp32 [T, {D // 2}], got {tuple(cos_t.shape)} strides "
+                                 f"{cos_t.stride()} / {tuple(sin_t.shape)} strides {sin_t.stride()}")
     _lib.call("dalm_b200_rope_pos", _p(buf), _ld(buf), col0, nheads, D, _p(cos_t), _p(sin_t), _p(pos), M, cos_t.shape[0], _stream())
     return buf
 
@@ -964,8 +1033,16 @@ def attention_decode(qkv, q_col: int, k_col: int, v_col: int, cache_k, cache_v, 
         raise _lib.DalmB200Error("attention_decode: cache_k / cache_v / mask shapes disagree")
     if qkv.shape[0] != B:
         raise _lib.DalmB200Error("attention_decode: one qkv row per cached sequence")
+    for c, n, what in ((q_col, Hq, "q"), (k_col, Hkv, "k"), (v_col, Hkv, "v")):
+        if c < 0 or c + n * D > qkv.shape[1]:
+            raise _lib.DalmB200Error(f"attention_decode: {what} columns [{c}, {c} + {n} x {D}) outside qkv {tuple(qkv.shape)}")
+    if cache_k.shape[2] < Hkv * D:
+        raise _lib.DalmB200Error(f"attention_decode: cache rows {tuple(cache_k.shape)} narrower than {Hkv} x {D}")
     if out is None:
         out = torch.empty(B, Hq * D, dtype=bf16, device=qkv.device)
+    _chk(out, bf16, "attention_decode out")
+    if out.dim() != 2 or out.shape[0] != B or out.shape[1] < Hq * D:
+        raise _lib.DalmB200Error(f"attention_decode: out {tuple(out.shape)} must be bf16 [{B}, >= {Hq * D}]")
     scale = 1.0 / math.sqrt(D) if scale is None else scale
     cur_host, cur_dev = _cur_arg(cur, B, "attention_decode")
     _lib.call("dalm_b200_attention_decode", _p(qkv), _ld(qkv), q_col, k_col, v_col, _p(cache_k), _p(cache_v),

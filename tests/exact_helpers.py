@@ -76,6 +76,27 @@ class Guarded:
                         f"({r - GUARD_R}, {c - self.c0}) of a [{self.rows}, {self.cols}] view")
 
 
+class Guarded1d:
+    """a flat output view of n elements between two sentinel bands of GUARD_C elements (16-byte aligned start): for outputs
+    the kernels index by explicit strides (a transposed gradient, a padded KV cache viewed with as_strided)"""
+
+    def __init__(self, n, dtype, dev, init=None):
+        itype, bits = _SENTINEL_BITS[dtype]
+        self.buf = torch.full((n + 2 * GUARD_C,), bits, dtype=itype, device=dev).view(dtype)
+        self.n, self.itype, self.bits = n, itype, bits
+        self.view = self.buf[GUARD_C:GUARD_C + n]
+        if init is not None:
+            self.view.copy_(init.reshape(-1))
+
+    def check(self, what):
+        b = self.buf.view(self.itype)
+        bad = torch.cat([b[:GUARD_C], b[GUARD_C + self.n:]]) != self.bits
+        if bad.any():
+            i = int(bad.nonzero()[0])
+            at = i - GUARD_C if i < GUARD_C else self.n + i - GUARD_C
+            pytest.fail(f"{what}: {int(bad.sum())} guard elements overwritten; first at output offset {at} of {self.n}")
+
+
 def _ulp_bf16(x):
     """spacing of bf16 numbers at |x| (fp64), normal range"""
     return torch.pow(2.0, torch.floor(torch.log2(x.abs().clamp_min(2.0 ** -126))) - 7)

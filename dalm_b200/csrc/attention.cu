@@ -1224,6 +1224,7 @@ template <int D, bool DROP, bool WIN> static int launch_bwd_wg(const AttnParams&
 static int check_common(const AttnParams& p, int D) {
   DALM_REQUIRE(D == 32 || D == 64 || D == 128, "attention: head_dim %d unsupported (32/64/128)", D);
   DALM_REQUIRE(p.B > 0 && p.L > 0 && p.Hq > 0 && p.Hkv > 0 && p.Hq % p.Hkv == 0, "attention: bad shape B=%d L=%d Hq=%d Hkv=%d", p.B, p.L, p.Hq, p.Hkv);
+  DALM_REQUIRE(p.B <= 65535 && p.Hq <= 65535, "attention: B=%d sequences / Hq=%d heads past 65535 (grid extents)", p.B, p.Hq);
   DALM_REQUIRE(p.ldq % 8 == 0 && p.ldk % 8 == 0 && p.ldv % 8 == 0 && p.ldo % 2 == 0, "attention: strides must keep 16-byte row alignment");
   DALM_REQUIRE(((uintptr_t)p.q & 15) == 0 && ((uintptr_t)p.k & 15) == 0 && ((uintptr_t)p.v & 15) == 0, "attention: q/k/v must be 16-byte aligned");
   DALM_REQUIRE(p.window >= 0, "attention: window %d must be >= 0", p.window);

@@ -135,7 +135,7 @@ extern "C" int dalm_b200_nf4_dequant_bf16(const void* packed, const float* absma
   DALM_REQUIRE(ldo >= cols + tail_cols && (ldo % 8) == 0 && ((uintptr_t)out & 15) == 0 && ((uintptr_t)packed & 7) == 0,
                "nf4_dequant: output stride / alignment");
   DALM_REQUIRE(tail_cols == 0 || (tail != nullptr && ldt >= tail_cols), "nf4_dequant: tail");
-  DALM_REQUIRE(rows <= 65535, "nf4_dequant: %lld rows exceed the grid's y extent", rows);
+  DALM_REQUIRE(rows <= 65535, "nf4_dequant: %lld rows exceed the grid's y extent of 65535", rows);
   const dim3 grid((unsigned)(((cols >> 4) + 1 + 255) / 256), (unsigned)rows);
   nf4_dequant_bf16_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(
       (const unsigned char*)packed, absmax, rows, cols, (__nv_bfloat16*)out, ldo, (const __nv_bfloat16*)tail, ldt, tail_cols);

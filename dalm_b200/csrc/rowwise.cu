@@ -965,7 +965,7 @@ extern "C" int dalm_b200_bert_embed(const int64_t* ids, const void* word, const 
 extern "C" int dalm_b200_roberta_embed(const int64_t* ids, const void* word, const void* pos, const void* type0, int pad_id,
                                        float* z, int64_t* pos_ids_out, int B, int L, int H, int V, int P, void* stream) {
   DALM_REQUIRE(B > 0 && B <= 65535 && L > 0 && V > 0 && P > 0 && H > 0 && (H % 4) == 0 && pad_id >= 0,
-               "roberta_embed: bad shape B=%d L=%d H=%d V=%d P=%d pad_id=%d", B, L, H, V, P, pad_id);
+               "roberta_embed: bad shape B=%d L=%d H=%d V=%d P=%d pad_id=%d (B at most 65535: a grid extent)", B, L, H, V, P, pad_id);
   DALM_REQUIRE(aligned(word, 8) && aligned(pos, 8) && aligned(type0, 8) && aligned(z, 16),
                "roberta_embed: tables must be 8-byte and z 16-byte aligned");
   roberta_embed_kernel<<<dim3((L + kReChunk - 1) / kReChunk, B), 256, 0, ST(stream)>>>(
@@ -985,62 +985,78 @@ extern "C" int dalm_b200_rope(void* buf, long long ld, int col0, int nheads, int
   count_launch();
   return check_launch("rope_kernel");
 }
+// rows go to grid.y, which holds at most 65535: longer batches (bs 8 x 8192 tokens) are launched in chunks of rows, each
+// chunk a view that starts at its first row (a batch of <= 65535 rows stays one launch)
+constexpr int GLU_ROWS = 65535;
+template <class Act>
+static int launch_glu_fwd(const void* gu, long long ldgu, void* act, long long lda, int M, int F, int il, const char* name,
+                          cudaStream_t st) {
+  for (long long r0 = 0; r0 < M; r0 += GLU_ROWS) {
+    dim3 grid((F / 8 + 255) / 256, (unsigned)min((long long)GLU_ROWS, M - r0));
+    glu_fwd_kernel<Act><<<grid, 256, 0, st>>>((const __nv_bfloat16*)gu + r0 * ldgu, ldgu, (__nv_bfloat16*)act + r0 * lda, lda, F, il);
+    count_launch();
+    if (int e = check_launch(name)) return e;
+  }
+  return 0;
+}
+template <class Act>
+static int launch_glu_bwd(void* gu, long long ldgu, const void* dact, long long ldd, int M, int F, int il, const char* name,
+                          cudaStream_t st) {
+  for (long long r0 = 0; r0 < M; r0 += GLU_ROWS) {
+    dim3 grid((F / 8 + 255) / 256, (unsigned)min((long long)GLU_ROWS, M - r0));
+    glu_bwd_kernel<Act><<<grid, 256, 0, st>>>((__nv_bfloat16*)gu + r0 * ldgu, ldgu, (const __nv_bfloat16*)dact + r0 * ldd, ldd, F, il);
+    count_launch();
+    if (int e = check_launch(name)) return e;
+  }
+  return 0;
+}
 extern "C" int dalm_b200_swiglu_fwd(const void* gu, long long ldgu, void* act, long long lda, int M, int F, int interleave, void* stream) {
   DALM_REQUIRE((F % 8) == 0 && (ldgu % 8) == 0 && (lda % 8) == 0, "swiglu: F and strides must be multiples of 8");
   DALM_REQUIRE(interleave == 0 || ((interleave % 8) == 0 && (F % interleave) == 0), "swiglu: interleave block must divide F and be a multiple of 8");
-  dim3 grid((F / 8 + 255) / 256, M);
-  glu_fwd_kernel<SiluAct><<<grid, 256, 0, ST(stream)>>>((const __nv_bfloat16*)gu, ldgu, (__nv_bfloat16*)act, lda, F, interleave);
-  count_launch();
-  return check_launch("swiglu_fwd_kernel");
+  return launch_glu_fwd<SiluAct>(gu, ldgu, act, lda, M, F, interleave, "swiglu_fwd_kernel", ST(stream));
 }
 extern "C" int dalm_b200_swiglu_bwd(void* gu, long long ldgu, const void* dact, long long ldd, int M, int F, int interleave, void* stream) {
   DALM_REQUIRE((F % 8) == 0 && (ldgu % 8) == 0 && (ldd % 8) == 0, "swiglu: F and strides must be multiples of 8");
   DALM_REQUIRE(interleave == 0 || ((interleave % 8) == 0 && (F % interleave) == 0), "swiglu: interleave block must divide F and be a multiple of 8");
-  dim3 grid((F / 8 + 255) / 256, M);
-  glu_bwd_kernel<SiluAct><<<grid, 256, 0, ST(stream)>>>((__nv_bfloat16*)gu, ldgu, (const __nv_bfloat16*)dact, ldd, F, interleave);
-  count_launch();
-  return check_launch("swiglu_bwd_kernel");
+  return launch_glu_bwd<SiluAct>(gu, ldgu, dact, ldd, M, F, interleave, "swiglu_bwd_kernel", ST(stream));
 }
-// rows go to grid.y, which holds at most 65535: longer batches (bs 8 x 8192 tokens) are launched in chunks of rows
-constexpr int GLU_ROWS = 65535;
 extern "C" int dalm_b200_geglu_fwd(const void* x, long long ldx, void* act, long long lda, int M, int F, void* stream) {
   DALM_REQUIRE((F % 8) == 0 && (ldx % 8) == 0 && (lda % 8) == 0, "geglu: F and strides must be multiples of 8");
-  for (int r0 = 0; r0 < M; r0 += GLU_ROWS) {
-    dim3 grid((F / 8 + 255) / 256, min(GLU_ROWS, M - r0));
-    glu_fwd_kernel<GeluAct><<<grid, 256, 0, ST(stream)>>>((const __nv_bfloat16*)x + (size_t)r0 * ldx, ldx,
-                                                         (__nv_bfloat16*)act + (size_t)r0 * lda, lda, F, 0);
-    count_launch();
-    if (int e = check_launch("geglu_fwd_kernel")) return e;
-  }
-  return 0;
+  return launch_glu_fwd<GeluAct>(x, ldx, act, lda, M, F, 0, "geglu_fwd_kernel", ST(stream));
 }
 extern "C" int dalm_b200_geglu_bwd(void* x, long long ldx, const void* dact, long long ldd, int M, int F, void* stream) {
   DALM_REQUIRE((F % 8) == 0 && (ldx % 8) == 0 && (ldd % 8) == 0, "geglu: F and strides must be multiples of 8");
-  for (int r0 = 0; r0 < M; r0 += GLU_ROWS) {
-    dim3 grid((F / 8 + 255) / 256, min(GLU_ROWS, M - r0));
-    glu_bwd_kernel<GeluAct><<<grid, 256, 0, ST(stream)>>>((__nv_bfloat16*)x + (size_t)r0 * ldx, ldx,
-                                                         (const __nv_bfloat16*)dact + (size_t)r0 * ldd, ldd, F, 0);
+  return launch_glu_bwd<GeluAct>(x, ldx, dact, ldd, M, F, 0, "geglu_bwd_kernel", ST(stream));
+}
+// a CTA row of the GELU grid covers GELU_ROWS rows and grid.y holds at most 65535: longer batches go in chunks of
+// GELU_CHUNK rows (a whole number of CTA rows, so every chunk but the last is full and a batch of <= GELU_CHUNK rows is one launch)
+constexpr long long GELU_CHUNK = 65535LL * GELU_ROWS;
+extern "C" int dalm_b200_gelu_fwd(const void* pre, long long ldp, void* act, long long lda, int M, int F, void* stream) {
+  DALM_REQUIRE((F % 8) == 0 && (ldp % 8) == 0 && (lda % 8) == 0, "gelu: F and strides must be multiples of 8");
+  for (long long r0 = 0; r0 < M; r0 += GELU_CHUNK) {
+    const int m = (int)min(GELU_CHUNK, M - r0);
+    dim3 grid((F / 8 + 255) / 256, (m + GELU_ROWS - 1) / GELU_ROWS);
+    gelu_fwd_kernel<<<grid, 256, 0, ST(stream)>>>((const __nv_bfloat16*)pre + r0 * ldp, ldp, (__nv_bfloat16*)act + r0 * lda, lda, m, F);
     count_launch();
-    if (int e = check_launch("geglu_bwd_kernel")) return e;
+    if (int e = check_launch("gelu_fwd_kernel")) return e;
   }
   return 0;
 }
-extern "C" int dalm_b200_gelu_fwd(const void* pre, long long ldp, void* act, long long lda, int M, int F, void* stream) {
-  DALM_REQUIRE((F % 8) == 0 && (ldp % 8) == 0 && (lda % 8) == 0, "gelu: F and strides must be multiples of 8");
-  dim3 grid((F / 8 + 255) / 256, (M + GELU_ROWS - 1) / GELU_ROWS);
-  gelu_fwd_kernel<<<grid, 256, 0, ST(stream)>>>((const __nv_bfloat16*)pre, ldp, (__nv_bfloat16*)act, lda, M, F);
-  count_launch();
-  return check_launch("gelu_fwd_kernel");
-}
 extern "C" int dalm_b200_gelu_bwd(const void* pre, long long ldp, void* dact, long long ldd, int M, int F, void* stream) {
   DALM_REQUIRE((F % 8) == 0 && (ldp % 8) == 0 && (ldd % 8) == 0, "gelu: F and strides must be multiples of 8");
-  dim3 grid((F / 8 + 255) / 256, (M + GELU_ROWS - 1) / GELU_ROWS);
-  gelu_bwd_kernel<<<grid, 256, 0, ST(stream)>>>((const __nv_bfloat16*)pre, ldp, (__nv_bfloat16*)dact, ldd, M, F);
-  count_launch();
-  return check_launch("gelu_bwd_kernel");
+  for (long long r0 = 0; r0 < M; r0 += GELU_CHUNK) {
+    const int m = (int)min(GELU_CHUNK, M - r0);
+    dim3 grid((F / 8 + 255) / 256, (m + GELU_ROWS - 1) / GELU_ROWS);
+    gelu_bwd_kernel<<<grid, 256, 0, ST(stream)>>>((const __nv_bfloat16*)pre + r0 * ldp, ldp, (__nv_bfloat16*)dact + r0 * ldd, ldd, m, F);
+    count_launch();
+    if (int e = check_launch("gelu_bwd_kernel")) return e;
+  }
+  return 0;
 }
 extern "C" int dalm_b200_pool_norm_fwd(const float* hidden, const int64_t* mask, float* pooled, float* emb, float* norm,
                                        int B, int L, int H, int normalize, void* stream) {
+  DALM_REQUIRE(B > 0 && B <= 65535 && L > 0 && H > 0, "pool_norm_fwd: bad shape B=%d L=%d H=%d (at most 65535 samples: B is a grid "
+               "extent)", B, L, H);
   if ((H % 128) == 0 && (reinterpret_cast<uintptr_t>(hidden) & 15) == 0) {
     pool_sum_kernel<<<dim3(H / 128, B), 256, 0, ST(stream)>>>(hidden, mask, pooled, L, H);
     if (int e = check_launch("pool_sum_kernel")) return e;
@@ -1103,6 +1119,7 @@ extern "C" int dalm_b200_lora_dx(void* dh, long long lddh, const void* G, long l
                                  const void* offset, void* stream) {
   DALM_REQUIRE((R == 8 || R == 16 || R == 24) && (K % 8) == 0 && (lddh % 8) == 0 && (lda % 8) == 0, "lora_dx: bad shape R=%d K=%d", R, K);
   DALM_REQUIRE(p >= 0.f && p < 1.f, "lora_dx: p must be in [0,1)");
+  DALM_REQUIRE(M >= 0 && M <= 65535 * 16, "lora_dx: M=%d rows past the grid's 65535 blocks of 16", M);
   // one thread per 8 columns: a CTA no wider than the row (bge-large, K = 1024: 128 threads - a 256-thread CTA keeps half of its
   // warps resident but idle)
   const int cols8 = K / 8;

@@ -285,10 +285,14 @@ __global__ void __launch_bounds__(256) topk_merge_kernel(const float* __restrict
 
 using namespace dalm;
 
+// Queries go in chunks of kTopkChunk (2048 query tiles), so that the query tiles' grid.y stays far below its 65535 limit and the
+// candidate workspace ([CTA][query][K] of one chunk, reused by the next) stays bounded for any nq: at most 1.1 GB at K = 32 on
+// 132 SMs. Each query's result depends on its own row only, so the chunking changes no output bit.
+constexpr int kTopkChunk = 16384;
 // workspace the caller must provide: dalm_b200_topk_ip_workspace(nq, K) bytes
 static int topk_grid_x() { return 2 * num_sms(); }
 extern "C" long long dalm_b200_topk_ip_workspace(int nq, int K) {
-  return (long long)topk_grid_x() * nq * K * (long long)(sizeof(float) + sizeof(int));
+  return (long long)topk_grid_x() * (nq < kTopkChunk ? nq : kTopkChunk) * K * (long long)(sizeof(float) + sizeof(int));
 }
 
 // out_scores [nq,K] fp32 (inner products, descending), out_idx [nq,K] int32 (passage rows; -1 past the end when N < K).
@@ -301,8 +305,9 @@ extern "C" int dalm_b200_topk_ip(const float* Q, const float* P, long long ldp, 
   DALM_REQUIRE((reinterpret_cast<uintptr_t>(P) & 15) == 0 && (reinterpret_cast<uintptr_t>(Q) & 15) == 0, "topk_ip: operands must be 16-byte aligned");
   DALM_REQUIRE(workspace != nullptr, "topk_ip: workspace is NULL (size it with dalm_b200_topk_ip_workspace)");
   const int nwarps = 8;
+  const int nq_max = nq < kTopkChunk ? nq : kTopkChunk;
   float* cs = reinterpret_cast<float*>(workspace);
-  int* ci = reinterpret_cast<int*>(cs + (size_t)topk_grid_x() * nq * K);
+  int* ci = reinterpret_cast<int*>(cs + (size_t)topk_grid_x() * nq_max * K);
   static bool attr_set = false;
   if (!attr_set) {
     DALM_CUDA(cudaFuncSetAttribute(topk_scan_kernel<kTopkQT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
@@ -310,31 +315,40 @@ extern "C" int dalm_b200_topk_ip(const float* Q, const float* P, long long ldp, 
     attr_set = true;
   }
   int gx;
+  size_t smem;
   const size_t smem_m = (size_t)nwarps * kTopkQT * 32 * (sizeof(float) + sizeof(int));
   const size_t smem_pipe = (size_t)(kTopkQT + kTopkPipeWarps * 2 * kTopkR) * D * sizeof(float);
-  if (D <= kTopkPipeMaxD && smem_pipe >= smem_m) {
+  const bool pipe = D <= kTopkPipeMaxD && smem_pipe >= smem_m;
+  if (pipe) {
     // pipelined sweep: one CTA per SM (its rings take most of the shared memory), 2 rows per warp step
     gx = smem_pipe * 2 <= 200 * 1024 ? 2 * num_sms() : num_sms();   // small D: two CTAs per SM keep enough bytes in flight
     const int max_gx = (N + kTopkR * kTopkPipeWarps - 1) / (kTopkR * kTopkPipeWarps);
     if (gx > max_gx) gx = max_gx;
-    const size_t smem = smem_pipe;
-    dim3 grid(gx, (nq + kTopkQT - 1) / kTopkQT);
-    topk_scan_pipe_kernel<kTopkQT><<<grid, kTopkPipeWarps * 32, smem, (cudaStream_t)stream>>>(Q, P, ldp, nq, N, D, K, cs, ci);
-    count_launch();
-    if (int e = check_launch("topk_scan_pipe_kernel")) return e;
+    smem = smem_pipe;
   } else {
     gx = topk_grid_x();
     const int max_gx = (N + 2 * nwarps - 1) / (2 * nwarps);
     if (gx > max_gx) gx = max_gx;
     const size_t smem_q = (size_t)kTopkQT * D * sizeof(float);
-    const size_t smem = smem_q > smem_m ? smem_q : smem_m;
+    smem = smem_q > smem_m ? smem_q : smem_m;
     DALM_REQUIRE(smem <= 200 * 1024, "topk_ip: D=%d too large for the query tile in shared memory", D);
-    dim3 grid(gx, (nq + kTopkQT - 1) / kTopkQT);
-    topk_scan_kernel<kTopkQT><<<grid, nwarps * 32, smem, (cudaStream_t)stream>>>(Q, P, ldp, nq, N, D, K, cs, ci);
-    count_launch();
-    if (int e = check_launch("topk_scan_kernel")) return e;
   }
-  topk_merge_kernel<<<nq, 256, 0, (cudaStream_t)stream>>>(cs, ci, gx, nq, K, out_scores, out_idx);
-  count_launch();
-  return check_launch("topk_merge_kernel");
+  for (int q0 = 0; q0 < nq; q0 += kTopkChunk) {
+    const int n = nq - q0 < kTopkChunk ? nq - q0 : kTopkChunk;
+    const float* Qc = Q + (size_t)q0 * D;
+    dim3 grid(gx, (n + kTopkQT - 1) / kTopkQT);
+    if (pipe) {
+      topk_scan_pipe_kernel<kTopkQT><<<grid, kTopkPipeWarps * 32, smem, (cudaStream_t)stream>>>(Qc, P, ldp, n, N, D, K, cs, ci);
+      count_launch();
+      if (int e = check_launch("topk_scan_pipe_kernel")) return e;
+    } else {
+      topk_scan_kernel<kTopkQT><<<grid, nwarps * 32, smem, (cudaStream_t)stream>>>(Qc, P, ldp, n, N, D, K, cs, ci);
+      count_launch();
+      if (int e = check_launch("topk_scan_kernel")) return e;
+    }
+    topk_merge_kernel<<<n, 256, 0, (cudaStream_t)stream>>>(cs, ci, gx, n, K, out_scores + (size_t)q0 * K, out_idx + (size_t)q0 * K);
+    count_launch();
+    if (int e = check_launch("topk_merge_kernel")) return e;
+  }
+  return 0;
 }

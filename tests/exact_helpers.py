@@ -67,13 +67,18 @@ class Guarded:
             self.view.copy_(init)
 
     def check(self, what):
-        b = self.buf.view(self.itype).clone()
-        b[GUARD_R:GUARD_R + self.rows, self.c0:self.c0 + self.cols] = self.bits
-        bad = b != self.bits
-        if bad.any():
-            r, c = bad.nonzero()[0].tolist()
-            pytest.fail(f"{what}: {int(bad.sum())} guard elements overwritten; first at buffer ({r}, {c}) = output "
-                        f"({r - GUARD_R}, {c - self.c0}) of a [{self.rows}, {self.cols}] view")
+        """the four bands around the view, each compared in place (no copy of the whole buffer: some outputs are GBs)"""
+        b = self.buf.view(self.itype)
+        r1, c0, c1 = GUARD_R + self.rows, self.c0, self.c0 + self.cols
+        for rs, cs in ((slice(0, GUARD_R), slice(None)), (slice(r1, None), slice(None)),
+                       (slice(GUARD_R, r1), slice(0, c0)), (slice(GUARD_R, r1), slice(c1, None))):
+            bad = b[rs, cs] != self.bits
+            if bad.any():
+                r, c = bad.nonzero()[0].tolist()
+                r += rs.start
+                c += cs.start or 0
+                pytest.fail(f"{what}: {int(bad.sum())} guard elements overwritten in one band; first at buffer ({r}, {c}) = "
+                            f"output ({r - GUARD_R}, {c - self.c0}) of a [{self.rows}, {self.cols}] view")
 
 
 class Guarded1d:
@@ -144,6 +149,34 @@ def _ints(shape, g, hi=2):
 
 def _gelu64(x):
     return 0.5 * x * (1.0 + torch.erf(x / math.sqrt(2.0)))
+
+
+def _gelu_grad64(x):
+    return 0.5 * (1.0 + torch.erf(x / math.sqrt(2.0))) + x * torch.exp(-0.5 * x * x) / math.sqrt(2.0 * math.pi)
+
+
+# erff in fp32: a few ulps, plus the cancellation in 1 + erf(x / sqrt 2) for negative x (~|x| 2^-23): gelu_erf(x) is within
+# _gelu_tol(x) of fp64, its derivative within _gelu_grad_tol(x)
+def _gelu_tol(x):
+    return 2.0 ** -21 * (_gelu64(x).abs() + x.abs())
+
+
+def _gelu_grad_tol(x):
+    return 2.0 ** -20 * (_gelu_grad64(x).abs() + 1)
+
+
+# __expf is within (2 + 1.16 |x|) ulp (CUDA programming guide); with the IEEE division and products that follow, silu(g)
+# and sigmoid(g) are within 2^-19 (1 + |g|) relative
+def _silu_tol(g):
+    return 2.0 ** -19 * (1 + g.abs())
+
+
+def _ce_dlse(V, lse, mx, span):
+    """bound on |lse - fp64| of a cross-entropy row of V logits (fp32, ce_rows_kernel): the sum of V exponentials has chain
+    depth V / 512 + 24, each __expf within (2 + 1.16 |x - max|) ulp; __logf within 2^-21.4 absolute on [0.5, 2] and 3 ulp
+    elsewhere; lse and the difference one rounding each. lse, mx (row max), span (max - min): fp64 [rows, 1]"""
+    U = 2.0 ** -24
+    return (V / 512 + 24) * U + 2.0 ** -23 * (2 + 1.2 * span) + 2.0 ** -21 + 3 * 2.0 ** -23 * (lse - mx) + U * lse.abs()
 
 
 def _pick_block_n(M, N, sms):

@@ -19,7 +19,8 @@ import numpy as np
 import pytest
 import torch
 
-from exact_helpers import PAD_R, Guarded, _dense_poisoned, _expect_close, _expect_equal, _poisoned, _ulp_bf16
+from exact_helpers import (PAD_R, Guarded, _ce_dlse, _dense_poisoned, _expect_close, _expect_equal, _gelu64, _gelu_grad64,
+                           _gelu_grad_tol, _gelu_tol, _poisoned, _silu_tol, _ulp_bf16)
 
 pytestmark = pytest.mark.gpu
 bf16, f32, f64 = torch.bfloat16, torch.float32, torch.float64
@@ -641,12 +642,6 @@ def test_rope(ops, cuda_dev, D, M):
         _expect_equal(buf.view[:, col0 + nh * D:], x[:, col0 + nh * D:], what + " right of the heads")
 
 
-# __expf is within (2 + 1.16 |x|) ulp (CUDA programming guide); with the IEEE division and products that follow, silu(g)
-# and sigmoid(g) are within 2^-19 (1 + |g|) relative
-def _silu_tol(g):
-    return 2.0 ** -19 * (1 + g.abs())
-
-
 @pytest.mark.parametrize("F,il", [(8, 0), (264, 0), (256, 128), (384, 128)])
 def test_swiglu(ops, cuda_dev, F, il):
     dev, M = cuda_dev, 5
@@ -678,14 +673,6 @@ def test_swiglu(ops, cuda_dev, F, il):
     _expect_close(work.view[:, ucols], du, _ulp_bf16(du) + _silu_tol(g) * du.abs(), what + " dup")
 
 
-def _gelu64(x):
-    return 0.5 * x * (1.0 + torch.erf(x / math.sqrt(2.0)))
-
-
-def _gelu_grad64(x):
-    return 0.5 * (1.0 + torch.erf(x / math.sqrt(2.0))) + x * torch.exp(-0.5 * x * x) / math.sqrt(2.0 * math.pi)
-
-
 @pytest.mark.parametrize("M", [1, 2, 3, 4, 5, 9])
 @pytest.mark.parametrize("F", [8, 264, 2056])
 def test_gelu(ops, cuda_dev, M, F):
@@ -699,15 +686,14 @@ def test_gelu(ops, cuda_dev, M, F):
     act.check(what)
     x = pre.double()
     ref = _gelu64(x)
-    # erff in fp32: a few ulps, plus the cancellation in 1 + erf(x / sqrt 2) for negative x (~|x| 2^-23)
-    _expect_close(act.view, ref, _ulp_bf16(ref) + 2.0 ** -21 * (ref.abs() + x.abs()), what + " fwd")
+    _expect_close(act.view, ref, _ulp_bf16(ref) + _gelu_tol(x), what + " fwd")
     d = torch.randn(M, F, generator=gen, device=dev).to(bf16)
     work = Guarded(M, F, bf16, dev, init=d)
     ops.gelu_bwd_(_poisoned(pre), work.view)
     work.check(what)
     gg = _gelu_grad64(x)
     ref = d.double() * gg
-    _expect_close(work.view, ref, _ulp_bf16(ref) + 2.0 ** -20 * d.double().abs() * (gg.abs() + 1), what + " bwd")
+    _expect_close(work.view, ref, _ulp_bf16(ref) + d.double().abs() * _gelu_grad_tol(x), what + " bwd")
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -786,9 +772,7 @@ def test_ce_rows_large_vocab(ops, cuda_dev, V, inplace):
     lp = (x64.gather(1, label[:, None]) - lse)[:, 0] * (w > 0)
     mx = x64.max(1, keepdim=True).values
     span = mx - x64.min(1, keepdim=True).values
-    # sum of V exponentials: chain depth V / 512 + 24, each __expf within (2 + 1.16 |x - max|) ulp; __logf within 2^-21.4
-    # absolute on [0.5, 2] and 3 ulp elsewhere; lse and the difference one rounding each
-    dlse = ((V / 512 + 24) * U + 2.0 ** -23 * (2 + 1.2 * span) + 2.0 ** -21 + 3 * 2.0 ** -23 * (lse - mx) + U * lse.abs())
+    dlse = _ce_dlse(V, lse, mx, span)
     _expect_close(tok_lp.view(1, -1), lp.view(1, -1), (dlse[:, 0] + U * lp.abs()).view(1, -1) * (w > 0), what + " tok_lp")
     prob = torch.exp(x64 - lse)
     onehot = torch.zeros_like(prob).scatter_(1, label[:, None], 1.0)

@@ -85,6 +85,13 @@ SIGNATURES = {
     "dalm_b200_attention_decode": [_P, _L, _I, _I, _I, _P, _P, _L, _L, _P, _L, _P, _L, _I, _I, _I, _I, _I, _P, _I, _F, _I, _P],
     "dalm_b200_greedy_step": [_P, _L, _I, _I, _P, _I, _L, _P, _P, _L, _P, _L, _I, _P, _I, _P, _P, _P, _P],
     "dalm_b200_sample_step": [_P, _L, _I, _I, _P, _I, _L, _P, _P, _L, _P, _L, _I, _P, _I, _P, _P, _P, _F, _I, _F, _U, _P, _P, _P],
+    "dalm_b200_gemm_bf16_grouped": [_I, _I, _P, _L, _P, _I, _P, _L, _P, _L, _I, _I, _I, _P, _P, _I, _P],
+    "dalm_b200_moe_router": [_P, _L, _I, _I, _I, _I, _P, _P, _P],
+    "dalm_b200_moe_router_bwd": [_P, _L, _P, _P, _P, _I, _I, _I, _I, _P, _L, _P],
+    "dalm_b200_moe_permute": [_P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P],
+    "dalm_b200_moe_gather": [_P, _L, _I, _I, _P, _I, _P, _I, _P, _L, _P],
+    "dalm_b200_moe_combine": [_P, _L, _P, _P, _I, _I, _I, _P, _L, _P, _L, _I, _P],
+    "dalm_b200_moe_down_bwd": [_P, _L, _P, _L, _P, _P, _I, _I, _P, _P, _L, _P],
 }
 _RESTYPES = {
     "dalm_b200_last_error": c_char_p,

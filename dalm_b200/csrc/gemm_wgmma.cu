@@ -52,6 +52,9 @@ struct GemmEpilogue {
   int norm_pre;                                   //   1: tmap_out2 receives the pre-norm q|k columns [M, rope_cols]
   int l2_hints;         // TMA L2 eviction priorities: bit 0 = A loads evict_last (the panel the resident CTAs share across waves),
                         // bit 1 = B loads evict_first (streamed once per band), bit 2 = output stores evict_first
+  // grouped kernels (GROUPED = true) only: A's rows are segments of one expert each, padded to the 128-row M tile
+  const int* grp_tiles; // [ceil(M / 128)] expert of each M tile; the live tiles are a prefix, each with an expert >= 0
+  const int* grp_live;  // device count of live M tiles, written by the routing kernels; the tiles after it exit
 };
 
 // Tile rasterisation. Persistent CTA i works on tiles i, i + grid, ...: the tiles resident at one moment are ~132 consecutive
@@ -446,13 +449,17 @@ __device__ __forceinline__ void wgmma_tile(float* d, uint64_t da, uint64_t db, i
 // producer refills it at once: while the consumers run a tile's epilogue, the next tile's first STAGES k-blocks load.
 // CL = 2: a cluster of two CTAs computes a 256 x BN tile (128 rows each); each CTA loads half of the shared B tile and
 // multicasts it to both, so every B panel is read from L2 once per two CTAs (block_n 2128 / 2256).
-template <int BN, int LAYOUT, Epi EPI, int CL>
+// GROUPED: B is a stack of per-expert weights [E, N, K] (layout 0) or [E, K, N] (layout 1), addressed as one 2-D tensor map
+// of E N (or E K) rows; M tile m multiplies by expert ep.grp_tiles[m]'s slab. Only the first *ep.grp_live M tiles run, so
+// the grid is sized for the static bound of padded rows and nothing on the host needs the routing.
+template <int BN, int LAYOUT, Epi EPI, int CL, bool GROUPED>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                     const __grid_constant__ CUtensorMap tmap_out, const __grid_constant__ CUtensorMap tmap_out2, const GemmEpilogue ep) {
   using Cfg = GemmCfg<BN>;
   constexpr int BM = Cfg::BM, BK = Cfg::BK, STAGES = Cfg::STAGES;
   static_assert(CL == 1 || (LAYOUT == 0 && EPI == Epi::Plain), "the cluster kernel takes the plain TN layout");
+  static_assert(!GROUPED || (CL == 1 && LAYOUT <= 1), "the grouped kernel takes the TN and NN layouts on single CTAs");
   extern __shared__ unsigned char smem_raw[];
   // 128B swizzle atoms need 1024-byte aligned tile bases
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -463,7 +470,8 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t rank = CL == 2 ? cluster_ctarank() : 0u;
   const int M = ep.M, N = ep.N, K = ep.K;
-  const int num_m = (M + CL * BM - 1) / (CL * BM), num_n = (N + BN - 1) / BN;
+  const int num_m = GROUPED ? min((M + BM - 1) / BM, __ldg(ep.grp_live)) : (M + CL * BM - 1) / (CL * BM);
+  const int num_n = (N + BN - 1) / BN;
   const int num_tiles = num_m * num_n;
   const int num_kb = (K + BK - 1) / BK;
   const int unit = blockIdx.x / CL, num_units = gridDim.x / CL;
@@ -498,6 +506,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
       for (int tile = unit; tile < num_tiles; tile += num_units) {
         int m_blk, n_blk;
         tile_coords(tile, num_m, num_n, group_m, m_blk, n_blk);
+        const int b_row0 = GROUPED ? __ldg(ep.grp_tiles + m_blk) * (LAYOUT == 1 ? K : N) : 0;   // the expert's slab of B
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           unsigned char* sa = smem + stage * Cfg::STAGE_BYTES;
@@ -515,9 +524,9 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
             }
             if constexpr (LAYOUT >= 1) {
 #pragma unroll
-              for (int c = 0; c < BN / 64; ++c) load(sb + c * 8192, &tmap_b, &full_bar[stage], n_blk * BN + c * 64, kb * BK, hint_b, pol_b);
+              for (int c = 0; c < BN / 64; ++c) load(sb + c * 8192, &tmap_b, &full_bar[stage], n_blk * BN + c * 64, b_row0 + kb * BK, hint_b, pol_b);
             } else {
-              load(sb, &tmap_b, &full_bar[stage], kb * BK, n_blk * BN, hint_b, pol_b);
+              load(sb, &tmap_b, &full_bar[stage], kb * BK, b_row0 + n_blk * BN, hint_b, pol_b);
             }
           }
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -637,37 +646,37 @@ int get_tmap(const void* ptr, long long rows, long long cols, long long ld, int 
   return 0;
 }
 
-template <int BN, int LAYOUT, Epi EPI>
+template <int BN, int LAYOUT, Epi EPI, bool GROUPED = false>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const GemmEpilogue& ep,
                        int max_ctas, cudaStream_t stream, const CUtensorMap* to2) {
   using Cfg = GemmCfg<BN>;
   static bool attr_set = false;
   if (!attr_set) {
-    DALM_CUDA(cudaFuncSetAttribute(gemm_bf16_tn_kernel<BN, LAYOUT, EPI, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    DALM_CUDA(cudaFuncSetAttribute(gemm_bf16_tn_kernel<BN, LAYOUT, EPI, 1, GROUPED>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     attr_set = true;
   }
   const int num_tiles = ((ep.M + 127) / 128) * ((ep.N + BN - 1) / BN);
   int grid = num_tiles < num_sms() ? num_tiles : num_sms();
   if (max_ctas > 0 && grid > max_ctas) grid = max_ctas;
-  gemm_bf16_tn_kernel<BN, LAYOUT, EPI, 1><<<grid, kGemmThreads, Cfg::SMEM_BYTES, stream>>>(ta, tb, to, to2 ? *to2 : to, ep);
+  gemm_bf16_tn_kernel<BN, LAYOUT, EPI, 1, GROUPED><<<grid, kGemmThreads, Cfg::SMEM_BYTES, stream>>>(ta, tb, to, to2 ? *to2 : to, ep);
   count_launch();
   return check_launch("gemm_bf16_tn_kernel");
 }
 
 // block_n (64 / 128 / 256) -> the single-CTA kernel of that tile width
-template <int LAYOUT, Epi EPI>
+template <int LAYOUT, Epi EPI, bool GROUPED = false>
 static int launch_gemm_bn(int bn, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const GemmEpilogue& ep,
                           int max_ctas, cudaStream_t stream, const CUtensorMap* to2 = nullptr) {
-  if (bn == 256) return launch_gemm<256, LAYOUT, EPI>(ta, tb, to, ep, max_ctas, stream, to2);
-  if (bn == 128) return launch_gemm<128, LAYOUT, EPI>(ta, tb, to, ep, max_ctas, stream, to2);
-  return launch_gemm<64, LAYOUT, EPI>(ta, tb, to, ep, max_ctas, stream, to2);
+  if (bn == 256) return launch_gemm<256, LAYOUT, EPI, GROUPED>(ta, tb, to, ep, max_ctas, stream, to2);
+  if (bn == 128) return launch_gemm<128, LAYOUT, EPI, GROUPED>(ta, tb, to, ep, max_ctas, stream, to2);
+  return launch_gemm<64, LAYOUT, EPI, GROUPED>(ta, tb, to, ep, max_ctas, stream, to2);
 }
 
 template <int BN>
 static int launch_gemm_cluster(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const GemmEpilogue& ep,
                                int max_ctas, cudaStream_t stream) {
   using Cfg = GemmCfg<BN>;
-  auto kern = gemm_bf16_tn_kernel<BN, 0, Epi::Plain, 2>;
+  auto kern = gemm_bf16_tn_kernel<BN, 0, Epi::Plain, 2, false>;
   static bool attr_set = false;
   if (!attr_set) {
     DALM_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -892,6 +901,40 @@ extern "C" int dalm_b200_gemm_bf16_rope(const void* A, long long lda, const void
   ep.q_norm = q_norm; ep.k_norm = k_norm; ep.nq_heads = nq_heads; ep.norm_eps = eps;
   ep.norm_rstd = rstd_out; ep.ld_rstd = ld_rstd; ep.norm_pre = pre_out != nullptr;
   return launch_gemm<256, 0, Epi::NormRoPE>(ta, tb, to, ep, 0, (cudaStream_t)stream, &to2);
+}
+
+// grouped GEMM over the experts of a routed MLP: out[M,N] (bf16) = A[M,K] . B[e]^T (layout 0, B dense [E, N, K]) or
+// A[M,K] . B[e] (layout 1, B dense [E, K, N]: the dgrad straight from the forward weights), e = tile_expert[m / 128].
+// M is the static bound of padded rows; only the first *live_tiles M tiles are computed (device values, no host sync).
+// swiglu = 1 (layout 0): B[e]'s gate / up rows interleaved in 128-feature blocks, out = gate|up and out2 [M, N/2] =
+// silu(gate) * up, as dalm_b200_gemm_bf16_swiglu.
+extern "C" int dalm_b200_gemm_bf16_grouped(int layout, int swiglu, const void* A, long long lda, const void* B, int E, void* out,
+                                           long long ldo, void* out2, long long ldo2, int M, int N, int K, const int* tile_expert,
+                                           const int* live_tiles, int max_ctas, void* stream) {
+  DALM_REQUIRE(layout == 0 || layout == 1, "gemm_grouped: layout must be 0 (TN) or 1 (NN)");
+  DALM_REQUIRE(M > 0 && N > 0 && K > 0 && E > 0 && (N % 8) == 0 && (K % 8) == 0, "gemm_grouped: bad shape M=%d N=%d K=%d E=%d", M, N, K, E);
+  // a k-block of the NN layout is 64 rows of B: it must not reach into the next expert's slab
+  DALM_REQUIRE(layout == 0 || (K % 64) == 0, "gemm_grouped: the NN layout needs K=%d to be a multiple of 64", K);
+  DALM_REQUIRE(!swiglu || (layout == 0 && (N % 256) == 0 && out2 != nullptr && ldo2 >= N / 2 && (ldo2 % 8) == 0 &&
+                           ((uintptr_t)out2 & 15) == 0),
+               "gemm_grouped: swiglu needs layout 0, N=%d a multiple of 256 and an aligned out2 [M, N/2]", N);
+  DALM_REQUIRE(lda >= K && ldo >= N && (ldo % 8) == 0 && ((uintptr_t)out & 15) == 0, "gemm_grouped: leading dimensions / alignment");
+  DALM_REQUIRE(tile_expert != nullptr && live_tiles != nullptr, "gemm_grouped: tile_expert and live_tiles are required");
+  const int bn = swiglu ? 256 : pick_block_n(M, N);
+  CUtensorMap ta, tb, to, to2;
+  if (int e = get_tmap(A, M, K, lda, 128, &ta)) return e;
+  if (layout == 1) { if (int e = get_tmap(B, (long long)E * K, N, N, 64, &tb)) return e; }
+  else             { if (int e = get_tmap(B, (long long)E * N, K, K, bn, &tb)) return e; }
+  if (int e = get_tmap(out, M, N, ldo, kBoxRows, &to, 0)) return e;
+  GemmEpilogue ep = gemm_epilogue(M, N, K, bn, out, ldo);
+  ep.grp_tiles = tile_expert; ep.grp_live = live_tiles;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (swiglu) {
+    if (int e = get_tmap(out2, M, N / 2, ldo2, kBoxRows, &to2, 0)) return e;
+    return launch_gemm<256, 0, Epi::SwiGLU, true>(ta, tb, to, ep, max_ctas, st, &to2);
+  }
+  if (layout == 1) return launch_gemm_bn<1, Epi::Plain, true>(bn, ta, tb, to, ep, max_ctas, st);
+  return launch_gemm_bn<0, Epi::Plain, true>(bn, ta, tb, to, ep, max_ctas, st);
 }
 
 // drop cached tensor maps (call when operand buffers are freed / re-allocated at the same address with other shapes)

@@ -21,6 +21,9 @@ Mistral (HF MistralForCausalLM) is Llama with sliding-window causal attention: p
 window (0 = none; also Qwen2 / Qwen3 with use_sliding_window), and every attention launch of that layer (training forward and
 backward, prefill, decode) takes it. Headless checkpoints (HF MistralModel / LlamaModel saved by AutoModel, e.g.
 e5-mistral-7b-instruct: `layers.*` with no `model.` prefix and no lm_head) load too; hf_state_dict writes their layout back.
+Qwen3-MoE (HF Qwen3MoeForCausalLM) is Qwen3 whose sparse layers (params.moe_layers) run a routed mixture of SwiGLU experts
+instead of the dense MLP: W["moe"] holds the router and the stacked expert weights, and engine/moe.py runs the layer in the
+training forward and backward, the prefill and the decode step. Expert weights stay frozen (LoRA or inference only).
 """
 from __future__ import annotations
 
@@ -29,9 +32,10 @@ from typing import Dict, List, Optional
 import torch
 
 from .. import ops
+from . import moe
 from .dense import DenseBank
 from .lora import LoraBank
-from .params import attention_biases, check_llama_family, rope_inv_freq, sliding_windows
+from .params import attention_biases, check_llama_family, moe_layers, rope_inv_freq, sliding_windows
 
 bf16, f32 = torch.bfloat16, torch.float32
 
@@ -73,11 +77,16 @@ class LlamaDecoder(torch.nn.Module):
             self.nf4 = Nf4Store(device)
         check_llama_family(cfg)
         self.cfg = cfg
-        self.kind = cfg.get("model_type") if cfg.get("model_type") in ("qwen2", "qwen3", "mistral") else "llama"
+        self.kind = cfg.get("model_type") if cfg.get("model_type") in ("qwen2", "qwen3", "mistral", "qwen3_moe") else "llama"
         self.qkv_bias, self.o_bias = attention_biases(self.kind, cfg)
-        self.qk_norm = self.kind == "qwen3"
+        self.qk_norm = self.kind in ("qwen3", "qwen3_moe")
         self.H = H = cfg["hidden_size"]
-        self.F = F = cfg["intermediate_size"]
+        self.F = F = cfg.get("intermediate_size") or 0          # qwen3_moe without dense layers may leave it out
+        # Qwen3-MoE: the layers that run the routed MLP (engine/moe.py) instead of the dense SwiGLU one
+        self.sparse = moe_layers(cfg) if self.kind == "qwen3_moe" else [False] * cfg["num_hidden_layers"]
+        if any(self.sparse) and (full or nf4_storage):
+            raise NotImplementedError("qwen3_moe: " + ("full fine-tuning is not built (grouped expert weight gradients are not "
+                                                       "built)" if full else "4-bit storage of the expert weights is not built"))
         self.nl = cfg["num_hidden_layers"]
         self.nh = cfg["num_attention_heads"]
         self.nkv = cfg.get("num_key_value_heads", self.nh)
@@ -294,17 +303,37 @@ class LlamaDecoder(torch.nn.Module):
                 W["Bblk"] = torch.zeros(64, self.Nqkv, dtype=bf16, device=self.dev)
             W["Wo"] = g(p + "self_attn.o_proj.weight", bf16)
             W["WoT"] = W["Wo"].t().contiguous()
-            if self.gu_il:     # gate / up rows interleaved in 128-feature blocks: SiLU(gate)*up is fused into this GEMM's epilogue
-                W["Wgu"] = ops.interleave_gate_up(g(p + "mlp.gate_proj.weight", bf16), g(p + "mlp.up_proj.weight", bf16), self.gu_il)
+            if self.sparse[l]:
+                W["moe"] = self._moe_weights(sd, p)
             else:
-                W["Wgu"] = torch.cat([g(p + "mlp.gate_proj.weight", bf16), g(p + "mlp.up_proj.weight", bf16)], 0)
-            W["WguT"] = W["Wgu"].t().contiguous()
-            W["Wd"] = g(p + "mlp.down_proj.weight", bf16)
-            W["WdT"] = W["Wd"].t().contiguous()
+                if self.gu_il:   # gate / up rows interleaved in 128-feature blocks: SiLU(gate)*up is fused into this GEMM's epilogue
+                    W["Wgu"] = ops.interleave_gate_up(g(p + "mlp.gate_proj.weight", bf16), g(p + "mlp.up_proj.weight", bf16), self.gu_il)
+                else:
+                    W["Wgu"] = torch.cat([g(p + "mlp.gate_proj.weight", bf16), g(p + "mlp.up_proj.weight", bf16)], 0)
+                W["WguT"] = W["Wgu"].t().contiguous()
+                W["Wd"] = g(p + "mlp.down_proj.weight", bf16)
+                W["WdT"] = W["Wd"].t().contiguous()
             W["g1"] = g(p + "input_layernorm.weight", f32)
             W["g2"] = g(p + "post_attention_layernorm.weight", f32)
             self._frozen_biases(W, p, g)
             self.layers.append(W)
+
+    def _moe_weights(self, sd, p: str) -> moe.MoeWeights:
+        """a sparse layer's router and experts, from the hub layout (mlp.experts.{e}.{gate,up,down}_proj.weight) or from
+        transformers 5's fused one (mlp.experts.gate_up_proj [E, 2I, H]: gate rows then up rows; mlp.experts.down_proj
+        [E, H, I])"""
+        cfg = self.cfg
+        E, I = int(cfg["num_experts"]), int(cfg["moe_intermediate_size"])
+        if p + "mlp.experts.gate_up_proj" in sd:
+            gu, down = sd[p + "mlp.experts.gate_up_proj"], sd[p + "mlp.experts.down_proj"]
+            gate_proj, up_proj = gu[:, :I], gu[:, I:]
+        else:
+            ex = lambda e, n: sd[p + f"mlp.experts.{e}.{n}_proj.weight"]
+            gate_proj = [ex(e, "gate") for e in range(E)]
+            up_proj = [ex(e, "up") for e in range(E)]
+            down = torch.stack([ex(e, "down").to(bf16) for e in range(E)])
+        return moe.pack_experts(sd[p + "mlp.gate.weight"], gate_proj, up_proj, down, int(cfg["num_experts_per_tok"]),
+                                bool(cfg.get("norm_topk_prob", False)), self.dev)
 
     def _init_layer_nf4(self, sd, l: int, g, lora: bool):
         """one layer in 4-bit storage: q|k|v, o, gate|up (interleaved like the resident mode), down as NF4 codes; blocks of 64
@@ -475,6 +504,11 @@ class LlamaDecoder(torch.nn.Module):
                                                   window=self.windows[li])
             a.x_mid = ops.gemm(a.att, W["Wo"], out_dtype=f32, resid=x, bias=W["bo"])
             a.h2, a.rstd2 = ops.rmsnorm_fwd(a.x_mid, W["g2"], self.eps)
+            if "moe" in W:
+                x, a.moe = moe.forward(a.h2, W["moe"], resid=a.x_mid)
+                if save:
+                    ctx.layers.append(a)
+                continue
             if self.gu_il:
                 a.gu, a.act = ops.gemm_swiglu(a.h2, W["Wgu"])                     # [M,2F] (interleaved) + silu(gate)*up [M,F]: one launch
             else:
@@ -510,6 +544,9 @@ class LlamaDecoder(torch.nn.Module):
                                        self.nh, self.nkv, self.hd, window=self.windows[li])
             x_mid = ops.gemm_rows(att, W["Wo"], out_dtype=f32, resid=x, bias=W["bo"])
             h2, _ = ops.rmsnorm_fwd(x_mid, W["g2"], self.eps)
+            if "moe" in W:
+                x, _ = moe.forward(h2, W["moe"], resid=x_mid)
+                continue
             act = ops.swiglu_fwd(ops.gemm_rows(h2, W["Wgu"]), F, interleave=self.gu_il)
             x = ops.gemm_rows(act, W["Wd"], out_dtype=f32, resid=x_mid)
         hf, _ = ops.rmsnorm_fwd(x, self.norm_g, self.eps)
@@ -569,13 +606,16 @@ class LlamaDecoder(torch.nn.Module):
         dx32, dx16 = ops.rmsnorm_bwd(ctx.x_final, self.norm_g, ctx.rstdf, dhf)
         for l in range(self.nl - 1, -1, -1):
             W, a = self.layers[l], ctx.layers[l]
-            if bank is not None:
-                ops.wgrad_(dx16, a.act, G(l, "Wd"), acc)
-            dact = self._dgrad(dx16, W, "Wd")                                      # [M,F]
-            ops.swiglu_bwd_(a.gu, dact, F, interleave=self.gu_il)                  # gu <- [dgate | dup] (same layout as gu)
-            if bank is not None:
-                ops.wgrad_(a.gu, a.h2, G(l, "Wgu"), acc)
-            dh2 = self._dgrad(a.gu, W, "Wgu")                                      # [M,H]
+            if "moe" in W:                                                         # experts and router frozen: input gradient only
+                dh2 = ops.cast_f32_bf16(moe.backward(dx16, a.moe, W["moe"]))
+            else:
+                if bank is not None:
+                    ops.wgrad_(dx16, a.act, G(l, "Wd"), acc)
+                dact = self._dgrad(dx16, W, "Wd")                                  # [M,F]
+                ops.swiglu_bwd_(a.gu, dact, F, interleave=self.gu_il)              # gu <- [dgate | dup] (same layout as gu)
+                if bank is not None:
+                    ops.wgrad_(a.gu, a.h2, G(l, "Wgu"), acc)
+                dh2 = self._dgrad(a.gu, W, "Wgu")                                  # [M,H]
             if bank is not None:
                 ops.col_reduce_(dy_bf16=dh2, z=a.x_mid, rstd=a.rstd2, out_prod=G(l, "g2"))
             dmid32, dmid16 = ops.rmsnorm_bwd(a.x_mid, W["g2"], a.rstd2, dh2, dres_in=dx32)

@@ -20,12 +20,16 @@ def _normal(gen: torch.Generator, shape, std: float, dtype, device) -> torch.Ten
 
 
 def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, device="cpu",
-                      bias_std: Optional[float] = None, qk_norm_std: Optional[float] = None) -> Dict[str, torch.Tensor]:
+                      bias_std: Optional[float] = None, qk_norm_std: Optional[float] = None,
+                      router_std: Optional[float] = None) -> Dict[str, torch.Tensor]:
     """HF parameter names for BertModel / XLMRobertaModel / RobertaModel / ModernBertModel (no prefix) / LlamaForCausalLM / Qwen2ForCausalLM /
     Qwen3ForCausalLM / MistralForCausalLM / FalconForCausalLM, init N(0, initializer_range), LN = (1, 0). Decoder attention biases (Qwen2's q/k/v, Llama's and Qwen3's
     `attention_bias`) are drawn from N(0, bias_std) (default: initializer_range) rather than HF's zeros, so that a dropped bias
     changes the outputs. Qwen3's q_norm / k_norm weights are 1 + N(0, qk_norm_std) (default: initializer_range), so that a
-    dropped or swapped norm shows; so are every LayerNorm weight of ModernBERT."""
+    dropped or swapped norm shows; so are every LayerNorm weight of ModernBERT. Qwen3MoeForCausalLM's sparse layers are
+    written in the hub layout (`mlp.gate.weight` [E, H], `mlp.experts.{e}.{gate,up,down}_proj.weight`), the router weights
+    drawn from N(0, router_std) (default: initializer_range): a larger std spreads the router probabilities, so that the
+    top-k choice is far from ties."""
     on_device = torch.device(device).type == "cuda" and cfg.get("_device_rng", False)
     gen = torch.Generator(device=device) if on_device else torch.Generator()
     gen.manual_seed(seed)
@@ -58,8 +62,9 @@ def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, 
             sd[p + "output.LayerNorm.bias"] = _normal(gen, (H,), std, dtype, device)
         sd["pooler.dense.weight"] = _normal(gen, (H, H), std, dtype, device)   # loaded by AutoModel, unused by the path
         sd["pooler.dense.bias"] = zeros(H)
-    elif kind in ("llama", "qwen2", "qwen3", "mistral"):
-        F, V = cfg["intermediate_size"], cfg["vocab_size"]
+    elif kind in ("llama", "qwen2", "qwen3", "mistral", "qwen3_moe"):
+        F, V = cfg.get("intermediate_size"), cfg["vocab_size"]
+        sparse = moe_layers(cfg) if kind == "qwen3_moe" else [False] * cfg["num_hidden_layers"]
         nh, nkv = cfg["num_attention_heads"], cfg.get("num_key_value_heads", cfg["num_attention_heads"])
         hd = cfg.get("head_dim") or H // nh
         qkv_bias, o_bias = attention_biases(kind, cfg)
@@ -77,13 +82,21 @@ def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, 
                 sd[p + "self_attn.v_proj.bias"] = _normal(gen, (nkv * hd,), bstd, dtype, device)
             if o_bias:
                 sd[p + "self_attn.o_proj.bias"] = _normal(gen, (H,), bstd, dtype, device)
-            if kind == "qwen3":
+            if kind in ("qwen3", "qwen3_moe"):
                 nstd = std if qk_norm_std is None else float(qk_norm_std)
                 sd[p + "self_attn.q_norm.weight"] = ones(hd) + _normal(gen, (hd,), nstd, dtype, device)
                 sd[p + "self_attn.k_norm.weight"] = ones(hd) + _normal(gen, (hd,), nstd, dtype, device)
-            sd[p + "mlp.gate_proj.weight"] = _normal(gen, (F, H), std, dtype, device)
-            sd[p + "mlp.up_proj.weight"] = _normal(gen, (F, H), std, dtype, device)
-            sd[p + "mlp.down_proj.weight"] = _normal(gen, (H, F), std, dtype, device)
+            if sparse[l]:
+                E, I = cfg["num_experts"], cfg["moe_intermediate_size"]
+                sd[p + "mlp.gate.weight"] = _normal(gen, (E, H), std if router_std is None else float(router_std), dtype, device)
+                for e in range(E):
+                    sd[p + f"mlp.experts.{e}.gate_proj.weight"] = _normal(gen, (I, H), std, dtype, device)
+                    sd[p + f"mlp.experts.{e}.up_proj.weight"] = _normal(gen, (I, H), std, dtype, device)
+                    sd[p + f"mlp.experts.{e}.down_proj.weight"] = _normal(gen, (H, I), std, dtype, device)
+            else:
+                sd[p + "mlp.gate_proj.weight"] = _normal(gen, (F, H), std, dtype, device)
+                sd[p + "mlp.up_proj.weight"] = _normal(gen, (F, H), std, dtype, device)
+                sd[p + "mlp.down_proj.weight"] = _normal(gen, (H, F), std, dtype, device)
             sd[p + "input_layernorm.weight"] = ones(H) + _normal(gen, (H,), std, dtype, device)
             sd[p + "post_attention_layernorm.weight"] = ones(H) + _normal(gen, (H,), std, dtype, device)
         sd["model.norm.weight"] = ones(H) + _normal(gen, (H,), std, dtype, device)
@@ -169,7 +182,7 @@ def model_kind(cfg: Dict) -> str:
     if mt in ("roberta", "xlm-roberta"):
         check_roberta(cfg)
         return "roberta"
-    if mt in ("llama", "qwen2", "qwen3", "mistral"):
+    if mt in ("llama", "qwen2", "qwen3", "mistral", "qwen3_moe"):
         check_llama_family(cfg)
         return mt
     if mt == "modernbert":
@@ -180,7 +193,7 @@ def model_kind(cfg: Dict) -> str:
         return "falcon"
     raise NotImplementedError(
         f"model_type {mt!r} is not built in dalm_b200 (supported: bert, roberta, xlm-roberta and modernbert encoders; llama, "
-        "qwen2, qwen3, mistral and falcon decoders)")
+        "qwen2, qwen3, qwen3_moe, mistral and falcon decoders)")
 
 
 def _rope_type(cfg: Dict) -> str:
@@ -257,10 +270,16 @@ def check_llama_family(cfg: Dict) -> None:
         check_rope_type(cfg)
     if mt != "mistral" and cfg.get("mlp_bias", False):        # MistralMLP has no bias whatever the key says
         raise NotImplementedError(f"{mt}: mlp_bias=true is not built (the fused SwiGLU MLP has no bias)")
-    if mt == "qwen3":
+    if mt == "qwen3_moe":
+        check_qwen3_moe(cfg)
+    if mt in ("qwen3", "qwen3_moe"):
         hd = cfg.get("head_dim") or cfg["hidden_size"] // cfg["num_attention_heads"]
         if hd != 128:
-            raise NotImplementedError(f"qwen3: head_dim={hd} is not built (the q/k norm kernels take head_dim 128)")
+            raise NotImplementedError(f"{mt}: head_dim={hd} is not built (the q/k norm kernels take head_dim 128)")
+    if mt == "qwen3_moe":
+        rt = _rope_type(cfg)
+        if rt != "default":
+            raise NotImplementedError(f"{mt}: RoPE type {rt!r} (rope_scaling / rope_parameters) is not built; only 'default'")
     if mt in ("qwen2", "qwen3"):
         if not cfg.get("use_sliding_window", False) and "sliding_attention" in (cfg.get("layer_types") or ()):
             # transformers then sets sliding_window to None but still builds sliding-window masks for those layers
@@ -278,6 +297,46 @@ def check_llama_family(cfg: Dict) -> None:
             raise NotImplementedError(f"{mt}: RoPE type {rt!r} (rope_scaling / rope_parameters) is not built; only 'default'")
 
 
+# Qwen3-MoE: the keys without which transformers would fill in Qwen3MoeConfig's 30B-A3B defaults (the shape is read from
+# config.json only), and the bounds of the routing kernels (csrc/moe.cu) and of the gate GEMM (N = E, then K = E: % 8)
+QWEN3_MOE_KEYS = ("num_experts", "num_experts_per_tok", "moe_intermediate_size")
+MOE_MAX_EXPERTS, MOE_MAX_TOPK = 256, 16
+
+
+def check_qwen3_moe(cfg: Dict) -> None:
+    """refuses a qwen3_moe config the routed MLP would otherwise compute wrong or cannot run"""
+    missing = [k for k in QWEN3_MOE_KEYS if k not in cfg]
+    if missing:
+        raise NotImplementedError(f"qwen3_moe: a config without {', '.join(missing)} is not built (transformers would fill in "
+                                  "Qwen3MoeConfig's defaults, the 30B-A3B shape; the shape is read from config.json only)")
+    E, k, I = int(cfg["num_experts"]), int(cfg["num_experts_per_tok"]), int(cfg["moe_intermediate_size"])
+    if E > 0:
+        if E % 8 or E > MOE_MAX_EXPERTS:
+            raise NotImplementedError(f"qwen3_moe: num_experts={E} is not built (the router kernels take a multiple of 8 up to "
+                                      f"{MOE_MAX_EXPERTS})")
+        if not 1 <= k <= min(E, MOE_MAX_TOPK):
+            raise NotImplementedError(f"qwen3_moe: num_experts_per_tok={k} is not built (the router takes 1 to "
+                                      f"min(num_experts, {MOE_MAX_TOPK}))")
+        if I <= 0 or I % 128:
+            raise NotImplementedError(f"qwen3_moe: moe_intermediate_size={I} is not built (the grouped SwiGLU GEMM takes a "
+                                      "multiple of 128: 128-feature gate / up blocks)")
+        if cfg["hidden_size"] % 64:
+            raise NotImplementedError(f"qwen3_moe: hidden_size={cfg['hidden_size']} is not built (the experts' down-projection "
+                                      "dgrad takes a multiple of 64)")
+    if not all(moe_layers(cfg)) and "intermediate_size" not in cfg:
+        raise NotImplementedError("qwen3_moe: dense MLP layers (mlp_only_layers / decoder_sparse_step) need intermediate_size "
+                                  "in config.json")
+
+
+def moe_layers(cfg: Dict) -> List[bool]:
+    """which layers of a qwen3_moe config run the routed MLP, as Qwen3MoeDecoderLayer decides: not in `mlp_only_layers`,
+    num_experts > 0 and (i + 1) % decoder_sparse_step == 0; the others run the dense SwiGLU MLP of `intermediate_size`"""
+    n = int(cfg["num_hidden_layers"])
+    only = set(cfg.get("mlp_only_layers") or ())
+    step = int(cfg.get("decoder_sparse_step", 1))
+    return [i not in only and int(cfg.get("num_experts", 0)) > 0 and (i + 1) % step == 0 for i in range(n)]
+
+
 MISTRAL_DEFAULT_WINDOW = 4096                                    # MistralConfig's sliding_window when the key is absent
 MISTRAL_SHAPE_KEYS = ("hidden_size", "intermediate_size", "num_hidden_layers", "num_attention_heads", "vocab_size")
 
@@ -288,11 +347,16 @@ def sliding_windows(cfg: Dict) -> List[int]:
       `layer_types` (alternating layers are Ministral, another model type), and so does this.
     - qwen2 / qwen3: `sliding_window` only with `use_sliding_window`, on the layers `layer_types` marks "sliding_attention",
       or when that list is absent on layers i >= `max_window_layers` (default 28).
+    - qwen3_moe: `sliding_window` (default 4096) on every layer when `use_sliding_window`, as Qwen3MoeConfig and its
+      attention read it (no `max_window_layers` or `layer_types`).
     - llama: none.
     A layer with window w lets query i see key j iff i - w < j <= i, in the indices of the padded row."""
     mt, n = cfg.get("model_type", ""), int(cfg["num_hidden_layers"])
     if mt == "mistral":
         w = cfg.get("sliding_window", MISTRAL_DEFAULT_WINDOW)
+        return [int(w) if w else 0] * n
+    if mt == "qwen3_moe":
+        w = cfg.get("sliding_window", 4096) if cfg.get("use_sliding_window", False) else 0
         return [int(w) if w else 0] * n
     if mt in ("qwen2", "qwen3"):
         w = cfg.get("sliding_window", 4096)
@@ -401,6 +465,7 @@ def attention_biases(kind: str, cfg: Dict):
         return True, False
     if kind == "mistral":
         return False, False
+    # qwen3_moe: Qwen3MoeAttention, Qwen3's attention (`attention_bias` on all four projections)
     ab = bool(cfg.get("attention_bias", False))
     return ab, ab
 

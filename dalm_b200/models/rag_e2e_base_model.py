@@ -114,6 +114,17 @@ def _named(engine_model, name_or_path: str):
     return engine_model
 
 
+def _check_qwen3_moe_mode(full: bool, bnb: bool) -> None:
+    """Qwen3-MoE generators run frozen or with LoRA on q_proj / v_proj; every other mode is refused, naming why"""
+    if full:
+        raise NotImplementedError("full fine-tuning of a qwen3_moe generator is not built: grouped expert weight gradients are "
+                                  "not built, and at ~18 bytes per parameter (fp32 master, gradient, Adam moments, bf16 copy) "
+                                  "Qwen3-30B-A3B would need ~550 GB; use LoRA (use_peft) on the generator")
+    if bnb:
+        raise NotImplementedError("use_bnb on a qwen3_moe generator is not built: the 4-bit treatment of the fused 3-D expert "
+                                  "weights differs across transformers versions, so no single reference exists to match")
+
+
 def _nf4_storage(bnb: bool, full: bool, kind: str) -> bool:
     """use_bnb + DALM_B200_NF4_STORAGE=1: keep the sub-model's Linear weights as packed NF4 codes and expand them per use
     (engine/nf4store.py) instead of the dequantised-resident default. BERT / (XLM-)RoBERTa encoders and Llama decoders."""
@@ -151,13 +162,15 @@ def build_decoder(name_or_path: str, lora: bool, device: torch.device, state_dic
                   cfg: Optional[Dict] = None, full: bool = False, bnb: bool = False) -> LlamaDecoder:
     cfg = cfg or params.load_config(name_or_path)
     kind = params.model_kind(cfg)                # raises for unsupported families
+    if kind == "qwen3_moe":
+        _check_qwen3_moe_mode(full, bnb)
     sd = state_dict if state_dict is not None else params.load_state_dict(name_or_path)
     nf4 = _nf4_storage(bnb, full, kind)
     if not nf4:
         sd = _maybe_bnb(sd, bnb, full, device)
     if kind == "falcon":
         dec = FalconDecoder(cfg, sd, device=device, lora=lora, full=full)      # raises for lora=True, like peft would
-    elif kind not in ("llama", "qwen2", "qwen3", "mistral"):
+    elif kind not in ("llama", "qwen2", "qwen3", "mistral", "qwen3_moe"):
         raise NotImplementedError(f"generator of kind {kind!r} is not a causal decoder")
     else:
         dec = LlamaDecoder(cfg, sd, device=device, lora=lora, full=full, nf4_storage=nf4)

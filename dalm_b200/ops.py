@@ -1095,3 +1095,152 @@ def sample_step_(logits, V: int, eos_ids, pad_id: int, unfinished, tokens, mask,
             raise _lib.DalmB200Error("sample_step: scores_out must be fp32 [B, >=V] with the logits' row stride")
     _lib.call("dalm_b200_sample_step", *args, float(temperature), int(top_k), float(top_p), int(seed) & (2**64 - 1), _p(u),
               _p(scores_out), _stream())
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# routed mixture-of-experts MLP (Qwen3-MoE)
+# ----------------------------------------------------------------------------------------------------------------
+i32 = torch.int32
+
+
+def moe_tiles(pairs: int, E: int) -> int:
+    """static bound of 128-row M tiles over `pairs` (token, slot) pairs whose E expert segments are each padded to the tile"""
+    return (pairs + 127 * E + 127) // 128
+
+
+def _dense_experts(w: torch.Tensor, name: str) -> None:
+    _chk(w, bf16, name)
+    if w.dim() != 3 or not w.is_contiguous():
+        raise _lib.DalmB200Error(f"{name}: expected a dense bf16 [E, rows, cols] stack, got shape {tuple(w.shape)} strides {w.stride()}")
+
+
+def gemm_grouped(a: torch.Tensor, w: torch.Tensor, tile_expert: torch.Tensor, live: torch.Tensor, out: Optional[torch.Tensor] = None,
+                 *, layout: int = 0, swiglu: bool = False, act: Optional[torch.Tensor] = None, max_ctas: int = 0):
+    """grouped GEMM over experts: row block m // 128 of `a` (bf16 [rows, K], rows = 128 n_tiles) is multiplied by expert
+    e = tile_expert[m // 128]: layout 0 out = a @ w[e]^T (w [E, N, K]), layout 1 out = a @ w[e] (w [E, K, N]). Only the first
+    live[0] tiles are computed; the rest of `out` is left as it was. swiglu: w[e] holds interleaved gate / up rows
+    (`interleave_gate_up`) -> (gu [rows, N], act [rows, N / 2] = silu(gate) * up)."""
+    _chk(a, bf16, "gemm_grouped a")
+    _dense_experts(w, "gemm_grouped w")
+    _vec(live, i32, "gemm_grouped live", 1)
+    M, K = a.shape
+    E = w.shape[0]
+    N = w.shape[1] if layout == 0 else w.shape[2]
+    if (w.shape[2] if layout == 0 else w.shape[1]) != K:
+        raise _lib.DalmB200Error(f"gemm_grouped: a is [{M}, {K}] but w is {tuple(w.shape)} (layout {layout})")
+    _vec(tile_expert, i32, "gemm_grouped tile_expert", (M + 127) // 128)
+    if out is None:
+        out = torch.empty(M, N, dtype=bf16, device=a.device)
+    _bf16_rows(out, "gemm_grouped out", M, N)
+    if swiglu and act is None:
+        act = torch.empty(M, N // 2, dtype=bf16, device=a.device)
+    if act is not None:
+        _bf16_rows(act, "gemm_grouped act", M, N // 2)
+    if max_ctas == 0 and GEMM_MAX_CTAS:
+        max_ctas = GEMM_MAX_CTAS
+    _lib.call("dalm_b200_gemm_bf16_grouped", int(layout), 1 if swiglu else 0, _p(a), _ld(a), _p(w), E, _p(out), _ld(out),
+              _p(act), _ld(act) if act is not None else 0, M, N, K, _p(tile_expert), _p(live), int(max_ctas), _stream())
+    return (out, act) if swiglu else out
+
+
+class MoeRouting:
+    """where each (token, slot) pair of a routed batch sits in the expert-sorted, tile-padded rows (see moe_permute)"""
+    __slots__ = ("M", "k", "E", "n_tiles", "counts", "seg_off", "tile_expert", "live", "pair_row", "row_pair", "chunk_counts")
+
+    def __init__(self, M: int, k: int, E: int, device, n_tiles: Optional[int] = None):
+        P = M * k
+        self.M, self.k, self.E = M, k, E
+        self.n_tiles = moe_tiles(P, E) if n_tiles is None else n_tiles
+        z = lambda n: torch.empty(n, dtype=i32, device=device)
+        self.counts, self.seg_off, self.tile_expert, self.live = z(E), z(E + 1), z(self.n_tiles), z(1)
+        self.pair_row, self.row_pair = z(P), z(128 * self.n_tiles)
+        self.chunk_counts = z(-(-P // 1024) * E)
+
+    @property
+    def rows(self) -> int:
+        return 128 * self.n_tiles
+
+
+def moe_router(logits: torch.Tensor, k: int, norm_topk: bool, ids: Optional[torch.Tensor] = None, w: Optional[torch.Tensor] = None):
+    """fp32 router logits [M, E] -> (ids int32 [M, k], weights fp32 [M, k]): softmax, top-k, renormalised when norm_topk"""
+    _chk(logits, f32, "moe_router logits")
+    M, E = logits.shape
+    ids = torch.empty(M, k, dtype=i32, device=logits.device) if ids is None else ids
+    w = torch.empty(M, k, dtype=f32, device=logits.device) if w is None else w
+    _vec(ids, i32, "moe_router ids", M * k); _vec(w, f32, "moe_router w", M * k)
+    _lib.call("dalm_b200_moe_router", _p(logits), _ld(logits), M, E, int(k), int(bool(norm_topk)), _p(ids), _p(w), _stream())
+    return ids, w
+
+
+def moe_router_bwd(logits: torch.Tensor, ids: torch.Tensor, w: torch.Tensor, dw: torch.Tensor, norm_topk: bool,
+                   out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """d(router logits) as bf16 [M, E] (the operand of dh += dlogits @ W_gate) from d(routing weights) fp32 [M, k]"""
+    _chk(logits, f32, "moe_router_bwd logits")
+    M, E = logits.shape
+    k = ids.shape[-1]
+    for t, dt, nm in ((ids, i32, "ids"), (w, f32, "w"), (dw, f32, "dw")):
+        _vec(t, dt, f"moe_router_bwd {nm}", M * k)
+    out = torch.empty(M, E, dtype=bf16, device=logits.device) if out is None else out
+    _bf16_rows(out, "moe_router_bwd out", M, E)
+    _lib.call("dalm_b200_moe_router_bwd", _p(logits), _ld(logits), _p(ids), _p(w), _p(dw), M, E, int(k), int(bool(norm_topk)),
+              _p(out), _ld(out), _stream())
+    return out
+
+
+def moe_permute(ids: torch.Tensor, E: int, routing: Optional[MoeRouting] = None) -> MoeRouting:
+    """expert-sorted, tile-padded placement of the pairs of ids (int32 [M, k]); `routing` is reused when given (a captured
+    step keeps its buffers)"""
+    M, k = ids.shape
+    r = MoeRouting(M, k, E, ids.device) if routing is None else routing
+    if (r.M, r.k, r.E) != (M, k, E):
+        raise _lib.DalmB200Error(f"moe_permute: routing buffers are for M={r.M} k={r.k} E={r.E}, not M={M} k={k} E={E}")
+    _vec(ids, i32, "moe_permute ids", M * k)
+    _lib.call("dalm_b200_moe_permute", _p(ids), M * k, E, r.n_tiles, _p(r.chunk_counts), _p(r.counts), _p(r.seg_off),
+              _p(r.tile_expert), _p(r.live), _p(r.pair_row), _p(r.row_pair), _stream())
+    return r
+
+
+def moe_gather(x: torch.Tensor, r: MoeRouting, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """rows [r.rows, H] (bf16): each live row holds its token's row of x (bf16 or fp32), padding rows 0"""
+    if x.dtype not in (bf16, f32):
+        raise _lib.DalmB200Error("moe_gather: x must be bf16 or fp32")
+    _chk(x, x.dtype, "moe_gather x")
+    H = x.shape[1]
+    out = torch.empty(r.rows, H, dtype=bf16, device=x.device) if out is None else out
+    _bf16_rows(out, "moe_gather out", r.rows, H)
+    _lib.call("dalm_b200_moe_gather", _p(x), _ld(x), 1 if x.dtype == f32 else 0, H, _p(r.row_pair), r.k, _p(r.live), r.rows,
+              _p(out), _ld(out), _stream())
+    return out
+
+
+def moe_combine(y: torch.Tensor, r: MoeRouting, w: Optional[torch.Tensor], resid: Optional[torch.Tensor] = None,
+                out: Optional[torch.Tensor] = None, out_dtype=f32) -> torch.Tensor:
+    """out[t] = resid[t] + sum_s w[t, s] y[row(t, s)] (fp32 sums, slots in order); w None = weights of 1. resid / out: fp32
+    or bf16 [M, H] of one dtype; resid may be out itself."""
+    _chk(y, bf16, "moe_combine y")
+    H = y.shape[1]
+    if out is None:
+        out = torch.empty(r.M, H, dtype=resid.dtype if resid is not None else out_dtype, device=y.device)
+    if out.dtype not in (bf16, f32) or (resid is not None and resid.dtype != out.dtype):
+        raise _lib.DalmB200Error("moe_combine: out and resid must both be bf16 or both fp32")
+    _chk(out, out.dtype, "moe_combine out")
+    if resid is not None:
+        _chk(resid, resid.dtype, "moe_combine resid")
+    if w is not None:
+        _vec(w, f32, "moe_combine w", r.M * r.k)
+    _lib.call("dalm_b200_moe_combine", _p(y), _ld(y), _p(r.pair_row), _p(w), r.M, r.k, H, _p(resid),
+              _ld(resid) if resid is not None else 0, _p(out), _ld(out), 1 if out.dtype == f32 else 0, _stream())
+    return out
+
+
+def moe_down_bwd(da: torch.Tensor, act: torch.Tensor, r: MoeRouting, w: torch.Tensor, d_act: Optional[torch.Tensor] = None):
+    """-> (dw fp32 [M, k] = <da[row], act[row]>, d_act bf16 [rows, I] = w da[row] on the live rows)"""
+    _chk(da, bf16, "moe_down_bwd da"); _chk(act, bf16, "moe_down_bwd act")
+    _vec(w, f32, "moe_down_bwd w", r.M * r.k)
+    I = act.shape[1]
+    d_act = torch.empty(r.rows, I, dtype=bf16, device=da.device) if d_act is None else d_act
+    _bf16_rows(d_act, "moe_down_bwd d_act", r.rows, I)
+    dw = torch.empty(r.M, r.k, dtype=f32, device=da.device)
+    _lib.call("dalm_b200_moe_down_bwd", _p(da), _ld(da), _p(act), _ld(act), _p(r.pair_row), _p(w), r.M * r.k, I, _p(dw),
+              _p(d_act), _ld(d_act), _stream())
+    return dw, d_act

@@ -83,6 +83,22 @@ QWEN3_SHAPES: Dict[str, Dict] = {
                      intermediate_size=12288, tie_word_embeddings=False),
 }
 
+# Qwen3-MoE (HF Qwen3MoeForCausalLM): Qwen3 attention, routed SwiGLU experts on the sparse layers (params.moe_layers)
+QWEN3_MOE_SHAPES: Dict[str, Dict] = {
+    # layer 1 of 3 dense (mlp_only_layers); 5 q|k heads: q/k norm + RoPE in the row kernel
+    "qwen3-moe-tiny": dict(hidden_size=384, num_hidden_layers=3, num_attention_heads=4, num_key_value_heads=1,
+                           intermediate_size=768, num_experts=8, num_experts_per_tok=2, moe_intermediate_size=128,
+                           mlp_only_layers=[1], norm_topk_prob=True, tie_word_embeddings=True),
+    # 8 q|k heads: q/k norm + RoPE in the QKV epilogue; every layer sparse, weights not renormalised
+    "qwen3-moe-hd128": dict(hidden_size=512, num_hidden_layers=2, num_attention_heads=6, num_key_value_heads=2,
+                            intermediate_size=1024, num_experts=16, num_experts_per_tok=4, moe_intermediate_size=256,
+                            mlp_only_layers=[], norm_topk_prob=False, tie_word_embeddings=False),
+    # published Qwen/Qwen3-30B-A3B config.json values (written from the model card; not re-fetched offline)
+    "qwen3-30b-a3b": dict(hidden_size=2048, num_hidden_layers=48, num_attention_heads=32, num_key_value_heads=4,
+                          intermediate_size=6144, num_experts=128, num_experts_per_tok=8, moe_intermediate_size=768,
+                          mlp_only_layers=[], norm_topk_prob=True, tie_word_embeddings=False),
+}
+
 
 # XLM-RoBERTa / RoBERTa encoders: BERT's layer, positions counted from pad_token_id + 1
 ROBERTA_SHAPES: Dict[str, Dict] = {
@@ -261,6 +277,19 @@ def qwen3_config(name: str, vocab_size: int = 151936) -> Dict:
         hidden_act="silu", rms_norm_eps=1e-6, rope_theta=1000000.0, rope_scaling=None, initializer_range=0.02, bos_token_id=0,
         eos_token_id=0, head_dim=128, attention_bias=False, attention_dropout=0.0, use_sliding_window=False, sliding_window=None,
         max_window_layers=s["num_hidden_layers"], **s,
+    )
+
+
+def qwen3_moe_config(name: str, vocab_size: int = 151936) -> Dict:
+    """Qwen3-MoE (HF Qwen3MoeForCausalLM): qwen3_config's attention and norms; the sparse layers route each token to its top
+    num_experts_per_tok of num_experts SwiGLU experts (moe_intermediate_size), decoder_sparse_step 1. No sliding window."""
+    s = dict(QWEN3_MOE_SHAPES[name])
+    return dict(
+        architectures=["Qwen3MoeForCausalLM"], model_type="qwen3_moe", vocab_size=vocab_size, max_position_embeddings=40960,
+        hidden_act="silu", rms_norm_eps=1e-6, rope_theta=1000000.0, rope_scaling=None, initializer_range=0.02, bos_token_id=0,
+        eos_token_id=0, head_dim=128, attention_bias=False, attention_dropout=0.0, use_sliding_window=False, sliding_window=None,
+        max_window_layers=s["num_hidden_layers"], decoder_sparse_step=1, output_router_logits=False,
+        router_aux_loss_coef=0.001, **s,
     )
 
 
@@ -543,14 +572,16 @@ QWEN3_GENERATION = {
 # ---------------------------------------------------------------------------------------------------------------
 def write_model_dir(out_dir: str, kind: str, name: str, vocab_size: Optional[int] = None, with_weights: bool = True,
                     seed: int = 0, generation_config: Optional[Dict] = None, bias_std: Optional[float] = None,
-                    qk_norm_std: Optional[float] = None, headless: Optional[bool] = None) -> str:
+                    qk_norm_std: Optional[float] = None, headless: Optional[bool] = None,
+                    router_std: Optional[float] = None) -> str:
     """kind: 'bert' | 'roberta' | 'modernbert' | 'llama' | 'qwen2' | 'qwen3' | 'mistral' | 'falcon' ('roberta' takes a ROBERTA_SHAPES name: XLM-R
     shapes get the XLM-R tokenizer, roberta-tiny the byte-level one; a Llama 3.x shape of LLAMA3_SHAPES takes kind 'llama' and
     gets the Llama 3 tokenizer; 'mistral' gets the Llama SentencePiece tokenizer). headless (mistral; default: the shape's own
     setting): a MistralModel directory, weights without the `model.` prefix and without lm_head. Writes config.json, tokenizer files and (optionally) seeded random-init
     safetensors in HF parameter naming so both transformers (oracle) and dalm_b200 (product) can load the same directory.
     generation_config: written as generation_config.json when given (e.g. QWEN2_GENERATION["base"]). bias_std: std of the
-    random attention biases, qk_norm_std the spread of Qwen3's q / k norm weights around 1 (engine/params.random_state_dict)."""
+    random attention biases, qk_norm_std the spread of Qwen3's q / k norm weights around 1, router_std the std of Qwen3-MoE's
+    router weights (engine/params.random_state_dict). 'qwen3_moe' takes a QWEN3_MOE_SHAPES name and Qwen2's tokenizer."""
     os.makedirs(out_dir, exist_ok=True)
     if kind == "bert":
         cfg = bert_config(name, vocab_size or 30522)
@@ -573,6 +604,9 @@ def write_model_dir(out_dir: str, kind: str, name: str, vocab_size: Optional[int
     elif kind == "qwen3":
         cfg = qwen3_config(name, vocab_size or 151936)
         build_qwen2_tokenizer(out_dir, cfg["vocab_size"])          # Qwen3 keeps Qwen2's byte-level BPE and Qwen2Tokenizer
+    elif kind == "qwen3_moe":
+        cfg = qwen3_moe_config(name, vocab_size or 151936)
+        build_qwen2_tokenizer(out_dir, cfg["vocab_size"])
     elif kind == "mistral":
         cfg = mistral_config(name, vocab_size)
         if headless is not None:
@@ -600,7 +634,8 @@ def write_model_dir(out_dir: str, kind: str, name: str, vocab_size: Optional[int
 
         from .engine.params import random_state_dict
 
-        sd = random_state_dict(kind, cfg, seed=seed, dtype=torch.float32, device="cpu", bias_std=bias_std, qk_norm_std=qk_norm_std)
+        sd = random_state_dict(kind, cfg, seed=seed, dtype=torch.float32, device="cpu", bias_std=bias_std, qk_norm_std=qk_norm_std,
+                               router_std=router_std)
         if cfg.get("architectures") == ["MistralModel"]:
             sd = headless_state_dict(sd)
         save_file({k: v.contiguous() for k, v in sd.items()}, os.path.join(out_dir, "model.safetensors"))

@@ -303,6 +303,45 @@ int dalm_b200_sample_step(const void* logits, long long ld, int B, int V, const 
                           int col, int* cur_dev, int T, int64_t* next_ids, int64_t* pos, int* alive, float temperature,
                           int top_k, float top_p, unsigned long long seed, const double* u, float* scores_out, void* stream);
 
+
+/* ---- routed mixture-of-experts MLP (Qwen3-MoE Qwen3MoeSparseMoeBlock: softmax router, top-k, SwiGLU experts) ----
+ * The experts run as grouped GEMMs over rows permuted so that each expert's (token, slot) pairs are contiguous, in pair order
+ * (by token, then slot), each segment padded to the 128-row M tile. Nothing needs a host synchronisation: the live M-tile
+ * count stays in device memory and every launch is sized for the static bound of n_tiles = ceil((P + 127 E) / 128) tiles,
+ * P = M k pairs. No floating-point atomics: every result is the same bits from run to run.
+ * gemm_bf16_grouped: out[M,N] (bf16) = A[M,K] B[e]^T (layout 0, B dense [E, N, K]) or A[M,K] B[e] (layout 1, B dense
+ *   [E, K, N], K % 64 == 0: the down / gate|up dgrads read the forward weights, no transposed copy), e = tile_expert[m / 128];
+ *   only the first *live_tiles M tiles run. swiglu = 1 (layout 0, N % 256 == 0): B[e]'s gate / up rows interleaved in
+ *   128-feature blocks, out = gate|up and out2 [M, N/2] = silu(gate) * up, as gemm_bf16_swiglu. max_ctas: 0 = all SMs. */
+int dalm_b200_gemm_bf16_grouped(int layout, int swiglu, const void* A, long long lda, const void* B, int E, void* out,
+                                long long ldo, void* out2, long long ldo2, int M, int N, int K, const int* tile_expert,
+                                const int* live_tiles, int max_ctas, void* stream);
+/* moe_router: fp32 logits [M, E] (row stride ld) -> softmax (fp32) -> top-k by logit (descending, ties to the lower index):
+ *   ids int32 [M, k], w fp32 [M, k] = the probabilities, divided by their sum when norm_topk. E <= 256, k <= min(E, 16). */
+int dalm_b200_moe_router(const float* logits, long long ld, int M, int E, int k, int norm_topk, int* ids, float* w, void* stream);
+/* moe_router_bwd: dlogits (bf16 [M, E], row stride ldd) from dw (fp32 [M, k]) through the renormalisation, the top-k
+ *   selection (ids) and the softmax, recomputed from the logits. */
+int dalm_b200_moe_router_bwd(const float* logits, long long ld, const int* ids, const float* w, const float* dw, int M, int E,
+                             int k, int norm_topk, void* dlogits, long long ldd, void* stream);
+/* moe_permute: ids int32 [P] -> counts [E], seg_off [E + 1] (padded row offsets), tile_expert [n_tiles] (-1 after the live
+ *   tiles), live [1] (live M tiles), pair_row [P] (row of each pair; -1 for an id outside [0, E)), row_pair [128 n_tiles]
+ *   (pair of each live row, -1 on padding rows). chunk_counts: int32 workspace [ceil(P / 1024) E]. */
+int dalm_b200_moe_permute(const int* ids, int P, int E, int n_tiles, int* chunk_counts, int* counts, int* seg_off,
+                          int* tile_expert, int* live, int* pair_row, int* row_pair, void* stream);
+/* moe_gather: out[r] (bf16 [n_rows, H]) = x[row_pair[r] / k] (bf16, or fp32 when x_f32), 0 on padding rows; rows from
+ *   128 *live on are not written. */
+int dalm_b200_moe_gather(const void* x, long long ldx, int x_f32, int H, const int* row_pair, int k, const int* live, int n_rows,
+                         void* out, long long ldo, void* stream);
+/* moe_combine: out[t] = resid[t] + sum_s w[t, s] y[pair_row[t, s]] in fp32, slots in order; y bf16 [rows, H]; resid / out
+ *   fp32 when f32 else bf16 [M, H], resid may alias out or be NULL; w NULL = weights of 1 (the sum of a token's k rows of
+ *   the gate|up dgrad). */
+int dalm_b200_moe_combine(const void* y, long long ldy, const int* pair_row, const float* w, int M, int k, int H, const void* resid,
+                          long long ldr, void* out, long long ldo, int f32, void* stream);
+/* moe_down_bwd: per pair p with row r = pair_row[p]: dw[p] = <da[r], act[r]> (fp32) and d_act[r] = w[p] da[r] (bf16; d_act may
+ *   be act itself), where
+ *   da = dy_rows W_down[e] is the down projection's dgrad of the token's unweighted output gradient. */
+int dalm_b200_moe_down_bwd(const void* da, long long ldda, const void* act, long long ldact, const int* pair_row, const float* w,
+                           int P, int I, float* dw, void* d_act, long long ldd, void* stream);
 #ifdef __cplusplus
 }
 #endif

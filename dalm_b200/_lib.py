@@ -82,6 +82,11 @@ SIGNATURES = {
     "dalm_b200_rope_pos": [_P, _L, _I, _I, _I, _P, _P, _P, _I, _I, _P],
     "dalm_b200_qk_norm_rope": [_P, _L, _I, _I, _P, _P, _F, _P, _P, _I, _I, _P, _I, _P, _L, _P, _L, _P],
     "dalm_b200_qk_norm_rope_bwd": [_P, _L, _I, _I, _P, _P, _P, _P, _I, _P, _L, _P, _L, _I, _P, _P, _P],
+    "dalm_b200_qk_fullnorm_rope": [_P, _L, _I, _I, _I, _P, _P, _F, _I, _P, _P, _I, _I, _P, _I, _P, _L, _P, _L, _P],
+    "dalm_b200_qk_fullnorm_rope_bwd": [_P, _L, _I, _I, _I, _P, _P, _P, _P, _I, _P, _L, _P, _L, _I, _P],
+    "dalm_b200_norm_wgrad": [_P, _I, _L, _P, _L, _P, _L, _I, _I, _I, _P, _P, _I, _I, _P, _I, _P, _P, _P],
+    "dalm_b200_postnorm_fwd": [_P, _L, _P, _P, _P, _P, _L, _P, _I, _I, _F, _P],
+    "dalm_b200_postnorm_bwd": [_P, _L, _P, _P, _P, _P, _L, _P, _P, _L, _I, _I, _P],
     "dalm_b200_attention_decode": [_P, _L, _I, _I, _I, _P, _P, _L, _L, _P, _L, _P, _L, _I, _I, _I, _I, _I, _P, _I, _F, _I, _P],
     "dalm_b200_greedy_step": [_P, _L, _I, _I, _P, _I, _L, _P, _P, _L, _P, _L, _I, _P, _I, _P, _P, _P, _P],
     "dalm_b200_sample_step": [_P, _L, _I, _I, _P, _I, _L, _P, _P, _L, _P, _L, _I, _P, _I, _P, _P, _P, _F, _I, _F, _U, _P, _P, _P],

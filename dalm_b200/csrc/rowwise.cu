@@ -267,6 +267,125 @@ __global__ void __launch_bounds__(256) rmsnorm_bwd_kernel(const float* __restric
 }
 
 // ------------------------------------------------------------------------------------------------------------
+// OLMo 2 / OLMo 3 post-sublayer RMSNorm with the residual add (transformers Olmo2DecoderLayer: x + post_norm(sublayer(x))):
+//   forward:  out (fp32) = resid + bf16(w * (y * rstd)),  rstd = rsqrt(mean(y^2) + eps),  y = the bf16 o_proj / down output;
+//             out16 (optional) = bf16(out), the next GEMM's operand
+//   backward: d = dres_in (+ dh, the bf16 gradient of the sublayer below that joins the residual stream here) -> dres_out = d
+//             (the residual gradient passes on unchanged) and dy (bf16) = rstd (w d - y_hat mean(w d y_hat)), y_hat = y rstd
+// One CTA per row; each thread holds up to kPostNormUnits 8-column units of the row in registers (H <= 8192, H % 8 == 0).
+// ------------------------------------------------------------------------------------------------------------
+constexpr int kPostNormUnits = 4;
+
+__device__ __forceinline__ void ld_bf16x8(const __nv_bfloat16* p, float* v) {
+  const uint4 raw = *reinterpret_cast<const uint4*>(p);
+  const uint32_t w[4] = {raw.x, raw.y, raw.z, raw.w};
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w[e]));
+    v[2 * e] = f.x; v[2 * e + 1] = f.y;
+  }
+}
+__device__ __forceinline__ void st_bf16x8(__nv_bfloat16* p, const float* v) {
+  uint32_t w[4];
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    __nv_bfloat162 t = __floats2bfloat162_rn(v[2 * e], v[2 * e + 1]);
+    w[e] = *reinterpret_cast<uint32_t*>(&t);
+  }
+  *reinterpret_cast<uint4*>(p) = make_uint4(w[0], w[1], w[2], w[3]);
+}
+__device__ __forceinline__ void ld_f32x8(const float* p, float* v) {
+  const float4 a = *reinterpret_cast<const float4*>(p), b = *reinterpret_cast<const float4*>(p + 4);
+  v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+}
+__device__ __forceinline__ void st_f32x8(float* p, const float* v) {
+  *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]);
+  *reinterpret_cast<float4*>(p + 4) = make_float4(v[4], v[5], v[6], v[7]);
+}
+
+__global__ void __launch_bounds__(256) postnorm_fwd_kernel(const __nv_bfloat16* __restrict__ y, long long ldy,
+                                                           const float* __restrict__ w, const float* __restrict__ resid,
+                                                           float* __restrict__ out, __nv_bfloat16* __restrict__ out16, long long ld16,
+                                                           float* __restrict__ rstd_out, int H, float eps) {
+  __shared__ float red[32];
+  const size_t r = blockIdx.x;
+  const int units = H / 8;
+  float v[kPostNormUnits][8];
+  float q = 0.f;
+#pragma unroll
+  for (int k = 0; k < kPostNormUnits; ++k) {
+    const int i = threadIdx.x + k * 256;
+    if (i < units) {
+      ld_bf16x8(y + r * ldy + i * 8, v[k]);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) q = fmaf(v[k][e], v[k][e], q);
+    }
+  }
+  const float rstd = rsqrtf(block_sum(q, red) / H + eps);
+  if (threadIdx.x == 0) rstd_out[r] = rstd;
+#pragma unroll
+  for (int k = 0; k < kPostNormUnits; ++k) {
+    const int i = threadIdx.x + k * 256;
+    if (i < units) {
+      float ww[8], x[8];
+      ld_f32x8(w + i * 8, ww);
+      ld_f32x8(resid + r * H + i * 8, x);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) x[e] += __bfloat162float(__float2bfloat16_rn(ww[e] * (v[k][e] * rstd)));
+      st_f32x8(out + r * H + i * 8, x);
+      if (out16 != nullptr) st_bf16x8(out16 + r * ld16 + i * 8, x);
+    }
+  }
+}
+
+__global__ void __launch_bounds__(256) postnorm_bwd_kernel(const __nv_bfloat16* __restrict__ y, long long ldy,
+                                                           const float* __restrict__ w, const float* __restrict__ rstd_in,
+                                                           const float* __restrict__ dres_in, const __nv_bfloat16* __restrict__ dh,
+                                                           long long lddh, float* __restrict__ dres_out,
+                                                           __nv_bfloat16* __restrict__ dy, long long lddy, int H) {
+  __shared__ float red[32];
+  const size_t r = blockIdx.x;
+  const int units = H / 8;
+  const float rstd = rstd_in[r];
+  float wd[kPostNormUnits][8], yh[kPostNormUnits][8];
+  float s = 0.f;
+#pragma unroll
+  for (int k = 0; k < kPostNormUnits; ++k) {
+    const int i = threadIdx.x + k * 256;
+    if (i < units) {
+      float d[8], ww[8];
+      ld_f32x8(dres_in + r * H + i * 8, d);
+      if (dh != nullptr) {
+        float t[8];
+        ld_bf16x8(dh + r * lddh + i * 8, t);
+#pragma unroll
+        for (int e = 0; e < 8; ++e) d[e] += t[e];
+      }
+      st_f32x8(dres_out + r * H + i * 8, d);
+      ld_f32x8(w + i * 8, ww);
+      ld_bf16x8(y + r * ldy + i * 8, yh[k]);
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        wd[k][e] = ww[e] * d[e];
+        yh[k][e] *= rstd;
+        s = fmaf(wd[k][e], yh[k][e], s);
+      }
+    }
+  }
+  const float m = block_sum(s, red) / H;
+#pragma unroll
+  for (int k = 0; k < kPostNormUnits; ++k) {
+    const int i = threadIdx.x + k * 256;
+    if (i < units) {
+      float o[8];
+#pragma unroll
+      for (int e = 0; e < 8; ++e) o[e] = rstd * fmaf(-yh[k][e], m, wd[k][e]);
+      st_bf16x8(dy + r * lddy + i * 8, o);
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------------
 // embeddings
 // ------------------------------------------------------------------------------------------------------------
 // BERT: z = word[id] + pos[l] + type[0]  (fp32 sum, LayerNorm follows as a separate launch)
@@ -954,6 +1073,30 @@ extern "C" int dalm_b200_rmsnorm_bwd(const float* x, const float* g, const float
                                                                    (__nv_bfloat16*)dres16, ld16, H);
   count_launch();
   return check_launch("rmsnorm_bwd_kernel");
+}
+extern "C" int dalm_b200_postnorm_fwd(const void* y, long long ldy, const float* w, const float* resid, float* out, void* out16,
+                                      long long ld16, float* rstd, int M, int H, float eps, void* stream) {
+  DALM_REQUIRE(M > 0 && H > 0 && (H % 8) == 0 && H <= 8 * kPostNormUnits * 256, "postnorm_fwd: bad shape M=%d H=%d (H %% 8 == 0, <= %d)",
+               M, H, 8 * kPostNormUnits * 256);
+  DALM_REQUIRE(y && w && resid && out && rstd && (ldy % 8) == 0 && (out16 == nullptr || (ld16 % 8) == 0), "postnorm_fwd: operands / strides");
+  DALM_REQUIRE(aligned(y, 16) && aligned(w, 16) && aligned(resid, 16) && aligned(out, 16) && aligned(out16, 16),
+               "postnorm_fwd: operands must be 16-byte aligned");
+  postnorm_fwd_kernel<<<M, 256, 0, ST(stream)>>>((const __nv_bfloat16*)y, ldy, w, resid, out, (__nv_bfloat16*)out16, ld16, rstd, H, eps);
+  count_launch();
+  return check_launch("postnorm_fwd_kernel");
+}
+extern "C" int dalm_b200_postnorm_bwd(const void* y, long long ldy, const float* w, const float* rstd, const float* dres_in,
+                                      const void* dh, long long lddh, float* dres_out, void* dy, long long lddy, int M, int H,
+                                      void* stream) {
+  DALM_REQUIRE(M > 0 && H > 0 && (H % 8) == 0 && H <= 8 * kPostNormUnits * 256, "postnorm_bwd: bad shape M=%d H=%d", M, H);
+  DALM_REQUIRE(y && w && rstd && dres_in && dres_out && dy && (ldy % 8) == 0 && (lddy % 8) == 0 && (dh == nullptr || (lddh % 8) == 0),
+               "postnorm_bwd: operands / strides");
+  DALM_REQUIRE(aligned(y, 16) && aligned(w, 16) && aligned(dres_in, 16) && aligned(dres_out, 16) && aligned(dh, 16) && aligned(dy, 16),
+               "postnorm_bwd: operands must be 16-byte aligned");
+  postnorm_bwd_kernel<<<M, 256, 0, ST(stream)>>>((const __nv_bfloat16*)y, ldy, w, rstd, dres_in, (const __nv_bfloat16*)dh, lddh, dres_out,
+                                                 (__nv_bfloat16*)dy, lddy, H);
+  count_launch();
+  return check_launch("postnorm_bwd_kernel");
 }
 extern "C" int dalm_b200_bert_embed(const int64_t* ids, const void* word, const void* pos, const void* type0, float* z,
                                     int M, int L, int H, int V, void* stream) {

@@ -24,6 +24,12 @@ e5-mistral-7b-instruct: `layers.*` with no `model.` prefix and no lm_head) load 
 Qwen3-MoE (HF Qwen3MoeForCausalLM) is Qwen3 whose sparse layers (params.moe_layers) run a routed mixture of SwiGLU experts
 instead of the dense MLP: W["moe"] holds the router and the stacked expert weights, and engine/moe.py runs the layer in the
 training forward and backward, the prefill and the decode step. Expert weights stay frozen (LoRA or inference only).
+OLMo 2 / OLMo 3 (HF Olmo2ForCausalLM / Olmo3ForCausalLM) normalise q and k over the whole projection width (qn [Nq], kn [Nkv],
+the qk_fullnorm_rope row kernel) and put the norms after each sublayer: x + post_attention_layernorm(o_proj(att)), then
++ post_feedforward_layernorm(mlp(.)), with no pre-norms (g2, g3; the postnorm kernels add the residual). The QKV and gate|up
+GEMMs read bf16(x), which the previous postnorm writes straight into their operand buffers. OLMo 3 adds layer-typed sliding
+windows and YaRN, whose attention factor scales the cos / sin tables. OLMoE (HF OlmoeForCausalLM) is a pre-norm layer with the
+full-width q/k norm and a routed MLP on every layer.
 """
 from __future__ import annotations
 
@@ -35,7 +41,8 @@ from .. import ops
 from . import moe
 from .dense import DenseBank
 from .lora import LoraBank
-from .params import attention_biases, check_llama_family, moe_layers, rope_inv_freq, sliding_windows
+from .params import (OLMO_KINDS, attention_biases, check_llama_family, check_olmo, moe_intermediate_size, moe_layers,
+                     rope_attention_factor, rope_inv_freq, sliding_windows)
 
 bf16, f32 = torch.bfloat16, torch.float32
 
@@ -75,17 +82,23 @@ class LlamaDecoder(torch.nn.Module):
         if nf4_storage:
             from .nf4store import Nf4Store
             self.nf4 = Nf4Store(device)
-        check_llama_family(cfg)
+        mt = cfg.get("model_type")
+        check_olmo(cfg) if mt in OLMO_KINDS else check_llama_family(cfg)
         self.cfg = cfg
-        self.kind = cfg.get("model_type") if cfg.get("model_type") in ("qwen2", "qwen3", "mistral", "qwen3_moe") else "llama"
+        self.kind = mt if mt in ("qwen2", "qwen3", "mistral", "qwen3_moe") + OLMO_KINDS else "llama"
         self.qkv_bias, self.o_bias = attention_biases(self.kind, cfg)
         self.qk_norm = self.kind in ("qwen3", "qwen3_moe")
+        self.fullnorm = self.kind in OLMO_KINDS                 # q/k RMSNorm over the whole q / k width (qn [Nq], kn [Nkv])
+        self.post_norm = self.kind in ("olmo2", "olmo3")        # norms after each sublayer (g2, g3), no pre-norms
+        if self.fullnorm and nf4_storage:
+            raise NotImplementedError(f"{self.kind}: 4-bit storage is not built")
         self.H = H = cfg["hidden_size"]
-        self.F = F = cfg.get("intermediate_size") or 0          # qwen3_moe without dense layers may leave it out
+        # qwen3_moe without dense layers may leave it out; olmoe's intermediate_size is its experts' width (no dense MLP)
+        self.F = F = (cfg.get("intermediate_size") or 0) if self.kind != "olmoe" else 0
         # Qwen3-MoE: the layers that run the routed MLP (engine/moe.py) instead of the dense SwiGLU one
-        self.sparse = moe_layers(cfg) if self.kind == "qwen3_moe" else [False] * cfg["num_hidden_layers"]
+        self.sparse = moe_layers(cfg) if self.kind in ("qwen3_moe", "olmoe") else [False] * cfg["num_hidden_layers"]
         if any(self.sparse) and (full or nf4_storage):
-            raise NotImplementedError("qwen3_moe: " + ("full fine-tuning is not built (grouped expert weight gradients are not "
+            raise NotImplementedError(f"{self.kind}: " + ("full fine-tuning is not built (grouped expert weight gradients are not "
                                                        "built)" if full else "4-bit storage of the expert weights is not built"))
         self.nl = cfg["num_hidden_layers"]
         self.nh = cfg["num_attention_heads"]
@@ -96,7 +109,8 @@ class LlamaDecoder(torch.nn.Module):
         self.dev = torch.device(device)
         if self.hd not in (32, 64, 128):
             raise NotImplementedError(f"head_dim {self.hd} not supported by the attention kernels")
-        self.inv_freq = rope_inv_freq(cfg, self.hd)           # default, linear or llama3 frequencies (fp32, CPU)
+        self.inv_freq = rope_inv_freq(cfg, self.hd)           # default, linear, llama3 or yarn frequencies (fp32, CPU)
+        self.rope_scale = rope_attention_factor(cfg, self.hd)  # yarn's attention factor on cos / sin, else 1
         self.windows = sliding_windows(cfg)                   # key window of each layer, 0 = full causal attention
         self.Nq, self.Nkv = self.nh * self.hd, self.nkv * self.hd
         self.Nqkv = self.Nq + 2 * self.Nkv
@@ -114,7 +128,7 @@ class LlamaDecoder(torch.nn.Module):
         self.layers: List[Dict[str, torch.Tensor]] = []
         # frozen-base modes keep the fused gate|up weight in the interleaved layout of the SwiGLU-epilogue GEMM (F % 128 == 0);
         # a fully fine-tuned model keeps HF's [gate; up] order inside its parameter bank (un-fused activation kernel)
-        self.fuse_rope = self.hd == 128
+        self.fuse_rope = self.hd == 128 and not self.fullnorm
         self.gu_il = 128 if (not full and F % 128 == 0) else 0
         if full:
             self._init_full(sd)
@@ -168,13 +182,17 @@ class LlamaDecoder(torch.nn.Module):
                 m.append((f"L{l}.bqkv", "acc", [p + f"self_attn.{n}_proj.bias" for n in "qkv"]))
             if self.o_bias:
                 m.append((f"L{l}.bo", "acc", [p + "self_attn.o_proj.bias"]))
-            if self.qk_norm:                                     # q / k norm weights: "acc" entries (the backward kernel's atomics)
+            if self.qk_norm or self.fullnorm:                    # q / k norm weights: "acc" entries (accumulated into, +=)
                 m += [(f"L{l}.qn", "acc", [p + "self_attn.q_norm.weight"]), (f"L{l}.kn", "acc", [p + "self_attn.k_norm.weight"])]
             m += [(f"L{l}.Wqkv", "gemm", [p + f"self_attn.{n}_proj.weight" for n in "qkv"]),
                   (f"L{l}.Wo", "gemm", [p + "self_attn.o_proj.weight"]),
                   (f"L{l}.Wgu", "gemm", [p + "mlp.gate_proj.weight", p + "mlp.up_proj.weight"]),
-                  (f"L{l}.Wd", "gemm", [p + "mlp.down_proj.weight"]),
-                  (f"L{l}.g1", "acc", [p + "input_layernorm.weight"]), (f"L{l}.g2", "acc", [p + "post_attention_layernorm.weight"])]
+                  (f"L{l}.Wd", "gemm", [p + "mlp.down_proj.weight"])]
+            if self.post_norm:
+                m += [(f"L{l}.g2", "acc", [p + "post_attention_layernorm.weight"]),
+                      (f"L{l}.g3", "acc", [p + "post_feedforward_layernorm.weight"])]
+            else:
+                m += [(f"L{l}.g1", "acc", [p + "input_layernorm.weight"]), (f"L{l}.g2", "acc", [p + "post_attention_layernorm.weight"])]
         return m
 
     def _init_full(self, sd) -> None:
@@ -207,14 +225,16 @@ class LlamaDecoder(torch.nn.Module):
         for l in range(self.nl):
             k = lambda n: f"L{l}.{n}"
             self.layers.append({"Wqkv_aug": bank.w16(k("Wqkv")), "Wo": bank.w16(k("Wo")), "Wgu": bank.w16(k("Wgu")),
-                                "Wd": bank.w16(k("Wd")), "g1": bank.w32(k("g1")), "g2": bank.w32(k("g2")),
+                                "Wd": bank.w16(k("Wd")), "g2": bank.w32(k("g2")),
+                                "g1": bank.w32(k("g1")) if not self.post_norm else None,
+                                "g3": bank.w32(k("g3")) if self.post_norm else None,
                                 "bqkv": bank.w32(k("bqkv")) if self.qkv_bias else None,
                                 "bo": bank.w32(k("bo")) if self.o_bias else None,
-                                "qn": bank.w32(k("qn")) if self.qk_norm else None,
-                                "kn": bank.w32(k("kn")) if self.qk_norm else None})
+                                "qn": bank.w32(k("qn")) if self.qk_norm or self.fullnorm else None,
+                                "kn": bank.w32(k("kn")) if self.qk_norm or self.fullnorm else None})
 
     def hf_state_dict(self) -> Dict[str, torch.Tensor]:
-        """fp32 CPU tensors under HF LlamaForCausalLM names (save_pretrained of a fully fine-tuned decoder), or under the
+        """fp32 CPU tensors under HF LlamaForCausalLM (or Olmo2 / Olmo3 / Olmoe) names (save_pretrained of a fully fine-tuned decoder), or under the
         unprefixed names of a headless checkpoint when the decoder was loaded from one"""
         if self.full is None:
             raise RuntimeError("hf_state_dict: only fully fine-tuned models own their weights (PEFT mode saves adapters)")
@@ -313,8 +333,12 @@ class LlamaDecoder(torch.nn.Module):
                 W["WguT"] = W["Wgu"].t().contiguous()
                 W["Wd"] = g(p + "mlp.down_proj.weight", bf16)
                 W["WdT"] = W["Wd"].t().contiguous()
-            W["g1"] = g(p + "input_layernorm.weight", f32)
-            W["g2"] = g(p + "post_attention_layernorm.weight", f32)
+            if self.post_norm:
+                W["g2"] = g(p + "post_attention_layernorm.weight", f32)
+                W["g3"] = g(p + "post_feedforward_layernorm.weight", f32)
+            else:
+                W["g1"] = g(p + "input_layernorm.weight", f32)
+                W["g2"] = g(p + "post_attention_layernorm.weight", f32)
             self._frozen_biases(W, p, g)
             self.layers.append(W)
 
@@ -323,7 +347,7 @@ class LlamaDecoder(torch.nn.Module):
         transformers 5's fused one (mlp.experts.gate_up_proj [E, 2I, H]: gate rows then up rows; mlp.experts.down_proj
         [E, H, I])"""
         cfg = self.cfg
-        E, I = int(cfg["num_experts"]), int(cfg["moe_intermediate_size"])
+        E, I = int(cfg["num_experts"]), moe_intermediate_size(cfg)
         if p + "mlp.experts.gate_up_proj" in sd:
             gu, down = sd[p + "mlp.experts.gate_up_proj"], sd[p + "mlp.experts.down_proj"]
             gate_proj, up_proj = gu[:, :I], gu[:, I:]
@@ -362,8 +386,8 @@ class LlamaDecoder(torch.nn.Module):
         W["bqkv"] = torch.cat([g(p + f"self_attn.{n}_proj.bias", f32) for n in "qkv"]) if self.qkv_bias else None
         W["bo"] = g(p + "self_attn.o_proj.bias", f32) if self.o_bias else None
         # Qwen3's q / k norm weights: forward-only fp32 vectors here too (use_bnb: the fp16 cast, as every norm weight)
-        W["qn"] = g(p + "self_attn.q_norm.weight", f32) if self.qk_norm else None
-        W["kn"] = g(p + "self_attn.k_norm.weight", f32) if self.qk_norm else None
+        W["qn"] = g(p + "self_attn.q_norm.weight", f32) if self.qk_norm or self.fullnorm else None
+        W["kn"] = g(p + "self_attn.k_norm.weight", f32) if self.qk_norm or self.fullnorm else None
 
     def _drop(self, training: bool, call: int, layer: int):
         if not training or self.p_lora <= 0.0:
@@ -401,7 +425,11 @@ class LlamaDecoder(torch.nn.Module):
         decode); the frequency scaling of the config lives in `inv_freq` only"""
         if L not in self._rope_cache:
             fr = torch.outer(torch.arange(L, dtype=torch.float32), self.inv_freq)                      # [L, hd/2]
-            self._rope_cache[L] = (fr.cos().to(self.dev).contiguous(), fr.sin().to(self.dev).contiguous())
+            cos, sin = fr.cos(), fr.sin()
+            scale = getattr(self, "rope_scale", 1.0)          # yarn: transformers scales cos / sin by the attention factor
+            if scale != 1.0:
+                cos, sin = cos * scale, sin * scale
+            self._rope_cache[L] = (cos.to(self.dev).contiguous(), sin.to(self.dev).contiguous())
         return self._rope_cache[L]
 
     # ------------------------------------------------------------------------------------------------------------
@@ -470,20 +498,30 @@ class LlamaDecoder(torch.nn.Module):
         self._call += 1
         ctx.call, ctx.training = self._call, self.training
         x = ops.embed_gather(ids, self.embed)                                    # fp32 residual stream [M,H]
+        if self.post_norm:                                                       # the first QKV GEMM reads bf16(embeddings)
+            h_next = _aug_buf(M, H, Ra, self.dev)
+            ops.cast_f32_bf16(x, h_next[:, :H])
         for li, W in enumerate(self.layers):
             a = _Ctx()
-            a.x_in = x
-            a.h1_aug = _aug_buf(M, H, Ra, self.dev)
-            _, a.rstd1 = ops.rmsnorm_fwd(x, W["g1"], self.eps, h=a.h1_aug[:, :H])
+            if self.post_norm:                   # no pre-norm: bf16(x), written by the layer below's postnorm (or the cast)
+                a.h1_aug = h_next
+            else:
+                a.x_in = x
+                a.h1_aug = _aug_buf(M, H, Ra, self.dev)
+                _, a.rstd1 = ops.rmsnorm_fwd(x, W["g1"], self.eps, h=a.h1_aug[:, :H])
             if Ra:
                 ops.skinny_gemm(a.h1_aug[:, :H], W["A_stack"], a.h1_aug[:, H:], K=H, R=Ra,   # u = dropout(h1) A^T [M,2r]
                                 dropx=self._drop(ctx.training, ctx.call, li))
             rope_cols = (self.nh + self.nkv) * self.hd
             a.pre = a.qk_rstd = None
-            if self.qk_norm and save and self.trainable:                         # what the q/k norm backward reads
+            if (self.qk_norm or self.fullnorm) and save and self.trainable:      # what the q/k norm backward reads
                 a.pre = torch.empty(M, rope_cols, dtype=bf16, device=self.dev)
-                a.qk_rstd = torch.empty(M, self.nh + self.nkv, dtype=f32, device=self.dev)
-            if pos is None and self.fuse_rope and rope_cols % 256 == 0:
+                a.qk_rstd = torch.empty(M, 2 if self.fullnorm else self.nh + self.nkv, dtype=f32, device=self.dev)
+            if self.fullnorm:
+                a.qkv = ops.gemm(a.h1_aug, W["Wqkv_aug"])                         # [M, Nq+2Nkv], then q/k norm + RoPE
+                ops.qk_fullnorm_rope_(a.qkv, self.nh, self.nkv, self.hd, W["qn"], W["kn"], self.eps, cos_t, sin_t,
+                                      L=L if pos is None else 0, pos=pos, pre=a.pre, rstd=a.qk_rstd, round_first=self.kind == "olmoe")
+            elif pos is None and self.fuse_rope and rope_cols % 256 == 0:
                 norm = dict(q_norm=W["qn"], k_norm=W["kn"], nq_heads=self.nh, eps=self.eps, pre_out=a.pre,
                             rstd_out=a.qk_rstd) if self.qk_norm else {}
                 a.qkv = ops.gemm_rope(a.h1_aug, W["Wqkv_aug"], cos_t, sin_t, L, rope_cols,   # QKV (+LoRA, + bias) with (q/k norm
@@ -502,10 +540,15 @@ class LlamaDecoder(torch.nn.Module):
             a.att, a.lse = ops.attention_auto_fwd(a.qkv[:, :self.Nq], a.qkv[:, self.Nq:self.Nq + self.Nkv],
                                                   a.qkv[:, self.Nq + self.Nkv:], ctx.mask, B, L, self.nh, self.nkv, self.hd, causal=True,
                                                   window=self.windows[li])
-            a.x_mid = ops.gemm(a.att, W["Wo"], out_dtype=f32, resid=x, bias=W["bo"])
-            a.h2, a.rstd2 = ops.rmsnorm_fwd(a.x_mid, W["g2"], self.eps)
+            if self.post_norm:                   # x_mid = x + post_attention_layernorm(o_proj(att)); h2 = bf16(x_mid)
+                a.yo = ops.gemm(a.att, W["Wo"])
+                a.h2 = torch.empty(M, H, dtype=bf16, device=self.dev)
+                x_mid, a.rstd2 = ops.postnorm_fwd(a.yo, W["g2"], x, self.eps, out16=a.h2)
+            else:
+                x_mid = a.x_mid = ops.gemm(a.att, W["Wo"], out_dtype=f32, resid=x, bias=W["bo"])
+                a.h2, a.rstd2 = ops.rmsnorm_fwd(x_mid, W["g2"], self.eps)
             if "moe" in W:
-                x, a.moe = moe.forward(a.h2, W["moe"], resid=a.x_mid)
+                x, a.moe = moe.forward(a.h2, W["moe"], resid=x_mid)
                 if save:
                     ctx.layers.append(a)
                 continue
@@ -514,7 +557,12 @@ class LlamaDecoder(torch.nn.Module):
             else:
                 a.gu = ops.gemm(a.h2, W["Wgu"])                                   # [M,2F]
                 a.act = ops.swiglu_fwd(a.gu, F)
-            x = ops.gemm(a.act, W["Wd"], out_dtype=f32, resid=a.x_mid)
+            if self.post_norm:                   # x = x_mid + post_feedforward_layernorm(down(act)), bf16(x) into the next QKV operand
+                a.yd = ops.gemm(a.act, W["Wd"])
+                h_next = _aug_buf(M, H, Ra, self.dev) if li + 1 < self.nl else None
+                x, a.rstd3 = ops.postnorm_fwd(a.yd, W["g3"], x_mid, self.eps, out16=h_next[:, :H] if h_next is not None else None)
+            else:
+                x = ops.gemm(a.act, W["Wd"], out_dtype=f32, resid=x_mid)
             if save:
                 ctx.layers.append(a)
         ctx.x_final = x
@@ -530,25 +578,43 @@ class LlamaDecoder(torch.nn.Module):
         H, F, Ra = self.H, self.F, self.Ra
         cos_t, sin_t = tables
         x = ops.embed_gather(ids, self.embed)                                    # fp32 residual stream [B,H]
+        if self.post_norm:
+            h_next = _aug_buf(B, H, Ra, self.dev)
+            ops.cast_f32_bf16(x, h_next[:, :H])
         for li, W in enumerate(self.layers):
-            h1_aug = _aug_buf(B, H, Ra, self.dev)
-            ops.rmsnorm_fwd(x, W["g1"], self.eps, h=h1_aug[:, :H])
+            if self.post_norm:
+                h1_aug = h_next
+            else:
+                h1_aug = _aug_buf(B, H, Ra, self.dev)
+                ops.rmsnorm_fwd(x, W["g1"], self.eps, h=h1_aug[:, :H])
             if Ra:
                 ops.skinny_gemm(h1_aug[:, :H], W["A_stack"], h1_aug[:, H:], K=H, R=Ra)
             qkv = ops.gemm_rows(h1_aug, W["Wqkv_aug"], bias=W["bqkv"])                # [B, Nq+2Nkv]
-            if self.qk_norm:
+            if self.fullnorm:
+                ops.qk_fullnorm_rope_(qkv, self.nh, self.nkv, self.hd, W["qn"], W["kn"], self.eps, cos_t, sin_t, pos=pos,
+                                      round_first=self.kind == "olmoe")
+            elif self.qk_norm:
                 ops.qk_norm_rope_(qkv, self.nh + self.nkv, self.nh, W["qn"], W["kn"], self.eps, cos_t, sin_t, pos=pos)
             else:
                 ops.rope_pos_(qkv, 0, self.nh + self.nkv, self.hd, cos_t, sin_t, pos)
             att = ops.attention_decode(qkv, 0, self.Nq, self.Nq + self.Nkv, caches[li][0], caches[li][1], kmask, cur,
                                        self.nh, self.nkv, self.hd, window=self.windows[li])
-            x_mid = ops.gemm_rows(att, W["Wo"], out_dtype=f32, resid=x, bias=W["bo"])
-            h2, _ = ops.rmsnorm_fwd(x_mid, W["g2"], self.eps)
+            if self.post_norm:
+                h2 = torch.empty(B, H, dtype=bf16, device=self.dev)
+                x_mid, _ = ops.postnorm_fwd(ops.gemm_rows(att, W["Wo"]), W["g2"], x, self.eps, out16=h2)
+            else:
+                x_mid = ops.gemm_rows(att, W["Wo"], out_dtype=f32, resid=x, bias=W["bo"])
+                h2, _ = ops.rmsnorm_fwd(x_mid, W["g2"], self.eps)
             if "moe" in W:
                 x, _ = moe.forward(h2, W["moe"], resid=x_mid)
                 continue
             act = ops.swiglu_fwd(ops.gemm_rows(h2, W["Wgu"]), F, interleave=self.gu_il)
-            x = ops.gemm_rows(act, W["Wd"], out_dtype=f32, resid=x_mid)
+            if self.post_norm:
+                h_next = _aug_buf(B, H, Ra, self.dev) if li + 1 < self.nl else None
+                x, _ = ops.postnorm_fwd(ops.gemm_rows(act, W["Wd"]), W["g3"], x_mid, self.eps,
+                                        out16=h_next[:, :H] if h_next is not None else None)
+            else:
+                x = ops.gemm_rows(act, W["Wd"], out_dtype=f32, resid=x_mid)
         hf, _ = ops.rmsnorm_fwd(x, self.norm_g, self.eps)
         return ops.gemm_rows(hf, self.lm_head)
 
@@ -604,8 +670,13 @@ class LlamaDecoder(torch.nn.Module):
         if bank is not None:
             ops.col_reduce_(dy_bf16=dhf, z=ctx.x_final, rstd=ctx.rstdf, out_prod=bank.g("norm_g"))
         dx32, dx16 = ops.rmsnorm_bwd(ctx.x_final, self.norm_g, ctx.rstdf, dhf)
+        dpend = None       # post-norm: d(bf16 x) of the layer above's QKV GEMM, joining the residual gradient at this layer's output
         for l in range(self.nl - 1, -1, -1):
             W, a = self.layers[l], ctx.layers[l]
+            if self.post_norm:                   # dxs = dx32 + dpend (passed on unchanged), dx16 = d(down output)
+                dxs, dx16 = ops.postnorm_bwd(a.yd, W["g3"], a.rstd3, dx32, dh=dpend)
+                if bank is not None:
+                    ops.norm_wgrad_(dxs, a.yd, a.rstd3, G(l, "g3"))
             if "moe" in W:                                                         # experts and router frozen: input gradient only
                 dh2 = ops.cast_f32_bf16(moe.backward(dx16, a.moe, W["moe"]))
             else:
@@ -616,9 +687,14 @@ class LlamaDecoder(torch.nn.Module):
                 if bank is not None:
                     ops.wgrad_(a.gu, a.h2, G(l, "Wgu"), acc)
                 dh2 = self._dgrad(a.gu, W, "Wgu")                                  # [M,H]
-            if bank is not None:
-                ops.col_reduce_(dy_bf16=dh2, z=a.x_mid, rstd=a.rstd2, out_prod=G(l, "g2"))
-            dmid32, dmid16 = ops.rmsnorm_bwd(a.x_mid, W["g2"], a.rstd2, dh2, dres_in=dx32)
+            if self.post_norm:                   # dmid32 = dxs + dh2, dmid16 = d(o_proj output)
+                dmid32, dmid16 = ops.postnorm_bwd(a.yo, W["g2"], a.rstd2, dxs, dh=dh2)
+                if bank is not None:
+                    ops.norm_wgrad_(dmid32, a.yo, a.rstd2, G(l, "g2"))
+            else:
+                if bank is not None:
+                    ops.col_reduce_(dy_bf16=dh2, z=a.x_mid, rstd=a.rstd2, out_prod=G(l, "g2"))
+                dmid32, dmid16 = ops.rmsnorm_bwd(a.x_mid, W["g2"], a.rstd2, dh2, dres_in=dx32)
             if bank is not None:
                 ops.wgrad_(dmid16, a.att, G(l, "Wo"), acc)
                 if self.o_bias:                                                    # d bo = column sums of d(o_proj output)
@@ -629,7 +705,11 @@ class LlamaDecoder(torch.nn.Module):
                      ctx.mask, a.att, a.lse, datt, B, L, self.nh, self.nkv, self.hd, causal=True,
                      dq=dqkv[:, :self.Nq], dk=dqkv[:, self.Nq:self.Nq + self.Nkv],
                      dv=dqkv[:, self.Nq + self.Nkv:self.Nqkv], window=self.windows[l])
-            if self.qk_norm:                                                       # un-rotate, then the q/k RMSNorm backward
+            if self.fullnorm:                                                      # un-rotate, then the full-width q/k norm backward
+                ops.qk_fullnorm_rope_bwd_(dqkv, self.nh, self.nkv, self.hd, W["qn"], W["kn"], cos_t, sin_t, L, a.pre, a.qk_rstd,
+                                          dw_q=G(l, "qn") if bank is not None else None,
+                                          dw_k=G(l, "kn") if bank is not None else None)
+            elif self.qk_norm:                                                     # un-rotate, then the q/k RMSNorm backward
                 ops.qk_norm_rope_bwd_(dqkv, self.nh + self.nkv, self.nh, W["qn"], W["kn"], cos_t, sin_t, L, a.pre, a.qk_rstd,
                                       dw_q=G(l, "qn") if bank is not None else None, dw_k=G(l, "kn") if bank is not None else None)
             else:
@@ -639,8 +719,11 @@ class LlamaDecoder(torch.nn.Module):
                 if self.qkv_bias:                                                  # d bqkv = column sums of d(pre-RoPE qkv)
                     ops.col_reduce_(dy_bf16=dqkv, out_sum=G(l, "bqkv"))
                 dh1 = ops.gemm(dqkv, W["Wqkv_aug"], layout=1)
-                ops.col_reduce_(dy_bf16=dh1, z=a.x_in, rstd=a.rstd1, out_prod=G(l, "g1"))
-                dx32, dx16 = ops.rmsnorm_bwd(a.x_in, W["g1"], a.rstd1, dh1, dres_in=dmid32)
+                if self.post_norm:
+                    dx32, dpend = dmid32, dh1
+                else:
+                    ops.col_reduce_(dy_bf16=dh1, z=a.x_in, rstd=a.rstd1, out_prod=G(l, "g1"))
+                    dx32, dx16 = ops.rmsnorm_bwd(a.x_in, W["g1"], a.rstd1, dh1, dres_in=dmid32)
                 bank.bucket_ready(f"L{l}.")                                        # this layer's four weight gradients are final
                 continue
             names = [f"model.layers.{l}.self_attn.{n}" for n in self.LORA_TARGETS]
@@ -664,7 +747,12 @@ class LlamaDecoder(torch.nn.Module):
             else:
                 dh1 = ops.gemm(dqkv[:, :self.Nqkv], W["WqkvT_aug"][:, :self.Nqkv])
                 ops.lora_dx_(dh1, dqkv[:, self.Nqkv:], W["A_stack"], K=H, R=Ra, drop=xdrop)
-            dx32, dx16 = ops.rmsnorm_bwd(a.x_in, W["g1"], a.rstd1, dh1, dres_in=dmid32)
+            if self.post_norm:
+                dx32, dpend = dmid32, dh1
+            else:
+                dx32, dx16 = ops.rmsnorm_bwd(a.x_in, W["g1"], a.rstd1, dh1, dres_in=dmid32)
         if bank is not None:
+            if self.post_norm:                                                     # d(embeddings) = residual + QKV-input gradients
+                dx32 = ops.masked_add(a=dx32, b=dpend)
             ops.embed_scatter_add_(dx32, ctx.ids, bank.g("embed"))                # embed_tokens
             bank.end_backward()

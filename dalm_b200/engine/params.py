@@ -23,13 +23,14 @@ def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, 
                       bias_std: Optional[float] = None, qk_norm_std: Optional[float] = None,
                       router_std: Optional[float] = None) -> Dict[str, torch.Tensor]:
     """HF parameter names for BertModel / XLMRobertaModel / RobertaModel / ModernBertModel (no prefix) / LlamaForCausalLM / Qwen2ForCausalLM /
-    Qwen3ForCausalLM / MistralForCausalLM / FalconForCausalLM, init N(0, initializer_range), LN = (1, 0). Decoder attention biases (Qwen2's q/k/v, Llama's and Qwen3's
+    Qwen3ForCausalLM / MistralForCausalLM / Olmo2ForCausalLM / Olmo3ForCausalLM / OlmoeForCausalLM / FalconForCausalLM, init N(0, initializer_range), LN = (1, 0). Decoder attention biases (Qwen2's q/k/v, Llama's and Qwen3's
     `attention_bias`) are drawn from N(0, bias_std) (default: initializer_range) rather than HF's zeros, so that a dropped bias
     changes the outputs. Qwen3's q_norm / k_norm weights are 1 + N(0, qk_norm_std) (default: initializer_range), so that a
     dropped or swapped norm shows; so are every LayerNorm weight of ModernBERT. Qwen3MoeForCausalLM's sparse layers are
     written in the hub layout (`mlp.gate.weight` [E, H], `mlp.experts.{e}.{gate,up,down}_proj.weight`), the router weights
     drawn from N(0, router_std) (default: initializer_range): a larger std spreads the router probabilities, so that the
-    top-k choice is far from ties."""
+    top-k choice is far from ties. The OLMo kinds' full-width q_norm / k_norm weights take qk_norm_std like Qwen3's; OLMo 2 / 3
+    write post_attention_layernorm / post_feedforward_layernorm and no input_layernorm; OLMoE's layers are all sparse."""
     on_device = torch.device(device).type == "cuda" and cfg.get("_device_rng", False)
     gen = torch.Generator(device=device) if on_device else torch.Generator()
     gen.manual_seed(seed)
@@ -62,12 +63,13 @@ def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, 
             sd[p + "output.LayerNorm.bias"] = _normal(gen, (H,), std, dtype, device)
         sd["pooler.dense.weight"] = _normal(gen, (H, H), std, dtype, device)   # loaded by AutoModel, unused by the path
         sd["pooler.dense.bias"] = zeros(H)
-    elif kind in ("llama", "qwen2", "qwen3", "mistral", "qwen3_moe"):
+    elif kind in ("llama", "qwen2", "qwen3", "mistral", "qwen3_moe") + OLMO_KINDS:
         F, V = cfg.get("intermediate_size"), cfg["vocab_size"]
-        sparse = moe_layers(cfg) if kind == "qwen3_moe" else [False] * cfg["num_hidden_layers"]
+        sparse = moe_layers(cfg) if kind in ("qwen3_moe", "olmoe") else [False] * cfg["num_hidden_layers"]
+        post_norm = kind in ("olmo2", "olmo3")
         nh, nkv = cfg["num_attention_heads"], cfg.get("num_key_value_heads", cfg["num_attention_heads"])
         hd = cfg.get("head_dim") or H // nh
-        qkv_bias, o_bias = attention_biases(kind, cfg)
+        qkv_bias, o_bias = attention_biases(kind, cfg) if kind not in OLMO_KINDS else (False, False)
         bstd = std if bias_std is None else float(bias_std)
         sd["model.embed_tokens.weight"] = _normal(gen, (V, H), std, dtype, device)
         for l in range(cfg["num_hidden_layers"]):
@@ -86,8 +88,12 @@ def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, 
                 nstd = std if qk_norm_std is None else float(qk_norm_std)
                 sd[p + "self_attn.q_norm.weight"] = ones(hd) + _normal(gen, (hd,), nstd, dtype, device)
                 sd[p + "self_attn.k_norm.weight"] = ones(hd) + _normal(gen, (hd,), nstd, dtype, device)
+            if kind in OLMO_KINDS:                                 # q / k RMSNorm over the whole projection width
+                nstd = std if qk_norm_std is None else float(qk_norm_std)
+                sd[p + "self_attn.q_norm.weight"] = ones(nh * hd) + _normal(gen, (nh * hd,), nstd, dtype, device)
+                sd[p + "self_attn.k_norm.weight"] = ones(nkv * hd) + _normal(gen, (nkv * hd,), nstd, dtype, device)
             if sparse[l]:
-                E, I = cfg["num_experts"], cfg["moe_intermediate_size"]
+                E, I = cfg["num_experts"], moe_intermediate_size(cfg)
                 sd[p + "mlp.gate.weight"] = _normal(gen, (E, H), std if router_std is None else float(router_std), dtype, device)
                 for e in range(E):
                     sd[p + f"mlp.experts.{e}.gate_proj.weight"] = _normal(gen, (I, H), std, dtype, device)
@@ -97,8 +103,12 @@ def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, 
                 sd[p + "mlp.gate_proj.weight"] = _normal(gen, (F, H), std, dtype, device)
                 sd[p + "mlp.up_proj.weight"] = _normal(gen, (F, H), std, dtype, device)
                 sd[p + "mlp.down_proj.weight"] = _normal(gen, (H, F), std, dtype, device)
-            sd[p + "input_layernorm.weight"] = ones(H) + _normal(gen, (H,), std, dtype, device)
-            sd[p + "post_attention_layernorm.weight"] = ones(H) + _normal(gen, (H,), std, dtype, device)
+            if post_norm:                                          # OLMo 2 / 3: norms after each sublayer, none before
+                sd[p + "post_attention_layernorm.weight"] = ones(H) + _normal(gen, (H,), std, dtype, device)
+                sd[p + "post_feedforward_layernorm.weight"] = ones(H) + _normal(gen, (H,), std, dtype, device)
+            else:
+                sd[p + "input_layernorm.weight"] = ones(H) + _normal(gen, (H,), std, dtype, device)
+                sd[p + "post_attention_layernorm.weight"] = ones(H) + _normal(gen, (H,), std, dtype, device)
         sd["model.norm.weight"] = ones(H) + _normal(gen, (H,), std, dtype, device)
         if not cfg.get("tie_word_embeddings", False):             # tied checkpoints store no lm_head (Qwen2 0.5B-3B)
             sd["lm_head.weight"] = _normal(gen, (V, H), std, dtype, device)
@@ -185,6 +195,9 @@ def model_kind(cfg: Dict) -> str:
     if mt in ("llama", "qwen2", "qwen3", "mistral", "qwen3_moe"):
         check_llama_family(cfg)
         return mt
+    if mt in OLMO_KINDS:
+        check_olmo(cfg)
+        return mt
     if mt == "modernbert":
         check_modernbert(cfg)
         return "modernbert"
@@ -193,7 +206,7 @@ def model_kind(cfg: Dict) -> str:
         return "falcon"
     raise NotImplementedError(
         f"model_type {mt!r} is not built in dalm_b200 (supported: bert, roberta, xlm-roberta and modernbert encoders; llama, "
-        "qwen2, qwen3, qwen3_moe, mistral and falcon decoders)")
+        "qwen2, qwen3, qwen3_moe, mistral, olmo2, olmo3, olmoe and falcon decoders)")
 
 
 def _rope_type(cfg: Dict) -> str:
@@ -218,8 +231,10 @@ def rope_parameters(cfg: Dict) -> Dict:
 
 
 # RoPE types whose frequencies are a fixed table: a position-indexed cos / sin table represents them exactly. `dynamic` changes
-# the frequencies with the sequence length, `yarn` / `longrope` also scale the attention, `proportional` rotates part of a head.
-BUILT_ROPE_TYPES = {"llama": ("default", "linear", "llama3")}
+# the frequencies with the sequence length, `longrope` switches tables with it, `proportional` rotates part of a head. `yarn`
+# also scales cos / sin by its attention factor, which the tables carry (rope_attention_factor).
+BUILT_ROPE_TYPES = {"llama": ("default", "linear", "llama3"), "olmo2": ("default", "yarn"), "olmo3": ("default", "yarn"),
+                    "olmoe": ("default", "yarn")}
 
 
 def check_rope_type(cfg: Dict) -> str:
@@ -239,6 +254,8 @@ def rope_inv_freq(cfg: Dict, head_dim: int) -> torch.Tensor:
     three have attention factor 1, so cos / sin tables built from these frequencies are the whole of the position encoding."""
     rt = check_rope_type(cfg)
     rp = rope_parameters(cfg)
+    if rt == "yarn":
+        return _yarn(cfg, head_dim)[0]
     base = rp["rope_theta"]
     inv_freq = 1.0 / (base ** (torch.arange(0, head_dim, 2, dtype=torch.int64).to(dtype=torch.float) / head_dim))
     if rt == "linear":
@@ -256,6 +273,51 @@ def rope_inv_freq(cfg: Dict, head_dim: int) -> torch.Tensor:
         medium = ~(wavelen < high_freq_wavelen) * ~(wavelen > low_freq_wavelen)
         inv_freq = torch.where(medium, smoothed, scaled)
     return inv_freq
+
+
+def rope_attention_factor(cfg: Dict, head_dim: int) -> float:
+    """the factor transformers' rotary embedding multiplies cos / sin by: `yarn`'s attention factor, 1 for every other type"""
+    return _yarn(cfg, head_dim)[1] if check_rope_type(cfg) == "yarn" else 1.0
+
+
+def _yarn(cfg: Dict, head_dim: int):
+    """(inv_freq fp32 [head_dim / 2], attention factor) of a `yarn` config, the fp32 operations of transformers'
+    _compute_yarn_parameters in its order: frequencies blended between interpolation (/ factor) and extrapolation along a
+    linear ramp over the dimensions whose wavelengths lie between beta_fast and beta_slow rotations of the original context"""
+    rp = rope_parameters(cfg)
+    base = rp["rope_theta"]
+    dim = head_dim
+    orig = cfg["original_max_position_embeddings"] if "original_max_position_embeddings" in cfg else \
+        (rp.get("original_max_position_embeddings") or cfg["max_position_embeddings"])
+    factor = rp.get("factor")
+    if factor is None:
+        factor = cfg["max_position_embeddings"] / orig
+    attention_factor, mscale, mscale_all_dim = rp.get("attention_factor"), rp.get("mscale"), rp.get("mscale_all_dim")
+
+    def get_mscale(scale, m=1):
+        return 1.0 if scale <= 1 else 0.1 * m * math.log(scale) + 1.0
+
+    if attention_factor is None:
+        if mscale and mscale_all_dim:
+            attention_factor = float(get_mscale(factor, mscale) / get_mscale(factor, mscale_all_dim))
+        else:
+            attention_factor = get_mscale(factor)
+    beta_fast, beta_slow = rp.get("beta_fast") or 32, rp.get("beta_slow") or 1
+
+    def correction_dim(rot):
+        return (dim * math.log(orig / (rot * 2 * math.pi))) / (2 * math.log(base))
+
+    low, high = correction_dim(beta_fast), correction_dim(beta_slow)
+    if rp.get("truncate", True):
+        low, high = math.floor(low), math.ceil(high)
+    low, high = max(low, 0), min(high, dim - 1)
+    if low == high:
+        high += 0.001                                            # transformers' guard against a zero-width ramp
+    pos_freqs = base ** (torch.arange(0, dim, 2).to(dtype=torch.float) / dim)
+    extrapolation, interpolation = 1.0 / pos_freqs, 1.0 / (factor * pos_freqs)
+    extra_factor = 1 - torch.clamp((torch.arange(dim // 2, dtype=torch.float32) - low) / (high - low), 0, 1)
+    inv_freq = interpolation * (1 - extra_factor) + extrapolation * extra_factor
+    return inv_freq, attention_factor
 
 
 def check_llama_family(cfg: Dict) -> None:
@@ -305,33 +367,48 @@ MOE_MAX_EXPERTS, MOE_MAX_TOPK = 256, 16
 
 def check_qwen3_moe(cfg: Dict) -> None:
     """refuses a qwen3_moe config the routed MLP would otherwise compute wrong or cannot run"""
-    missing = [k for k in QWEN3_MOE_KEYS if k not in cfg]
-    if missing:
-        raise NotImplementedError(f"qwen3_moe: a config without {', '.join(missing)} is not built (transformers would fill in "
-                                  "Qwen3MoeConfig's defaults, the 30B-A3B shape; the shape is read from config.json only)")
-    E, k, I = int(cfg["num_experts"]), int(cfg["num_experts_per_tok"]), int(cfg["moe_intermediate_size"])
-    if E > 0:
-        if E % 8 or E > MOE_MAX_EXPERTS:
-            raise NotImplementedError(f"qwen3_moe: num_experts={E} is not built (the router kernels take a multiple of 8 up to "
-                                      f"{MOE_MAX_EXPERTS})")
-        if not 1 <= k <= min(E, MOE_MAX_TOPK):
-            raise NotImplementedError(f"qwen3_moe: num_experts_per_tok={k} is not built (the router takes 1 to "
-                                      f"min(num_experts, {MOE_MAX_TOPK}))")
-        if I <= 0 or I % 128:
-            raise NotImplementedError(f"qwen3_moe: moe_intermediate_size={I} is not built (the grouped SwiGLU GEMM takes a "
-                                      "multiple of 128: 128-feature gate / up blocks)")
-        if cfg["hidden_size"] % 64:
-            raise NotImplementedError(f"qwen3_moe: hidden_size={cfg['hidden_size']} is not built (the experts' down-projection "
-                                      "dgrad takes a multiple of 64)")
+    check_moe_bounds(cfg)
     if not all(moe_layers(cfg)) and "intermediate_size" not in cfg:
         raise NotImplementedError("qwen3_moe: dense MLP layers (mlp_only_layers / decoder_sparse_step) need intermediate_size "
                                   "in config.json")
 
 
+def check_moe_bounds(cfg: Dict) -> None:
+    """refuses a routed-MLP config (qwen3_moe, olmoe) outside the bounds of the routing kernels and the grouped GEMMs"""
+    mt = cfg.get("model_type", "")
+    keys = QWEN3_MOE_KEYS if mt != "olmoe" else ("num_experts", "num_experts_per_tok", "intermediate_size")
+    missing = [k for k in keys if k not in cfg]
+    if missing:
+        raise NotImplementedError(f"{mt}: a config without {', '.join(missing)} is not built (transformers would fill in "
+                                  "its config class's defaults; the shape is read from config.json only)")
+    E, k, I = int(cfg["num_experts"]), int(cfg["num_experts_per_tok"]), moe_intermediate_size(cfg)
+    if E > 0:
+        if E % 8 or E > MOE_MAX_EXPERTS:
+            raise NotImplementedError(f"{mt}: num_experts={E} is not built (the router kernels take a multiple of 8 up to "
+                                      f"{MOE_MAX_EXPERTS})")
+        if not 1 <= k <= min(E, MOE_MAX_TOPK):
+            raise NotImplementedError(f"{mt}: num_experts_per_tok={k} is not built (the router takes 1 to "
+                                      f"min(num_experts, {MOE_MAX_TOPK}))")
+        if I <= 0 or I % 128:
+            raise NotImplementedError(f"{mt}: {'intermediate_size' if mt == 'olmoe' else 'moe_intermediate_size'}={I} is not built (the grouped SwiGLU GEMM takes a "
+                                      "multiple of 128: 128-feature gate / up blocks)")
+        if cfg["hidden_size"] % 64:
+            raise NotImplementedError(f"{mt}: hidden_size={cfg['hidden_size']} is not built (the experts' down-projection "
+                                      "dgrad takes a multiple of 64)")
+
+
+def moe_intermediate_size(cfg: Dict) -> int:
+    """each expert's SwiGLU width: qwen3_moe's `moe_intermediate_size`; OLMoE sizes its experts by `intermediate_size`"""
+    return int(cfg["intermediate_size"] if cfg.get("model_type") == "olmoe" else cfg["moe_intermediate_size"])
+
+
 def moe_layers(cfg: Dict) -> List[bool]:
     """which layers of a qwen3_moe config run the routed MLP, as Qwen3MoeDecoderLayer decides: not in `mlp_only_layers`,
-    num_experts > 0 and (i + 1) % decoder_sparse_step == 0; the others run the dense SwiGLU MLP of `intermediate_size`"""
+    num_experts > 0 and (i + 1) % decoder_sparse_step == 0; the others run the dense SwiGLU MLP of `intermediate_size`.
+    olmoe: every layer (OlmoeDecoderLayer always builds the sparse block)."""
     n = int(cfg["num_hidden_layers"])
+    if cfg.get("model_type") == "olmoe":
+        return [True] * n
     only = set(cfg.get("mlp_only_layers") or ())
     step = int(cfg.get("decoder_sparse_step", 1))
     return [i not in only and int(cfg.get("num_experts", 0)) > 0 and (i + 1) % step == 0 for i in range(n)]
@@ -349,7 +426,9 @@ def sliding_windows(cfg: Dict) -> List[int]:
       or when that list is absent on layers i >= `max_window_layers` (default 28).
     - qwen3_moe: `sliding_window` (default 4096) on every layer when `use_sliding_window`, as Qwen3MoeConfig and its
       attention read it (no `max_window_layers` or `layer_types`).
-    - llama: none.
+    - olmo3: `sliding_window` (default 4096) on the layers `layer_types` marks "sliding_attention"; without the list, as
+      Olmo3Config fills it in: every fourth layer (i + 1) % 4 == 0 full, the others sliding.
+    - llama, olmo2, olmoe: none.
     A layer with window w lets query i see key j iff i - w < j <= i, in the indices of the padded row."""
     mt, n = cfg.get("model_type", ""), int(cfg["num_hidden_layers"])
     if mt == "mistral":
@@ -358,6 +437,14 @@ def sliding_windows(cfg: Dict) -> List[int]:
     if mt == "qwen3_moe":
         w = cfg.get("sliding_window", 4096) if cfg.get("use_sliding_window", False) else 0
         return [int(w) if w else 0] * n
+    if mt == "olmo3":
+        w = cfg.get("sliding_window", 4096)
+        types = cfg.get("layer_types")
+        if types is None:                                        # Olmo3Config: every fourth layer full, the others sliding
+            types = ["sliding_attention" if (i + 1) % 4 != 0 else "full_attention" for i in range(n)]
+        if len(types) != n:
+            raise ValueError(f"{mt}: layer_types lists {len(types)} layers, num_hidden_layers is {n}")
+        return [int(w) if (t == "sliding_attention" and w) else 0 for t in types]
     if mt in ("qwen2", "qwen3"):
         w = cfg.get("sliding_window", 4096)
         if not cfg.get("use_sliding_window", False) or not w:
@@ -370,6 +457,42 @@ def sliding_windows(cfg: Dict) -> List[int]:
             raise ValueError(f"{mt}: layer_types lists {len(types)} layers, num_hidden_layers is {n}")
         return [int(w) if t == "sliding_attention" else 0 for t in types]
     return [0] * n
+
+
+OLMO_KINDS = ("olmo2", "olmo3", "olmoe")
+# keys without which transformers would fill in its config class's defaults (the 7B shapes); the shape is read from config.json
+OLMO_SHAPE_KEYS = ("hidden_size", "intermediate_size", "num_hidden_layers", "num_attention_heads", "vocab_size")
+
+
+def check_olmo(cfg: Dict) -> None:
+    """refuses the settings of an olmo2 / olmo3 / olmoe config that LlamaDecoder would otherwise compute wrong or cannot run"""
+    mt = cfg.get("model_type", "")
+    missing = [k for k in OLMO_SHAPE_KEYS if k not in cfg]
+    if missing:
+        raise NotImplementedError(f"{mt}: a config without {', '.join(missing)} is not built (transformers would fill in its "
+                                  "config class's defaults; the shape is read from config.json only)")
+    if cfg.get("clip_qkv") is not None:
+        raise NotImplementedError(f"{mt}: clip_qkv={cfg['clip_qkv']} is not built (q / k / v are not clamped)")
+    act = cfg.get("hidden_act", "silu")
+    if act != "silu":
+        raise NotImplementedError(f"{mt}: hidden_act={act!r} is not built; only 'silu' (the SwiGLU MLP)")
+    hd = cfg.get("head_dim") or cfg["hidden_size"] // cfg["num_attention_heads"]
+    if hd not in (64, 128):
+        raise NotImplementedError(f"{mt}: head_dim={hd} is not built (the full-width q/k norm kernels take 64 / 128)")
+    nkv = cfg.get("num_key_value_heads") or cfg["num_attention_heads"]
+    if (cfg["num_attention_heads"] + nkv) * hd > 10240:
+        raise NotImplementedError(f"{mt}: {cfg['num_attention_heads']} q + {nkv} k heads of {hd} are not built (the q/k norm "
+                                  "kernel takes at most 10240 q|k columns)")
+    if cfg["hidden_size"] % 8 or cfg["hidden_size"] > 8192:
+        raise NotImplementedError(f"{mt}: hidden_size={cfg['hidden_size']} is not built (the post-sublayer norm takes a "
+                                  "multiple of 8 up to 8192)")
+    if cfg.get("attention_bias", False):
+        raise NotImplementedError(f"{mt}: attention_bias=true is not built")
+    check_rope_type(cfg)
+    if mt == "olmoe":
+        check_moe_bounds(cfg)
+    else:
+        sliding_windows(cfg)
 
 
 def check_roberta(cfg: Dict) -> None:

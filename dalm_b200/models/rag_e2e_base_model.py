@@ -69,7 +69,7 @@ def build_encoder(name_or_path: str, lora: bool, device: torch.device, state_dic
                   cfg: Optional[Dict] = None, autoregressive: bool = False, full: bool = False, bnb: bool = False):
     """BERT-family encoder (bge-*), (XLM-)RoBERTa encoder (multilingual-e5, bge-m3, xlm-roberta-*), ModernBERT encoder
     (gte-modernbert, modernbert-embed; frozen or fully fine-tuned), or — `retriever_is_autoregressive` — a Llama / Qwen2 / Qwen3 /
-    Mistral decoder (e5-mistral-7b-instruct, SFR-Embedding-Mistral) used as an encoder
+    Mistral / OLMo 2 / OLMo 3 decoder (e5-mistral-7b-instruct, SFR-Embedding-Mistral) used as an encoder
     (last hidden state, eos pooling; LoRA targets q_proj / v_proj: reference rag_e2e_base_model.py:66-70,84-90)"""
     cfg = cfg or params.load_config(name_or_path)
     kind = params.model_kind(cfg)
@@ -82,9 +82,9 @@ def build_encoder(name_or_path: str, lora: bool, device: torch.device, state_dic
     if not nf4:
         sd = _maybe_bnb(sd, bnb, full, device)
     if autoregressive:
-        if kind not in ("llama", "qwen2", "qwen3", "mistral"):
-            raise NotImplementedError("autoregressive retrievers are built for Llama, Qwen2 and Qwen3 models only; Mistral "
-                                      "runs as Llama with a sliding window")
+        if kind not in ("llama", "qwen2", "qwen3", "mistral", "olmo2", "olmo3"):
+            raise NotImplementedError("autoregressive retrievers are built for Llama, Qwen2 and Qwen3 models only, and for OLMo 2 "
+                                      "and OLMo 3; Mistral runs as Llama with a sliding window")
         return _named(LlamaDecoder(cfg, sd, device=device, lora=lora, lora_seed=0, full=full, nf4_storage=nf4), name_or_path)
     if kind not in ("bert", "roberta"):
         raise NotImplementedError("non-autoregressive retrievers must be BERT (bge-*) or (XLM-)RoBERTa (multilingual-e5, bge-m3) "
@@ -114,14 +114,19 @@ def _named(engine_model, name_or_path: str):
     return engine_model
 
 
-def _check_qwen3_moe_mode(full: bool, bnb: bool) -> None:
-    """Qwen3-MoE generators run frozen or with LoRA on q_proj / v_proj; every other mode is refused, naming why"""
+# the published checkpoint of each routed-MoE kind and its full fine-tuning footprint at ~18 bytes per parameter
+_MOE_FULL_FT = {"qwen3_moe": "Qwen3-30B-A3B would need ~550 GB", "olmoe": "OLMoE-1B-7B would need ~125 GB"}
+
+
+def _check_moe_mode(kind: str, full: bool, bnb: bool) -> None:
+    """routed-MoE generators (Qwen3-MoE, OLMoE) run frozen or with LoRA on q_proj / v_proj; every other mode is refused, naming
+    why"""
     if full:
-        raise NotImplementedError("full fine-tuning of a qwen3_moe generator is not built: grouped expert weight gradients are "
+        raise NotImplementedError(f"full fine-tuning of a {kind} generator is not built: grouped expert weight gradients are "
                                   "not built, and at ~18 bytes per parameter (fp32 master, gradient, Adam moments, bf16 copy) "
-                                  "Qwen3-30B-A3B would need ~550 GB; use LoRA (use_peft) on the generator")
+                                  f"{_MOE_FULL_FT[kind]}; use LoRA (use_peft) on the generator")
     if bnb:
-        raise NotImplementedError("use_bnb on a qwen3_moe generator is not built: the 4-bit treatment of the fused 3-D expert "
+        raise NotImplementedError(f"use_bnb on a {kind} generator is not built: the 4-bit treatment of the fused 3-D expert "
                                   "weights differs across transformers versions, so no single reference exists to match")
 
 
@@ -162,15 +167,15 @@ def build_decoder(name_or_path: str, lora: bool, device: torch.device, state_dic
                   cfg: Optional[Dict] = None, full: bool = False, bnb: bool = False) -> LlamaDecoder:
     cfg = cfg or params.load_config(name_or_path)
     kind = params.model_kind(cfg)                # raises for unsupported families
-    if kind == "qwen3_moe":
-        _check_qwen3_moe_mode(full, bnb)
+    if kind in _MOE_FULL_FT:
+        _check_moe_mode(kind, full, bnb)
     sd = state_dict if state_dict is not None else params.load_state_dict(name_or_path)
     nf4 = _nf4_storage(bnb, full, kind)
     if not nf4:
         sd = _maybe_bnb(sd, bnb, full, device)
     if kind == "falcon":
         dec = FalconDecoder(cfg, sd, device=device, lora=lora, full=full)      # raises for lora=True, like peft would
-    elif kind not in ("llama", "qwen2", "qwen3", "mistral", "qwen3_moe"):
+    elif kind not in ("llama", "qwen2", "qwen3", "mistral", "qwen3_moe", "olmo2", "olmo3", "olmoe"):
         raise NotImplementedError(f"generator of kind {kind!r} is not a causal decoder")
     else:
         dec = LlamaDecoder(cfg, sd, device=device, lora=lora, full=full, nf4_storage=nf4)

@@ -717,6 +717,136 @@ def qk_norm_rope_bwd_(dbuf: torch.Tensor, nheads: int, nq_heads: int, q_norm: to
     return dbuf
 
 
+def _chk_rope_tables(cos_t: torch.Tensor, sin_t: torch.Tensor, hd: int, what: str, T: Optional[int] = None) -> None:
+    _chk(cos_t, f32, what + " cos"); _chk(sin_t, f32, what + " sin")
+    if (cos_t.dim() != 2 or cos_t.shape[1] != hd // 2 or sin_t.shape != cos_t.shape or (T is not None and cos_t.shape[0] != T)
+            or not cos_t.is_contiguous() or not sin_t.is_contiguous()):
+        raise _lib.DalmB200Error(f"{what}: cos / sin must be contiguous fp32 [{T if T is not None else 'T'}, {hd // 2}]")
+
+
+def qk_fullnorm_rope_(buf: torch.Tensor, nq_heads: int, nk_heads: int, hd: int, q_norm: torch.Tensor, k_norm: torch.Tensor,
+                      eps: float, cos_t: torch.Tensor, sin_t: torch.Tensor, L: int = 0, pos: Optional[torch.Tensor] = None,
+                      pre: Optional[torch.Tensor] = None, rstd: Optional[torch.Tensor] = None,
+                      round_first: bool = False) -> torch.Tensor:
+    """OLMo 2 / 3 / OLMoE q/k RMSNorm over the whole q (nq_heads * hd) and k (nk_heads * hd) widths, then RoPE, in place on
+    the first (nq_heads + nk_heads) * hd columns of buf (bf16, token-major). round_first: OlmoeRMSNorm's rounding (bf16 before
+    the weight multiply) instead of Olmo2RMSNorm's. Positions: pos[M] (int64) when given, else row % L. pre (bf16
+    [M, >= width]) / rstd (fp32 [M, 2]) optionally receive the pre-norm columns and the q / k rstd. Allocates nothing."""
+    _chk(buf, bf16, "qk_fullnorm_rope buf")
+    _chk_rope_tables(cos_t, sin_t, hd, "qk_fullnorm_rope")
+    Nq, Nk = nq_heads * hd, nk_heads * hd
+    _vec(q_norm, f32, "qk_fullnorm_rope q_norm", Nq); _vec(k_norm, f32, "qk_fullnorm_rope k_norm", Nk)
+    M = buf.shape[0]
+    if buf.dim() != 2 or buf.shape[1] < Nq + Nk:
+        raise _lib.DalmB200Error(f"qk_fullnorm_rope: buf must be bf16 [M, >= {Nq + Nk}], got {tuple(buf.shape)}")
+    if pos is not None:
+        _vec(pos, i64, "qk_fullnorm_rope pos", M)
+    _chk_fullnorm_saves(pre, rstd, M, Nq + Nk, "qk_fullnorm_rope")
+    _lib.call("dalm_b200_qk_fullnorm_rope", _p(buf), _ld(buf), int(nq_heads), int(nq_heads + nk_heads), int(hd), _p(q_norm),
+              _p(k_norm), float(eps), int(bool(round_first)), _p(cos_t), _p(sin_t), cos_t.shape[0], int(L), _p(pos), M, _p(pre),
+              _ld(pre) if pre is not None else 0, _p(rstd), _ld(rstd) if rstd is not None else 0, _stream())
+    return buf
+
+
+def _chk_fullnorm_saves(pre: Optional[torch.Tensor], rstd: Optional[torch.Tensor], M: int, cols: int, what: str) -> None:
+    if pre is not None:
+        _chk(pre, bf16, what + " pre")
+        if pre.dim() != 2 or pre.shape[0] != M or pre.shape[1] < cols:
+            raise _lib.DalmB200Error(f"{what}: pre must be bf16 [{M}, >= {cols}], got {tuple(pre.shape)}")
+    if rstd is not None:
+        _chk(rstd, f32, what + " rstd")
+        if rstd.dim() != 2 or rstd.shape[0] != M or rstd.shape[1] < 2:
+            raise _lib.DalmB200Error(f"{what}: rstd must be fp32 [{M}, 2], got {tuple(rstd.shape)}")
+
+
+def qk_fullnorm_rope_bwd_(dbuf: torch.Tensor, nq_heads: int, nk_heads: int, hd: int, q_norm: torch.Tensor, k_norm: torch.Tensor,
+                          cos_t: torch.Tensor, sin_t: torch.Tensor, L: int, pre: torch.Tensor, rstd: torch.Tensor,
+                          dw_q: Optional[torch.Tensor] = None, dw_k: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """backward of `qk_fullnorm_rope_` (positions row % L), in place on d(out)'s q|k columns: they become d(pre-norm q|k).
+    dw_q / dw_k (fp32 [Nq] / [Nkv], both or neither) accumulate the norm weights' gradients (+=), deterministically
+    (`norm_wgrad_`, run first: it reads the rotated gradient)."""
+    _chk(dbuf, bf16, "qk_fullnorm_rope_bwd dbuf")
+    _chk_rope_tables(cos_t, sin_t, hd, "qk_fullnorm_rope_bwd", T=L)
+    Nq, Nk = nq_heads * hd, nk_heads * hd
+    _vec(q_norm, f32, "qk_fullnorm_rope_bwd q_norm", Nq); _vec(k_norm, f32, "qk_fullnorm_rope_bwd k_norm", Nk)
+    M = dbuf.shape[0]
+    if dbuf.dim() != 2 or dbuf.shape[1] < Nq + Nk:
+        raise _lib.DalmB200Error(f"qk_fullnorm_rope_bwd: dbuf must be bf16 [M, >= {Nq + Nk}], got {tuple(dbuf.shape)}")
+    if pre is None or rstd is None:
+        raise _lib.DalmB200Error("qk_fullnorm_rope_bwd: needs the saved pre-norm columns and rstd")
+    _chk_fullnorm_saves(pre, rstd, M, Nq + Nk, "qk_fullnorm_rope_bwd")
+    if (dw_q is None) != (dw_k is None):
+        raise _lib.DalmB200Error("qk_fullnorm_rope_bwd: dw_q and dw_k go together")
+    if dw_q is not None:
+        norm_wgrad_(dbuf[:, :Nq + Nk], pre, rstd, dw_q, dw_k, hd=hd, cos_t=cos_t, sin_t=sin_t, L=L)
+    _lib.call("dalm_b200_qk_fullnorm_rope_bwd", _p(dbuf), _ld(dbuf), int(nq_heads), int(nq_heads + nk_heads), int(hd), _p(q_norm),
+              _p(k_norm), _p(cos_t), _p(sin_t), int(L), _p(pre), _ld(pre), _p(rstd), _ld(rstd), M, _stream())
+    return dbuf
+
+
+NORM_WGRAD_MAX_SPLITS = 64
+
+
+def norm_wgrad_(dy: torch.Tensor, x: torch.Tensor, rstd: torch.Tensor, dw0: torch.Tensor, dw1: Optional[torch.Tensor] = None,
+                hd: int = 8, cos_t: Optional[torch.Tensor] = None, sin_t: Optional[torch.Tensor] = None, L: int = 0) -> None:
+    """RMSNorm weight gradient over bf16 inputs x [M, N] (normalised by rstd), without atomics (the same bits on every run):
+    dw0[c] += sum_m g[m,c] x[m,c] rstd[m,0] over the first len(dw0) columns, dw1 (+=) over the rest with rstd[m,1]. g = dy
+    (fp32 or bf16 [M, N]), un-rotated within heads of width hd at positions m % L when cos_t / sin_t are given. rstd: fp32 [M]
+    (one segment) or [M, 2]."""
+    M, N = x.shape[0], dy.shape[1]
+    _chk(x, bf16, "norm_wgrad x")
+    if dy.dtype not in (bf16, f32):
+        raise _lib.DalmB200Error("norm_wgrad: dy must be bf16 or fp32")
+    _chk(dy, dy.dtype, "norm_wgrad dy"); _chk(rstd, f32, "norm_wgrad rstd")
+    N0 = dw0.numel()
+    _vec(dw0, f32, "norm_wgrad dw0", N0)
+    if dw1 is not None:
+        _vec(dw1, f32, "norm_wgrad dw1", N - N0)
+    if dy.shape[0] != M or x.shape[1] < N or N0 + (dw1.numel() if dw1 is not None else 0) != N:
+        raise _lib.DalmB200Error(f"norm_wgrad: dy {tuple(dy.shape)}, x {tuple(x.shape)}, dw widths {N0} + "
+                                 f"{dw1.numel() if dw1 is not None else 0} disagree")
+    segs = 2 if dw1 is not None else 1
+    if rstd.shape[0] != M or (rstd.dim() == 2 and rstd.shape[1] < segs) or (rstd.dim() == 1 and segs == 2):
+        raise _lib.DalmB200Error(f"norm_wgrad: rstd must be fp32 [{M}] or [{M}, {segs}], got {tuple(rstd.shape)}")
+    if cos_t is not None:
+        _chk_rope_tables(cos_t, sin_t, hd, "norm_wgrad", T=L)
+    splits = max(1, min(NORM_WGRAD_MAX_SPLITS, (M + 63) // 64))
+    part = torch.empty(splits, N, dtype=f32, device=x.device)
+    _lib.call("dalm_b200_norm_wgrad", _p(dy), 1 if dy.dtype == f32 else 0, _ld(dy), _p(x), _ld(x), _p(rstd),
+              rstd.stride(0), int(N0), int(N), int(hd), _p(cos_t), _p(sin_t), int(L), M, _p(part), splits, _p(dw0), _p(dw1),
+              _stream())
+
+
+def postnorm_fwd(y: torch.Tensor, w: torch.Tensor, resid: torch.Tensor, eps: float, out16: Optional[torch.Tensor] = None):
+    """OLMo 2 / 3 post-sublayer norm and residual add: (out fp32 [M,H] = resid + bf16(w * y rstd), rstd fp32 [M]); y is the
+    bf16 sublayer output. out16 (bf16 [M,H] view) optionally receives bf16(out), the next GEMM's operand."""
+    _chk(y, bf16, "postnorm_fwd y")
+    M, H = y.shape
+    _rows32(resid, "postnorm_fwd resid", H, M); _vec(w, f32, "postnorm_fwd w", H)
+    if out16 is not None:
+        _bf16_rows(out16, "postnorm_fwd out16", M, H)
+    out = torch.empty(M, H, dtype=f32, device=y.device)
+    rstd = torch.empty(M, dtype=f32, device=y.device)
+    _lib.call("dalm_b200_postnorm_fwd", _p(y), _ld(y), _p(w), _p(resid), _p(out), _p(out16), _ld(out16) if out16 is not None else 0,
+              _p(rstd), M, H, float(eps), _stream())
+    return out, rstd
+
+
+def postnorm_bwd(y: torch.Tensor, w: torch.Tensor, rstd: torch.Tensor, dres: torch.Tensor, dh: Optional[torch.Tensor] = None):
+    """backward of `postnorm_fwd`: d = dres (fp32 [M,H]) + dh (bf16, the branch gradient joining the residual here; optional)
+    -> (d fp32, the residual gradient passed on; dy bf16 [M,H], the gradient of the sublayer output y)"""
+    _chk(y, bf16, "postnorm_bwd y")
+    M, H = y.shape
+    _rows32(dres, "postnorm_bwd dres", H, M); _vec(w, f32, "postnorm_bwd w", H); _vec(rstd, f32, "postnorm_bwd rstd", M)
+    if dh is not None:
+        _bf16_rows(dh, "postnorm_bwd dh", M, H)
+    d = torch.empty(M, H, dtype=f32, device=y.device)
+    dy = torch.empty(M, H, dtype=bf16, device=y.device)
+    _lib.call("dalm_b200_postnorm_bwd", _p(y), _ld(y), _p(w), _p(rstd), _p(dres), _p(dh), _ld(dh) if dh is not None else 0, _p(d),
+              _p(dy), _ld(dy), M, H, _stream())
+    return d, dy
+
+
 def interleave_gate_up(gate_w: torch.Tensor, up_w: torch.Tensor, block: int = 128) -> torch.Tensor:
     """[F,K] gate and up weights -> [2F,K] with rows [gate blk0 | up blk0 | gate blk1 | ...] (blocks of `block` features)"""
     F, K = gate_w.shape

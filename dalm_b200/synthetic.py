@@ -99,6 +99,55 @@ QWEN3_MOE_SHAPES: Dict[str, Dict] = {
                           mlp_only_layers=[], norm_topk_prob=True, tie_word_embeddings=False),
 }
 
+# OLMo 2 / OLMo 3 (HF Olmo2ForCausalLM / Olmo3ForCausalLM: post-sublayer norms, full-width q/k norm) and OLMoE (HF
+# OlmoeForCausalLM: pre-norm layers, full-width q/k norm, every MLP routed, experts of width intermediate_size). Published shapes written from the model cards'
+# config.json values (not re-fetched offline).
+OLMO_SHAPES: Dict[str, Dict] = {
+    "olmo2-tiny": dict(model_type="olmo2", hidden_size=256, num_hidden_layers=2, num_attention_heads=4, num_key_value_heads=4,
+                       intermediate_size=512),                                                   # head_dim 64
+    "olmo2-hd128-gqa": dict(model_type="olmo2", hidden_size=512, num_hidden_layers=2, num_attention_heads=4,
+                            num_key_value_heads=2, intermediate_size=1024),                     # head_dim 128, GQA
+    # layers 0-2 sliding (window 16), layer 3 full (Olmo3Config's default layer_types); YaRN with its default attention factor
+    "olmo3-tiny": dict(model_type="olmo3", hidden_size=256, num_hidden_layers=4, num_attention_heads=4, num_key_value_heads=2,
+                       intermediate_size=512, sliding_window=16, max_position_embeddings=512,
+                       rope_scaling=dict(rope_type="yarn", factor=4.0, original_max_position_embeddings=128, beta_fast=32,
+                                         beta_slow=1)),
+    # 3 sparse layers of 8 experts (top-2, not renormalised): a ragged token count leaves padding rows in every expert segment
+    "olmoe-tiny": dict(model_type="olmoe", hidden_size=256, num_hidden_layers=3, num_attention_heads=4, num_key_value_heads=4,
+                       intermediate_size=128, num_experts=8, num_experts_per_tok=2, norm_topk_prob=False),
+    "olmo-2-1124-7b": dict(model_type="olmo2", hidden_size=4096, num_hidden_layers=32, num_attention_heads=32,
+                           num_key_value_heads=32, intermediate_size=11008, vocab_size=100352, rope_theta=500000.0,
+                           max_position_embeddings=4096),
+    "olmo-3-7b": dict(model_type="olmo3", hidden_size=4096, num_hidden_layers=32, num_attention_heads=32, num_key_value_heads=32,
+                      intermediate_size=11008, vocab_size=100278, rope_theta=500000.0, max_position_embeddings=65536,
+                      sliding_window=4096, rope_scaling=dict(rope_type="yarn", factor=8.0, original_max_position_embeddings=8192,
+                                                             attention_factor=1.2079441541679836, beta_fast=32, beta_slow=1)),
+    "olmoe-1b-7b": dict(model_type="olmoe", hidden_size=2048, num_hidden_layers=16, num_attention_heads=16,
+                        num_key_value_heads=16, intermediate_size=1024, num_experts=64, num_experts_per_tok=8,
+                        norm_topk_prob=False, vocab_size=50304, rope_theta=10000.0,
+                        rms_norm_eps=1e-5),
+}
+OLMO_ARCH = {"olmo2": "Olmo2ForCausalLM", "olmo3": "Olmo3ForCausalLM", "olmoe": "OlmoeForCausalLM"}
+
+
+def olmo_config(name: str, vocab_size: Optional[int] = None) -> Dict:
+    """an OLMO_SHAPES entry as a full config.json: SwiGLU, no biases, untied head, ids 0 = eos / pad of the synthetic byte-level
+    tokenizer. olmo3 without layer_types gets Olmo3Config's (every fourth layer full)."""
+    s = dict(OLMO_SHAPES[name])
+    mt = s.pop("model_type")
+    cfg = dict(architectures=[OLMO_ARCH[mt]], model_type=mt, hidden_act="silu", rms_norm_eps=1e-6, rope_theta=500000.0,
+               rope_scaling=None, max_position_embeddings=4096, initializer_range=0.02, attention_bias=False,
+               attention_dropout=0.0, bos_token_id=None, eos_token_id=0, pad_token_id=0, tie_word_embeddings=False)
+    if mt == "olmoe":
+        cfg.update(clip_qkv=None, output_router_logits=False, router_aux_loss_coef=0.01)
+    cfg.update(s)
+    if vocab_size is not None:
+        cfg["vocab_size"] = vocab_size
+    cfg.setdefault("vocab_size", 100352)
+    if mt == "olmo3" and "layer_types" not in cfg:
+        cfg["layer_types"] = ["sliding_attention" if (i + 1) % 4 != 0 else "full_attention" for i in range(cfg["num_hidden_layers"])]
+    return cfg
+
 
 # XLM-RoBERTa / RoBERTa encoders: BERT's layer, positions counted from pad_token_id + 1
 ROBERTA_SHAPES: Dict[str, Dict] = {
@@ -581,7 +630,8 @@ def write_model_dir(out_dir: str, kind: str, name: str, vocab_size: Optional[int
     safetensors in HF parameter naming so both transformers (oracle) and dalm_b200 (product) can load the same directory.
     generation_config: written as generation_config.json when given (e.g. QWEN2_GENERATION["base"]). bias_std: std of the
     random attention biases, qk_norm_std the spread of Qwen3's q / k norm weights around 1, router_std the std of Qwen3-MoE's
-    router weights (engine/params.random_state_dict). 'qwen3_moe' takes a QWEN3_MOE_SHAPES name and Qwen2's tokenizer."""
+    router weights (engine/params.random_state_dict). 'qwen3_moe' takes a QWEN3_MOE_SHAPES name and Qwen2's tokenizer;
+    'olmo2' / 'olmo3' / 'olmoe' an OLMO_SHAPES name of that kind and the same byte-level tokenizer."""
     os.makedirs(out_dir, exist_ok=True)
     if kind == "bert":
         cfg = bert_config(name, vocab_size or 30522)
@@ -607,6 +657,11 @@ def write_model_dir(out_dir: str, kind: str, name: str, vocab_size: Optional[int
     elif kind == "qwen3_moe":
         cfg = qwen3_moe_config(name, vocab_size or 151936)
         build_qwen2_tokenizer(out_dir, cfg["vocab_size"])
+    elif kind in ("olmo2", "olmo3", "olmoe"):
+        cfg = olmo_config(name, vocab_size)
+        if cfg["model_type"] != kind:
+            raise ValueError(f"{name} is an {cfg['model_type']} shape, not {kind}")
+        build_qwen2_tokenizer(out_dir, cfg["vocab_size"])          # a byte-level BPE, as OLMo's own tokenizers are
     elif kind == "mistral":
         cfg = mistral_config(name, vocab_size)
         if headless is not None:

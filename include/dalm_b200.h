@@ -160,6 +160,15 @@ int dalm_b200_rmsnorm_fwd(const float* x, const float* g, void* h, long long ldh
                           void* stream);
 int dalm_b200_rmsnorm_bwd(const float* x, const float* g, const float* rstd, const void* dh, long long lddh,
                           const float* dres_in, float* dres_out, void* dres16, long long ld16, int M, int H, void* stream);
+/* postnorm_fwd: OLMo 2 / 3 post-sublayer RMSNorm with the residual add: out (fp32 [M,H]) = resid + bf16(w * y rstd), y the bf16
+ *   sublayer output (row stride ldy), rstd (fp32 [M]) = rsqrt(mean(y^2) + eps); out16 (bf16, ld16; may be NULL) = bf16(out).
+ *   H % 8 == 0, H <= 8192.
+ * postnorm_bwd: d = dres_in + dh (dh: bf16 [M,H] or NULL) -> dres_out = d (fp32), dy (bf16) = rstd (w d - y_hat mean(w d y_hat)),
+ *   y_hat = y rstd: the gradient the o_proj / down dgrad reads. */
+int dalm_b200_postnorm_fwd(const void* y, long long ldy, const float* w, const float* resid, float* out, void* out16, long long ld16,
+                           float* rstd, int M, int H, float eps, void* stream);
+int dalm_b200_postnorm_bwd(const void* y, long long ldy, const float* w, const float* rstd, const float* dres_in, const void* dh,
+                           long long lddh, float* dres_out, void* dy, long long lddy, int M, int H, void* stream);
 int dalm_b200_bert_embed(const int64_t* ids, const void* word, const void* pos, const void* type0, float* z, int M, int L,
                          int H, int V, void* stream);
 /* RoBERTa / XLM-RoBERTa (HF create_position_ids_from_input_ids): position = pad_id + (id != pad_id) * (count of non-pad ids in
@@ -278,6 +287,28 @@ int dalm_b200_qk_norm_rope(void* buf, long long ld, int nheads, int nq_heads, co
 int dalm_b200_qk_norm_rope_bwd(void* dbuf, long long ld, int nheads, int nq_heads, const float* q_norm, const float* k_norm,
                                const float* cos_t, const float* sin_t, int L, const void* pre, long long ld_pre, const float* rstd,
                                long long ld_rstd, int M, float* dw_q, float* dw_k, void* stream);
+/* qk_fullnorm_rope: OLMo 2 / OLMo 3 / OLMoE q/k RMSNorm over the whole projection width, then RoPE (HF rotate_half, head_dim
+ * hd = 64 or 128), in place on the first nheads * hd columns of a token-major bf16 buffer [M, ld]: q = columns [0, Nq), Nq =
+ * nq_heads * hd, normalised with q_norm (fp32 [Nq]); k = the next Nkv = (nheads - nq_heads) * hd columns with k_norm (fp32
+ * [Nkv]); Nq + Nkv <= 10240. Normalised value: bf16(w * x rstd) (Olmo2RMSNorm), or with round_first bf16(w * bf16(x rstd))
+ * (OlmoeRMSNorm). Position of row m: clamp(pos[m], 0, T-1) when pos != NULL, else m % L; cos / sin fp32 [T, hd/2]. pre (bf16,
+ * ld_pre) and rstd (fp32 [M, 2]: q, k; ld_rstd) optionally receive the pre-norm values and the two rstd. No allocation, no host
+ * synchronisation.
+ * qk_fullnorm_rope_bwd: in place on d(out) of the same columns (positions m % L): un-rotates, then the full-width RMSNorm
+ * backward from the saved pre / rstd. Weight gradients: norm_wgrad.
+ * norm_wgrad: dw0[c] += sum_m g[m,c] x[m,c] rstd[m, 0] for c < ncols0, dw1[c - ncols0] += ... rstd[m, 1] for c >= ncols0; g = dy
+ * (fp32 when dy_f32, else bf16), un-rotated within heads of width hd (64 / 128) at positions m % L when cos_t != NULL (hd = 8:
+ * no rotation); x bf16. Rows are split into `splits` fixed slices, whose column sums go to part (fp32 [splits, ncols]) and are
+ * then added in slice order: no atomics, the same bits on every run. */
+int dalm_b200_qk_fullnorm_rope(void* buf, long long ld, int nq_heads, int nheads, int hd, const float* q_norm, const float* k_norm,
+                               float eps, int round_first, const float* cos_t, const float* sin_t, int T, int L, const int64_t* pos,
+                               int M, void* pre, long long ld_pre, float* rstd, long long ld_rstd, void* stream);
+int dalm_b200_qk_fullnorm_rope_bwd(void* dbuf, long long ld, int nq_heads, int nheads, int hd, const float* q_norm,
+                                   const float* k_norm, const float* cos_t, const float* sin_t, int L, const void* pre,
+                                   long long ld_pre, const float* rstd, long long ld_rstd, int M, void* stream);
+int dalm_b200_norm_wgrad(const void* dy, int dy_f32, long long ld_dy, const void* x, long long ld_x, const float* rstd,
+                         long long ld_rstd, int ncols0, int ncols, int hd, const float* cos_t, const float* sin_t, int L, int M,
+                         float* part, int splits, float* dw0, float* dw1, void* stream);
 int dalm_b200_attention_decode(const void* qkv, long long ldq, int q_col, int k_col, int v_col, void* cache_k, void* cache_v,
                                long long cache_sb, long long cache_st, const int64_t* mask, long long ldm, void* out,
                                long long ldo, int B, int Hq, int Hkv, int D, int cur, const int* cur_dev, int T, float scale,

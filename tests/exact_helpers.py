@@ -192,6 +192,117 @@ def _pick_block_n(M, N, sms):
 
 
 # ----------------------------------------------------------------------------------------------------------------
+# routed experts: the grouped GEMM over padded expert segments, and the routing's definition
+# ----------------------------------------------------------------------------------------------------------------
+def _segments(counts):
+    """padded row offsets of segments with these row counts"""
+    off, o = [], 0
+    for c in counts:
+        off.append(o)
+        o += -(-c // 128) * 128
+    return off, o
+
+
+def _grouped_case(ops, dev, counts, extra, layout, swiglu, N, K, max_ctas, seed, experts=None, E=None, device_ref=False):
+    """gemm_grouped on segments of counts[i] rows (padded to the 128-row tile, in this order) with segment i on expert
+    experts[i] (default i) of an E-expert stack (default len(counts)), `extra` unused tiles after the live ones. Integer
+    operands in [-2, 2]: every row of every segment bit-exact against fp64, the rows past the live tiles untouched.
+    device_ref: operands drawn on the device and the fp64 reference computed there, one segment at a time (production
+    widths); otherwise drawn from a host generator and checked on the host."""
+    experts = list(range(len(counts))) if experts is None else list(experts)
+    E = len(counts) if E is None else E
+    off, live_rows = _segments(counts)
+    n_tiles = live_rows // 128 + extra
+    rows = 128 * n_tiles
+    wshape = (E, N, K) if layout == 0 else (E, K, N)
+    wbuf = torch.full((E + 1,) + wshape[1:], float("nan"), dtype=bf16, device=dev)   # a NaN expert after the last one
+    if device_ref:
+        g = torch.Generator(device=dev).manual_seed(seed)
+        buf = torch.full((rows + PAD_R, K + PAD_C), float("nan"), dtype=bf16, device=dev)
+        a = buf[:rows, :K]
+        a.copy_(torch.randint(-2, 3, (rows, K), generator=g, device=dev, dtype=torch.int8))
+        live_row = torch.zeros(rows, dtype=torch.bool, device=dev)
+        for o, c in zip(off, counts):
+            live_row[o:o + c] = True
+        a.masked_fill_(~live_row[:, None], float("nan"))            # padding rows of every segment and the tail: NaN
+        wbuf[:E].copy_(torch.randint(-2, 3, wshape, generator=g, device=dev, dtype=torch.int8))
+        a_ref = a
+    else:
+        g = torch.Generator().manual_seed(seed)
+        a_host = torch.full((rows, K), float("nan"))
+        for o, c in zip(off, counts):
+            a_host[o:o + c] = _ints((c, K), g)
+        a = _poisoned(a_host.to(dev, bf16))
+        wbuf[:E] = _ints(wshape, g).to(dev, bf16)
+        a_ref = a_host
+    w = wbuf[:E]
+    tiles = torch.full((n_tiles,), -1, dtype=torch.int32)
+    for o, c, e in zip(off, counts, experts):
+        tiles[o // 128:(o + -(-c // 128) * 128) // 128] = e
+    tile_expert = tiles.to(dev)
+    live = torch.tensor([live_rows // 128], dtype=torch.int32, device=dev)
+    out = Guarded(rows, N, bf16, dev)
+    act = Guarded(rows, N // 2, bf16, dev) if swiglu else None
+    ops.gemm_grouped(a, w, tile_expert, live, out=out.view, layout=layout, swiglu=swiglu, act=act.view if swiglu else None,
+                     max_ctas=max_ctas)
+    segs = counts if len(counts) <= 12 else f"{len(counts)} segments, {sum(counts)} rows"
+    what = f"gemm_grouped layout {layout} swiglu {swiglu} counts {segs} +{extra} tiles N {N} K {K} max_ctas {max_ctas}"
+    if device_ref:
+        got, got_act = out.view, act.view if swiglu else None
+    else:
+        w64 = w.double().cpu()
+        got, got_act = out.view.cpu(), act.view.cpu() if swiglu else None
+    for i, (o, c, e) in enumerate(zip(off, counts, experts)):
+        if c == 0:
+            continue
+        x = a_ref[o:o + c].double()
+        we = w[e].double() if device_ref else w64[e]
+        acc = x @ (we.t() if layout == 0 else we)
+        _expect_equal(got[o:o + c], acc.to(bf16), f"{what} segment {i} (expert {e}, rows from {o})", 128, 256)
+        if swiglu:
+            blk = acc.view(c, N // 256, 2, 128)
+            gate, up = blk[:, :, 0].reshape(c, N // 2), blk[:, :, 1].reshape(c, N // 2)
+            ref = gate * torch.sigmoid(gate) * up
+            _expect_close(got_act[o:o + c], ref, _ulp_bf16(ref) + 2.0 ** -20 * ref.abs() + 2.0 ** -100,
+                          f"{what} act segment {i} (expert {e})", 128, 128)
+    # the tail tiles past the live count are not computed: their rows keep the sentinel
+    for v, nm in ((out, "out"), (act, "act")):
+        if v is None:
+            continue
+        tail = v.view[live_rows:].contiguous().view(torch.int16)
+        assert bool((tail == v.bits).all()), f"{what}: {nm} rows past the live tiles were written"
+        v.check(f"{what} {nm}")
+
+
+def _check_routing(r, ids, E):
+    """a moe_permute result against its definition: counts, padded segment offsets, the tile -> expert table, the live tile
+    count, and the pair <-> row maps (within a segment, pairs by token, then by slot)"""
+    ids = ids.cpu().long().view(-1)
+    P = ids.numel()
+    counts = torch.bincount(ids, minlength=E)
+    assert torch.equal(r.counts.cpu().long(), counts)
+    pad = (counts + 127) // 128 * 128
+    off = torch.cat([torch.zeros(1, dtype=torch.long), pad.cumsum(0)])
+    assert torch.equal(r.seg_off.cpu().long(), off)
+    live = int(off[-1]) // 128
+    assert int(r.live.item()) == live
+    te = torch.full((r.n_tiles,), -1, dtype=torch.long)
+    for e in range(E):
+        te[int(off[e]) // 128:int(off[e + 1]) // 128] = e
+    assert torch.equal(r.tile_expert.cpu().long(), te)
+    pr = r.pair_row.cpu().long()
+    want = torch.empty(P, dtype=torch.long)
+    for e in range(E):
+        sel = (ids == e).nonzero().view(-1)                 # pair order: by token, then slot
+        want[sel] = off[e] + torch.arange(sel.numel())
+    assert torch.equal(pr, want), "pair -> row map"
+    rp = r.row_pair.cpu().long()[:live * 128]
+    wrp = torch.full((live * 128,), -1, dtype=torch.long)
+    wrp[want] = torch.arange(P)
+    assert torch.equal(rp, wrp), "row -> pair map"
+
+
+# ----------------------------------------------------------------------------------------------------------------
 # attention against fp64
 # ----------------------------------------------------------------------------------------------------------------
 def _attn_fns(ops, kind):

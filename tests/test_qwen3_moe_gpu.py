@@ -12,8 +12,8 @@ on the same routing, and bit-identical from run to run.
 import pytest
 import torch
 
-from exact_helpers import (Guarded, _expect_close, _expect_equal, _ints, _poisoned, _ulp_bf16, _ulp_f32,  # noqa: F401
-                           dev, ops)
+from exact_helpers import (Guarded, _check_routing, _expect_close, _expect_equal, _grouped_case, _poisoned,  # noqa: F401
+                           _ulp_bf16, _ulp_f32, dev, ops)
 
 bf16, f32, f64, i32 = torch.bfloat16, torch.float32, torch.float64, torch.int32
 
@@ -21,15 +21,6 @@ bf16, f32, f64, i32 = torch.bfloat16, torch.float32, torch.float64, torch.int32
 # ----------------------------------------------------------------------------------------------------------------
 # grouped GEMM
 # ----------------------------------------------------------------------------------------------------------------
-def _segments(counts):
-    """padded row offsets of segments with these row counts"""
-    off, o = [], 0
-    for c in counts:
-        off.append(o)
-        o += -(-c // 128) * 128
-    return off, o
-
-
 # per-expert row counts: empty experts, segments of 1 row and of 128 n rows, everything on one expert; `extra` unused tail
 # tiles past the live ones
 COUNT_CASES = [
@@ -38,53 +29,6 @@ COUNT_CASES = [
     ([1, 1, 1, 1, 1, 1, 1, 1, 1, 1], 3),
     ([128, 384, 0, 129, 127], 0),
 ]
-
-
-def _grouped_case(ops, dev, counts, extra, layout, swiglu, N, K, max_ctas, seed):
-    g = torch.Generator().manual_seed(seed)
-    E = len(counts)
-    off, live_rows = _segments(counts)
-    n_tiles = live_rows // 128 + extra
-    rows = 128 * n_tiles
-    a_host = torch.full((rows, K), float("nan"))
-    for e, c in enumerate(counts):
-        a_host[off[e]:off[e] + c] = _ints((c, K), g)
-    a = _poisoned(a_host.to(dev, bf16))
-    wshape = (E, N, K) if layout == 0 else (E, K, N)
-    wbuf = torch.full((E + 1,) + wshape[1:], float("nan"), dtype=bf16, device=dev)   # a NaN expert after the last one
-    wbuf[:E] = _ints(wshape, g).to(dev, bf16)
-    w = wbuf[:E]
-    tiles = torch.full((n_tiles,), -1, dtype=i32)
-    for e, c in enumerate(counts):
-        tiles[off[e] // 128:(off[e] + -(-c // 128) * 128) // 128] = e
-    tile_expert = tiles.to(dev)
-    live = torch.tensor([live_rows // 128], dtype=i32, device=dev)
-    out = Guarded(rows, N, bf16, dev)
-    act = Guarded(rows, N // 2, bf16, dev) if swiglu else None
-    ops.gemm_grouped(a, w, tile_expert, live, out=out.view, layout=layout, swiglu=swiglu, act=act.view if swiglu else None,
-                     max_ctas=max_ctas)
-    what = f"gemm_grouped layout {layout} swiglu {swiglu} counts {counts} +{extra} tiles N {N} K {K} max_ctas {max_ctas}"
-    w64 = w.double().cpu()
-    got, got_act = out.view.cpu(), act.view.cpu() if swiglu else None
-    for e, c in enumerate(counts):
-        if c == 0:
-            continue
-        x = a_host[off[e]:off[e] + c].double()
-        acc = x @ (w64[e].t() if layout == 0 else w64[e])
-        _expect_equal(got[off[e]:off[e] + c], acc.to(bf16), f"{what} expert {e}", 128, 256)
-        if swiglu:
-            blk = acc.view(c, N // 256, 2, 128)
-            gate, up = blk[:, :, 0].reshape(c, N // 2), blk[:, :, 1].reshape(c, N // 2)
-            ref = gate * torch.sigmoid(gate) * up
-            _expect_close(got_act[off[e]:off[e] + c], ref, _ulp_bf16(ref) + 2.0 ** -20 * ref.abs() + 2.0 ** -100,
-                          f"{what} act expert {e}", 128, 128)
-    # the tail tiles past the live count are not computed: their rows keep the sentinel
-    for v, nm in ((out, "out"), (act, "act")):
-        if v is None:
-            continue
-        tail = v.view[live_rows:].contiguous().view(torch.int16)
-        assert bool((tail == v.bits).all()), f"{what}: {nm} rows past the live tiles were written"
-        v.check(f"{what} {nm}")
 
 
 @pytest.mark.gpu
@@ -133,32 +77,6 @@ def test_router(ops, dev, E, k, norm):
     p = _probs64(logits).gather(1, ids.long())
     ref = p / p.sum(-1, keepdim=True) if norm else p
     _expect_close(w, ref, 8 * _ulp_f32(ref), f"router weights E {E} k {k} norm {norm}")
-
-
-def _check_routing(r, ids, E):
-    ids = ids.cpu().long().view(-1)
-    P = ids.numel()
-    counts = torch.bincount(ids, minlength=E)
-    assert torch.equal(r.counts.cpu().long(), counts)
-    pad = (counts + 127) // 128 * 128
-    off = torch.cat([torch.zeros(1, dtype=torch.long), pad.cumsum(0)])
-    assert torch.equal(r.seg_off.cpu().long(), off)
-    live = int(off[-1]) // 128
-    assert int(r.live.item()) == live
-    te = torch.full((r.n_tiles,), -1, dtype=torch.long)
-    for e in range(E):
-        te[int(off[e]) // 128:int(off[e + 1]) // 128] = e
-    assert torch.equal(r.tile_expert.cpu().long(), te)
-    pr = r.pair_row.cpu().long()
-    want = torch.empty(P, dtype=torch.long)
-    for e in range(E):
-        sel = (ids == e).nonzero().view(-1)                 # pair order: by token, then slot
-        want[sel] = off[e] + torch.arange(sel.numel())
-    assert torch.equal(pr, want), "pair -> row map"
-    rp = r.row_pair.cpu().long()[:live * 128]
-    wrp = torch.full((live * 128,), -1, dtype=torch.long)
-    wrp[want] = torch.arange(P)
-    assert torch.equal(rp, wrp), "row -> pair map"
 
 
 @pytest.mark.gpu

@@ -62,6 +62,36 @@ def _bf16_rows(t: torch.Tensor, name: str, rows: int, cols: int) -> None:
         raise _lib.DalmB200Error(f"{name}: expected a bf16 view of at least [{rows}, {cols}], got shape {tuple(t.shape)}")
 
 
+def _out_rows(t: torch.Tensor, name: str, M: int, N: int, dev: torch.device, dtypes=(bf16, f32)) -> None:
+    """an output or residual the GEMM epilogues index as t[m * ld + n], m < M, n < N: on the operands' device, with a
+    contiguous inner dimension and at least [M, N] elements (a smaller view would be written or read past)"""
+    if not t.is_cuda or t.device != dev:
+        raise _lib.DalmB200Error(f"{name}: expected a tensor on {dev}, got one on {t.device}")
+    if t.dtype not in dtypes:
+        raise _lib.DalmB200Error(f"{name}: expected dtype {' or '.join(str(d) for d in dtypes)}, got {t.dtype}")
+    if t.dim() != 2 or t.stride(-1) != 1 or t.shape[0] < M or t.shape[1] < N:
+        raise _lib.DalmB200Error(f"{name}: expected a 2-D view of at least [{M}, {N}] with contiguous rows, got shape "
+                                 f"{tuple(t.shape)} strides {t.stride()}")
+
+
+def _operands(a: torch.Tensor, b: torch.Tensor, what: str, layout: int = 0, K: Optional[int] = None,
+              N: Optional[int] = None) -> Tuple[int, int, int]:
+    """2-D GEMM operands on one device in `layout` (see `gemm`) -> (M, K, N). Without a K override the contraction extents
+    of a and b must agree; overrides must fit inside the operands (the kernels read K elements of both and N of b)"""
+    if a.dim() != 2 or b.dim() != 2 or b.device != a.device:
+        raise _lib.DalmB200Error(f"{what}: expected 2-D operands on one device, got {tuple(a.shape)} on {a.device} and "
+                                 f"{tuple(b.shape)} on {b.device}")
+    M, ka = (a.shape[1], a.shape[0]) if layout == 2 else (a.shape[0], a.shape[1])
+    kb, nb = (b.shape[1], b.shape[0]) if layout == 0 else (b.shape[0], b.shape[1])
+    if K is None and ka != kb:
+        raise _lib.DalmB200Error(f"{what}: the operands disagree on K ({ka} vs {kb}): a {tuple(a.shape)}, b {tuple(b.shape)}")
+    K = ka if K is None else K
+    N = nb if N is None else N
+    if K > min(ka, kb) or N > nb:
+        raise _lib.DalmB200Error(f"{what}: K={K} / N={N} exceed the operands a {tuple(a.shape)}, b {tuple(b.shape)}")
+    return M, K, N
+
+
 def _reach(t: torch.Tensor) -> int:
     """largest element offset a (non-negatively strided) view covers"""
     return sum((s - 1) * st for s, st in zip(t.shape, t.stride()))
@@ -250,24 +280,14 @@ def gemm(a: torch.Tensor, b: torch.Tensor, out: Optional[torch.Tensor] = None, *
     act 1: GELU(erf).  act 2: GELU backward - out = bf16(alpha * A @ B + bias) * gelu'(resid), resid = the bf16 pre-activation
     (multiplied, not added): d(pre) straight out of the output projection's dgrad GEMM."""
     _chk(a, bf16, "gemm a"); _chk(b, bf16, "gemm b")
-    if layout == 0:
-        M, Kd, Nd = a.shape[0], a.shape[1], b.shape[0]
-    elif layout == 1:
-        M, Kd, Nd = a.shape[0], a.shape[1], b.shape[1]
-    else:
-        M, Kd, Nd = a.shape[1], a.shape[0], b.shape[1]
-    K = Kd if K is None else K
-    N = Nd if N is None else N
+    M, K, N = _operands(a, b, f"gemm layout {layout}", layout, K, N)
     if out is None:
         out = torch.empty(M, N, dtype=out_dtype, device=a.device)
-    if out.dtype not in (bf16, f32):
-        raise _lib.DalmB200Error("gemm: out must be bf16 or fp32")
-    if bias is not None:
-        _chk(bias, f32, "gemm bias")
+    _out_rows(out, "gemm out", M, N, a.device)
+    _chk_bias(bias, N, "gemm bias")
     rf32 = 0
     if resid is not None:
-        if resid.dtype not in (bf16, f32):
-            raise _lib.DalmB200Error("gemm: resid must be bf16 or fp32")
+        _out_rows(resid, "gemm resid", M, N, a.device)
         rf32 = 1 if resid.dtype == f32 else 0
     if max_ctas == 0 and GEMM_MAX_CTAS:
         max_ctas = GEMM_MAX_CTAS
@@ -571,12 +591,13 @@ def gemm_swiglu(a: torch.Tensor, w_il: torch.Tensor, gu: Optional[torch.Tensor] 
     """LlamaMLP's gate|up projection with SiLU(gate) * up in the GEMM epilogue. w_il: [2F, K] bf16, gate / up rows interleaved in
     blocks of 128 features (see `interleave_gate_up`). -> (gu [M,2F] interleaved bf16, act [M,F] bf16)"""
     _chk(a, bf16, "gemm_swiglu a"); _chk(w_il, bf16, "gemm_swiglu w")
-    M, K = a.shape
-    N = w_il.shape[0]
+    M, K, N = _operands(a, w_il, "gemm_swiglu")
     if gu is None:
         gu = torch.empty(M, N, dtype=bf16, device=a.device)
     if act is None:
         act = torch.empty(M, N // 2, dtype=bf16, device=a.device)
+    _out_rows(gu, "gemm_swiglu gu", M, N, a.device, (bf16,))
+    _out_rows(act, "gemm_swiglu act", M, N // 2, a.device, (bf16,))
     timer = GEMM_TIMER
     if timer is not None:
         timer.begin(2.0 * M * N * K, (M, N, K, 0, "bfloat16", "swiglu", "-"))
@@ -598,14 +619,14 @@ def gemm_gelu(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = N
     """intermediate projection of a GELU MLP with the activation in the GEMM epilogue: -> (pre = a w^T + bias, gelu(pre)), both
     bf16 [M,N], one launch. Bit-identical to gemm(...) followed by gelu_fwd (the activation is taken of the rounded bf16 pre)."""
     _chk(a, bf16, "gemm_gelu a"); _chk(w, bf16, "gemm_gelu w")
-    M, K = a.shape
-    N = w.shape[0]
-    if bias is not None:
-        _chk(bias, f32, "gemm_gelu bias")
+    M, K, N = _operands(a, w, "gemm_gelu")
+    _chk_bias(bias, N, "gemm_gelu bias")
     if pre is None:
         pre = torch.empty(M, N, dtype=bf16, device=a.device)
     if act is None:
         act = torch.empty(M, N, dtype=bf16, device=a.device)
+    _out_rows(pre, "gemm_gelu pre", M, N, a.device, (bf16,))
+    _out_rows(act, "gemm_gelu act", M, N, a.device, (bf16,))
     timer = GEMM_TIMER
     if timer is not None:
         timer.begin(2.0 * M * N * K, (M, N, K, 0, "bfloat16", "gelu2", "bias" if bias is not None else "-"))
@@ -633,8 +654,7 @@ def gemm_rope(a: torch.Tensor, w: torch.Tensor, cos_t: torch.Tensor, sin_t: torc
     [0, nq_heads) with q_norm, the rest with k_norm. pre_out (bf16 [M, rope_cols]) / rstd_out (fp32 [M, rope_cols // 128])
     receive the pre-norm columns and the heads' rstd, which `qk_norm_rope_bwd_` reads."""
     _chk(a, bf16, "gemm_rope a"); _chk(w, bf16, "gemm_rope w"); _chk(cos_t, f32, "gemm_rope cos"); _chk(sin_t, f32, "gemm_rope sin")
-    M, K = a.shape
-    N = w.shape[0]
+    M, K, N = _operands(a, w, "gemm_rope")
     _chk_bias(bias, N, "gemm_rope bias")
     if cos_t.shape != (L, 64) or sin_t.shape != (L, 64) or not cos_t.is_contiguous() or not sin_t.is_contiguous():
         raise _lib.DalmB200Error("gemm_rope: cos / sin must be contiguous fp32 [L, 64] (head_dim 128)")
@@ -645,6 +665,7 @@ def gemm_rope(a: torch.Tensor, w: torch.Tensor, cos_t: torch.Tensor, sin_t: torc
         _chk_norm_saves(pre_out, rstd_out, M, rope_cols, "gemm_rope")
     if out is None:
         out = torch.empty(M, N, dtype=bf16, device=a.device)
+    _out_rows(out, "gemm_rope out", M, N, a.device, (bf16,))
     timer = GEMM_TIMER
     if timer is not None:
         timer.begin(2.0 * M * N * K, (M, N, K, 0, "bfloat16", "rope" if q_norm is None else "norm_rope",
@@ -1103,15 +1124,13 @@ def decode_gemm(a: torch.Tensor, w: torch.Tensor, out: Optional[torch.Tensor] = 
     """out[M,N] = act(a[M,K] @ w[N,K]^T + bias) + resid for the M <= 16 token rows of a decode step: weight-streaming kernel,
     every weight read once. a, w bf16 with contiguous rows (row strides multiples of 8); bias fp32 [N]; resid / out bf16 or fp32."""
     _chk(a, bf16, "decode_gemm a"); _chk(w, bf16, "decode_gemm w")
-    M, K = a.shape
-    N = w.shape[0]
-    if w.shape[1] != K:
-        raise _lib.DalmB200Error(f"decode_gemm: a is [{M},{K}] but w is {tuple(w.shape)}")
+    M, K, N = _operands(a, w, "decode_gemm")
     _chk_bias(bias, N, "decode_gemm bias")
     if out is None:
         out = torch.empty(M, N, dtype=out_dtype, device=a.device)
-    if out.dtype not in (bf16, f32) or (resid is not None and resid.dtype not in (bf16, f32)):
-        raise _lib.DalmB200Error("decode_gemm: out / resid must be bf16 or fp32")
+    _out_rows(out, "decode_gemm out", M, N, a.device)
+    if resid is not None:
+        _out_rows(resid, "decode_gemm resid", M, N, a.device)
     _lib.call("dalm_b200_decode_gemm", _p(a), _ld(a), _p(w), _ld(w), _p(out), _ld(out), 1 if out.dtype == f32 else 0, _p(bias), _p(resid),
               _ld(resid) if resid is not None else 0, 1 if (resid is not None and resid.dtype == f32) else 0, int(act), M, N, K,
               _stream())

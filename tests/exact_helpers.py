@@ -111,28 +111,31 @@ def _ulp_f32(x):
     return torch.pow(2.0, torch.floor(torch.log2(x.abs().clamp_min(2.0 ** -126))) - 23)
 
 
-def _where(bad, what, tile_m=128, tile_n=None):
+def _where(bad, what, tile_m=128, tile_n=None, row0=0):
     r, c = bad.nonzero()[0].tolist()
+    r += row0
     tile = f" = tile (m {r // tile_m}, n {c // tile_n})" if tile_n else ""
-    return f"{what}: {int(bad.sum())} of {bad.numel()} elements wrong; first at (row {r}, col {c}){tile}"
+    rows = f" of rows from {row0}" if row0 else ""
+    return f"{what}: {int(bad.sum())} of {bad.numel()} elements{rows} wrong; first at (row {r}, col {c}){tile}"
 
 
-def _expect_equal(got, want, what, tile_m=128, tile_n=None):
-    """got (kernel output, any float dtype) == want (same dtype) element for element (+0 == -0), no NaN"""
+def _expect_equal(got, want, what, tile_m=128, tile_n=None, row0=0):
+    """got (kernel output, any float dtype) == want (same dtype) element for element (+0 == -0), no NaN. row0: the row of
+    the full output where these rows start (a chunk of a large output), for the failure message"""
     g, w = got.double(), want.double()
     bad = (g != w) | torch.isnan(g)
     if bad.any():
         r, c = bad.nonzero()[0].tolist()
-        pytest.fail(_where(bad, what, tile_m, tile_n) + f": got {g[r, c].item()!r}, want {w[r, c].item()!r}")
+        pytest.fail(_where(bad, what, tile_m, tile_n, row0) + f": got {g[r, c].item()!r}, want {w[r, c].item()!r}")
 
 
-def _expect_close(got, ref, tol, what, tile_m=128, tile_n=None):
+def _expect_close(got, ref, tol, what, tile_m=128, tile_n=None, row0=0):
     """|got - ref| <= tol element-wise (fp64), no NaN"""
     g = got.double()
     bad = ~((g - ref).abs() <= tol)
     if bad.any():
         r, c = bad.nonzero()[0].tolist()
-        pytest.fail(_where(bad, what, tile_m, tile_n) + f": got {g[r, c].item()!r}, ref {ref[r, c].item()!r}, "
+        pytest.fail(_where(bad, what, tile_m, tile_n, row0) + f": got {g[r, c].item()!r}, ref {ref[r, c].item()!r}, "
                     f"tol {tol[r, c].item() if torch.is_tensor(tol) else tol!r}")
 
 

@@ -14,7 +14,7 @@ HBM layout per layer (bf16 unless noted):
 Residual stream and its gradient are fp32; every GEMM operand is bf16.
 Qwen2 is this architecture plus q/k/v biases (HF Qwen2ForCausalLM); Qwen3 (HF Qwen3ForCausalLM) adds the per-head q/k RMSNorm,
 fused into the QKV GEMM's RoPE epilogue (training shapes) or applied by the qk_norm_rope row kernel (decode, prefill, other
-widths); the backward saves the pre-norm q|k columns and their rstd. Configs are checked by params.check_llama_family.
+widths); the backward saves the pre-norm q|k columns and their rstd. Configs are checked and resolved by params.resolve_decoder.
 Llama 3.x is this architecture with GQA and frequency-scaled RoPE: params.rope_inv_freq builds the default, `linear` and
 `llama3` frequencies, and every RoPE kernel reads the cos / sin tables `_rope` makes from them.
 Mistral (HF MistralForCausalLM) is Llama with sliding-window causal attention: params.sliding_windows gives each layer's key
@@ -41,8 +41,7 @@ from .. import ops
 from . import moe
 from .dense import DenseBank
 from .lora import LoraBank
-from .params import (OLMO_KINDS, attention_biases, check_llama_family, check_olmo, moe_intermediate_size, moe_layers,
-                     rope_attention_factor, rope_inv_freq, sliding_windows)
+from .params import check_decoder_mode, moe_intermediate_size, resolve_decoder
 
 bf16, f32 = torch.bfloat16, torch.float32
 
@@ -66,6 +65,7 @@ def _with_prefix(sd: Dict[str, torch.Tensor]) -> Dict[str, torch.Tensor]:
 
 class LlamaDecoder(torch.nn.Module):
     LORA_TARGETS = ("q_proj", "v_proj")               # reference rag_e2e_base_model.py:76-77
+    OPTIONAL = ("bqkv", "bo", "qn", "kn")              # layer entries that are None where the architecture has no such tensor
 
     def __init__(self, cfg: Dict, state_dict: Dict[str, torch.Tensor], device="cuda", lora: bool = False,
                  lora_seed: int = 1, full: bool = False, nf4_storage: bool = False):
@@ -76,46 +76,24 @@ class LlamaDecoder(torch.nn.Module):
             raise ValueError("lora and full fine-tuning are mutually exclusive for one model")
         if nf4_storage and full:
             raise ValueError("4-bit base weights cannot be fully fine-tuned")
+        self.cfg = cfg
+        self.arch = a = resolve_decoder(cfg)
+        check_decoder_mode(a.kind, full=full, nf4_storage=nf4_storage)
         # use_bnb with 4-bit STORAGE (engine/nf4store.py): `state_dict` then holds the ORIGINAL checkpoint values; the layers'
         # Linear weights are kept as NF4 codes and expanded to bf16 per use, everything else takes transformers' fp16 cast
         self.nf4 = None
         if nf4_storage:
             from .nf4store import Nf4Store
             self.nf4 = Nf4Store(device)
-        mt = cfg.get("model_type")
-        check_olmo(cfg) if mt in OLMO_KINDS else check_llama_family(cfg)
-        self.cfg = cfg
-        self.kind = mt if mt in ("qwen2", "qwen3", "mistral", "qwen3_moe") + OLMO_KINDS else "llama"
-        self.qkv_bias, self.o_bias = attention_biases(self.kind, cfg)
-        self.qk_norm = self.kind in ("qwen3", "qwen3_moe")
-        self.fullnorm = self.kind in OLMO_KINDS                 # q/k RMSNorm over the whole q / k width (qn [Nq], kn [Nkv])
-        self.post_norm = self.kind in ("olmo2", "olmo3")        # norms after each sublayer (g2, g3), no pre-norms
-        if self.fullnorm and nf4_storage:
-            raise NotImplementedError(f"{self.kind}: 4-bit storage is not built")
-        self.H = H = cfg["hidden_size"]
-        # qwen3_moe without dense layers may leave it out; olmoe's intermediate_size is its experts' width (no dense MLP)
-        self.F = F = (cfg.get("intermediate_size") or 0) if self.kind != "olmoe" else 0
-        # Qwen3-MoE: the layers that run the routed MLP (engine/moe.py) instead of the dense SwiGLU one
-        self.sparse = moe_layers(cfg) if self.kind in ("qwen3_moe", "olmoe") else [False] * cfg["num_hidden_layers"]
-        if any(self.sparse) and (full or nf4_storage):
-            raise NotImplementedError(f"{self.kind}: " + ("full fine-tuning is not built (grouped expert weight gradients are not "
-                                                       "built)" if full else "4-bit storage of the expert weights is not built"))
-        self.nl = cfg["num_hidden_layers"]
-        self.nh = cfg["num_attention_heads"]
-        self.nkv = cfg.get("num_key_value_heads", self.nh)
-        self.hd = cfg.get("head_dim") or H // self.nh
-        self.V = cfg["vocab_size"]
-        self.eps = float(cfg.get("rms_norm_eps", 1e-5))
+        self.H, self.F, self.nl, self.nh, self.nkv, self.hd, self.V, self.eps = a.H, a.F, a.nl, a.nh, a.nkv, a.hd, a.V, a.eps
+        self.qkv_bias, self.o_bias, self.sparse = a.qkv_bias, a.o_bias, a.sparse
+        self.qk_norm, self.post_norm = a.traits.qk_norm, a.traits.post_norm
+        self.inv_freq, self.rope_scale, self.windows = a.inv_freq, a.rope_scale, a.windows
         self.dev = torch.device(device)
-        if self.hd not in (32, 64, 128):
-            raise NotImplementedError(f"head_dim {self.hd} not supported by the attention kernels")
-        self.inv_freq = rope_inv_freq(cfg, self.hd)           # default, linear, llama3 or yarn frequencies (fp32, CPU)
-        self.rope_scale = rope_attention_factor(cfg, self.hd)  # yarn's attention factor on cos / sin, else 1
-        self.windows = sliding_windows(cfg)                   # key window of each layer, 0 = full causal attention
         self.Nq, self.Nkv = self.nh * self.hd, self.nkv * self.hd
         self.Nqkv = self.Nq + 2 * self.Nkv
         self.r = 8
-        self.Ra = 2 * self.r if lora else 0
+        self.Ra = 0
         # headless checkpoints (AutoModel: embed_tokens.*, layers.*, norm.*) are read under the model.-prefixed names
         self.headless = not any(k.startswith("model.") for k in state_dict)
         sd = _with_prefix(state_dict) if self.headless else state_dict
@@ -128,27 +106,22 @@ class LlamaDecoder(torch.nn.Module):
         self.layers: List[Dict[str, torch.Tensor]] = []
         # frozen-base modes keep the fused gate|up weight in the interleaved layout of the SwiGLU-epilogue GEMM (F % 128 == 0);
         # a fully fine-tuned model keeps HF's [gate; up] order inside its parameter bank (un-fused activation kernel)
-        self.fuse_rope = self.hd == 128 and not self.fullnorm
-        self.gu_il = 128 if (not full and F % 128 == 0) else 0
+        self.fuse_rope = self.hd == 128 and self.qk_norm != "full"
+        self.gu_il = 128 if (not full and self.F % 128 == 0) else 0
         if full:
             self._init_full(sd)
         else:
-            self._init_frozen(sd, g, lora)
+            self._init_frozen(sd, g)
         self._rope_cache: Dict[int, tuple] = {}
         # Llama has no hidden / attention dropout (attention_dropout = 0); only peft's LoRA input dropout (0.05) applies
-        self.p_lora = 0.05 if lora else 0.0
+        self.p_lora = 0.0
         self.drop_seed = 0x11A3AB200 + lora_seed
         self.drop_offset = torch.zeros(1, dtype=torch.int64, device=self.dev)
         self._call = 0
         self.lora: Optional[LoraBank] = None
+        self._pack_tab = None
         if lora:
-            outs = {"q_proj": self.Nq, "v_proj": self.Nkv}
-            specs = [(f"model.layers.{l}.self_attn.{n}", H, outs[n]) for l in range(self.nl) for n in self.LORA_TARGETS]
-            self.lora = LoraBank(specs, r=self.r, alpha=16, dropout=0.05, device=self.dev, seed=lora_seed)
-            self.lora_flat = torch.nn.Parameter(self.lora.flat, requires_grad=True)
-            self.lora_flat.grad = self.lora.grad
-            self.lora.param = self.lora_flat
-            self.repack_lora()
+            self.enable_lora(lora_seed)
         self.eval()                                           # like from_pretrained(): dropout only after .train()
 
     # ---- what is trainable ---------------------------------------------------------------------------------------
@@ -172,27 +145,35 @@ class LlamaDecoder(torch.nn.Module):
         if self.full is not None:
             self.full.zero_grad()
 
+    def _layer_tensors(self):
+        """(engine slot, bank kind, HF names under `model.layers.{l}.`) of every tensor of a layer, in the DenseBank's order.
+        "acc" entries (norm gains, biases, q / k norm weights) are fp32 vectors whose gradients are accumulated into (+=)"""
+        t = []
+        if self.qkv_bias:
+            t.append(("bqkv", "acc", [f"self_attn.{n}_proj.bias" for n in "qkv"]))
+        if self.o_bias:
+            t.append(("bo", "acc", ["self_attn.o_proj.bias"]))
+        if self.qk_norm:
+            t += [("qn", "acc", ["self_attn.q_norm.weight"]), ("kn", "acc", ["self_attn.k_norm.weight"])]
+        t += [("Wqkv_aug", "gemm", [f"self_attn.{n}_proj.weight" for n in "qkv"]), ("Wo", "gemm", ["self_attn.o_proj.weight"]),
+              ("Wgu", "gemm", ["mlp.gate_proj.weight", "mlp.up_proj.weight"]), ("Wd", "gemm", ["mlp.down_proj.weight"])]
+        if self.post_norm:                                       # norms after each sublayer (g2, g3), no pre-norm
+            t += [("g2", "acc", ["post_attention_layernorm.weight"]), ("g3", "acc", ["post_feedforward_layernorm.weight"])]
+        else:
+            t += [("g1", "acc", ["input_layernorm.weight"]), ("g2", "acc", ["post_attention_layernorm.weight"])]
+        return t
+
+    @staticmethod
+    def _bank_key(l: int, slot: str) -> str:
+        return f"L{l}.{slot.removesuffix('_aug')}"
+
     def _param_map(self, has_head: bool):
         m = [("embed", "acc", ["model.embed_tokens.weight"]), ("norm_g", "acc", ["model.norm.weight"])]
         if has_head:
             m.append(("lm_head", "gemm", ["lm_head.weight"]))
         for l in range(self.nl):
-            p = f"model.layers.{l}."
-            if self.qkv_bias:                                    # biases: "acc" entries (column sums accumulated by atomics)
-                m.append((f"L{l}.bqkv", "acc", [p + f"self_attn.{n}_proj.bias" for n in "qkv"]))
-            if self.o_bias:
-                m.append((f"L{l}.bo", "acc", [p + "self_attn.o_proj.bias"]))
-            if self.qk_norm or self.fullnorm:                    # q / k norm weights: "acc" entries (accumulated into, +=)
-                m += [(f"L{l}.qn", "acc", [p + "self_attn.q_norm.weight"]), (f"L{l}.kn", "acc", [p + "self_attn.k_norm.weight"])]
-            m += [(f"L{l}.Wqkv", "gemm", [p + f"self_attn.{n}_proj.weight" for n in "qkv"]),
-                  (f"L{l}.Wo", "gemm", [p + "self_attn.o_proj.weight"]),
-                  (f"L{l}.Wgu", "gemm", [p + "mlp.gate_proj.weight", p + "mlp.up_proj.weight"]),
-                  (f"L{l}.Wd", "gemm", [p + "mlp.down_proj.weight"])]
-            if self.post_norm:
-                m += [(f"L{l}.g2", "acc", [p + "post_attention_layernorm.weight"]),
-                      (f"L{l}.g3", "acc", [p + "post_feedforward_layernorm.weight"])]
-            else:
-                m += [(f"L{l}.g1", "acc", [p + "input_layernorm.weight"]), (f"L{l}.g2", "acc", [p + "post_attention_layernorm.weight"])]
+            m += [(self._bank_key(l, slot), kind, [f"model.layers.{l}." + n for n in names])
+                  for slot, kind, names in self._layer_tensors()]
         return m
 
     def _init_full(self, sd) -> None:
@@ -223,15 +204,10 @@ class LlamaDecoder(torch.nn.Module):
         self.tied = not has_head
         self.lm_head = bank.w16("lm_head") if has_head else self.embed
         for l in range(self.nl):
-            k = lambda n: f"L{l}.{n}"
-            self.layers.append({"Wqkv_aug": bank.w16(k("Wqkv")), "Wo": bank.w16(k("Wo")), "Wgu": bank.w16(k("Wgu")),
-                                "Wd": bank.w16(k("Wd")), "g2": bank.w32(k("g2")),
-                                "g1": bank.w32(k("g1")) if not self.post_norm else None,
-                                "g3": bank.w32(k("g3")) if self.post_norm else None,
-                                "bqkv": bank.w32(k("bqkv")) if self.qkv_bias else None,
-                                "bo": bank.w32(k("bo")) if self.o_bias else None,
-                                "qn": bank.w32(k("qn")) if self.qk_norm or self.fullnorm else None,
-                                "kn": bank.w32(k("kn")) if self.qk_norm or self.fullnorm else None})
+            W = dict.fromkeys(self.OPTIONAL)
+            for slot, kind, _ in self._layer_tensors():
+                W[slot] = (bank.w16 if kind == "gemm" else bank.w32)(self._bank_key(l, slot))
+            self.layers.append(W)
 
     def hf_state_dict(self) -> Dict[str, torch.Tensor]:
         """fp32 CPU tensors under HF LlamaForCausalLM (or Olmo2 / Olmo3 / Olmoe) names (save_pretrained of a fully fine-tuned decoder), or under the
@@ -257,7 +233,8 @@ class LlamaDecoder(torch.nn.Module):
         self.full.sync_shadow()
 
     def enable_lora(self, lora_seed: int = 1) -> None:
-        """frozen (inference-built) decoder -> adapter-carrying one, see BertEncoder.enable_lora"""
+        """frozen decoder -> adapter-carrying one (also how the constructor attaches them), see BertEncoder.enable_lora: the
+        q|k|v weight gains its Ra LoRA columns, and the layers their rank-stacked A / B operands"""
         if self.lora is not None:
             return
         if self.full is not None:
@@ -270,14 +247,12 @@ class LlamaDecoder(torch.nn.Module):
                 self.nf4.tails[(li, "Wqkv_aug")] = torch.zeros(rows, self.Ra, dtype=bf16, device=self.dev)
                 if self.nf4.slots["Wqkv_aug"].shape[1] < cols + 64:
                     self.nf4.slots["Wqkv_aug"] = torch.empty(rows, cols + 64, dtype=bf16, device=self.dev)
-                W["A_stack"] = torch.zeros(64, H, dtype=bf16, device=self.dev)
-                W["Bblk"] = torch.zeros(64, self.Nqkv, dtype=bf16, device=self.dev)
-                continue
-            old, oldT = W["Wqkv_aug"], W["WqkvT_aug"]
-            W["Wqkv_aug"] = _aug_buf(self.Nqkv, H, self.Ra, self.dev, zero=True)
-            W["Wqkv_aug"][:, :H] = old[:, :H]
-            W["WqkvT_aug"] = _aug_buf(H, self.Nqkv, self.Ra, self.dev, zero=True)
-            W["WqkvT_aug"][:, :self.Nqkv] = oldT[:, :self.Nqkv]
+            else:
+                old, oldT = W["Wqkv_aug"], W["WqkvT_aug"]
+                W["Wqkv_aug"] = _aug_buf(self.Nqkv, H, self.Ra, self.dev, zero=True)
+                W["Wqkv_aug"][:, :H] = old[:, :H]
+                W["WqkvT_aug"] = _aug_buf(H, self.Nqkv, self.Ra, self.dev, zero=True)
+                W["WqkvT_aug"][:, :self.Nqkv] = oldT[:, :self.Nqkv]
             W["A_stack"] = torch.zeros(64, H, dtype=bf16, device=self.dev)
             W["Bblk"] = torch.zeros(64, self.Nqkv, dtype=bf16, device=self.dev)
         outs = {"q_proj": self.Nq, "v_proj": self.Nkv}
@@ -287,7 +262,6 @@ class LlamaDecoder(torch.nn.Module):
         self.lora_flat.grad = self.lora.grad
         self.lora.param = self.lora_flat
         self.p_lora = 0.05
-        self._pack_tab = None
         self.repack_lora()
 
     def _dgrad(self, dy: torch.Tensor, W: Dict[str, torch.Tensor], name: str) -> torch.Tensor:
@@ -295,51 +269,35 @@ class LlamaDecoder(torch.nn.Module):
             return ops.gemm(dy, W[name], layout=1)
         return ops.gemm(dy, W[name + "T"])
 
-    def _init_frozen(self, sd, g, lora: bool) -> None:
-        H = self.H
+    def _init_frozen(self, sd, g) -> None:
         self.embed = g("model.embed_tokens.weight", bf16)
         self.norm_g = g("model.norm.weight", f32)
         lm = g("lm_head.weight", bf16) if "lm_head.weight" in sd else self.embed      # tied / headless (AutoModel) checkpoints
         if self.Vp != self.V:
-            lm = torch.cat([lm, torch.zeros(self.Vp - self.V, H, dtype=bf16, device=self.dev)], 0)
+            lm = torch.cat([lm, torch.zeros(self.Vp - self.V, self.H, dtype=bf16, device=self.dev)], 0)
         self.lm_head = lm
         self.lm_headT = self.lm_head.t().contiguous()
-        H_, Ra = H, self.Ra
         for l in range(self.nl):
             p = f"model.layers.{l}."
             if self.nf4 is not None:
-                self.layers.append(self._init_layer_nf4(sd, l, g, lora))
+                self.layers.append(self._init_layer_nf4(sd, l, g))
                 continue
             W = {}
-            wqkv = torch.cat([g(p + "self_attn.q_proj.weight", bf16), g(p + "self_attn.k_proj.weight", bf16),
-                              g(p + "self_attn.v_proj.weight", bf16)], 0)
-            W["Wqkv_aug"] = _aug_buf(self.Nqkv, H_, Ra, self.dev, zero=True)
-            W["Wqkv_aug"][:, :H_] = wqkv
-            W["WqkvT_aug"] = _aug_buf(H_, self.Nqkv, Ra, self.dev, zero=True)
-            W["WqkvT_aug"][:, :self.Nqkv] = wqkv.t()
-            del wqkv
-            if lora:
-                W["A_stack"] = torch.zeros(64, H_, dtype=bf16, device=self.dev)
-                W["Bblk"] = torch.zeros(64, self.Nqkv, dtype=bf16, device=self.dev)
+            W["Wqkv_aug"] = torch.cat([g(p + "self_attn.q_proj.weight", bf16), g(p + "self_attn.k_proj.weight", bf16),
+                                       g(p + "self_attn.v_proj.weight", bf16)], 0)
+            W["WqkvT_aug"] = W["Wqkv_aug"].t().contiguous()
             W["Wo"] = g(p + "self_attn.o_proj.weight", bf16)
             W["WoT"] = W["Wo"].t().contiguous()
             if self.sparse[l]:
                 W["moe"] = self._moe_weights(sd, p)
             else:
-                if self.gu_il:   # gate / up rows interleaved in 128-feature blocks: SiLU(gate)*up is fused into this GEMM's epilogue
-                    W["Wgu"] = ops.interleave_gate_up(g(p + "mlp.gate_proj.weight", bf16), g(p + "mlp.up_proj.weight", bf16), self.gu_il)
-                else:
-                    W["Wgu"] = torch.cat([g(p + "mlp.gate_proj.weight", bf16), g(p + "mlp.up_proj.weight", bf16)], 0)
+                # gate / up rows interleaved in 128-feature blocks: SiLU(gate)*up is fused into this GEMM's epilogue
+                gate, up = g(p + "mlp.gate_proj.weight", bf16), g(p + "mlp.up_proj.weight", bf16)
+                W["Wgu"] = ops.interleave_gate_up(gate, up, self.gu_il) if self.gu_il else torch.cat([gate, up], 0)
                 W["WguT"] = W["Wgu"].t().contiguous()
                 W["Wd"] = g(p + "mlp.down_proj.weight", bf16)
                 W["WdT"] = W["Wd"].t().contiguous()
-            if self.post_norm:
-                W["g2"] = g(p + "post_attention_layernorm.weight", f32)
-                W["g3"] = g(p + "post_feedforward_layernorm.weight", f32)
-            else:
-                W["g1"] = g(p + "input_layernorm.weight", f32)
-                W["g2"] = g(p + "post_attention_layernorm.weight", f32)
-            self._frozen_biases(W, p, g)
+            self._frozen_vectors(W, l, g)
             self.layers.append(W)
 
     def _moe_weights(self, sd, p: str) -> moe.MoeWeights:
@@ -359,7 +317,7 @@ class LlamaDecoder(torch.nn.Module):
         return moe.pack_experts(sd[p + "mlp.gate.weight"], gate_proj, up_proj, down, int(cfg["num_experts_per_tok"]),
                                 bool(cfg.get("norm_topk_prob", False)), self.dev)
 
-    def _init_layer_nf4(self, sd, l: int, g, lora: bool):
+    def _init_layer_nf4(self, sd, l: int, g):
         """one layer in 4-bit storage: q|k|v, o, gate|up (interleaved like the resident mode), down as NF4 codes; blocks of 64
         run along the input features, so fusing / interleaving ROWS leaves every block (and its absmax) what bitsandbytes
         computes for the separate nn.Linear weights"""
@@ -367,27 +325,21 @@ class LlamaDecoder(torch.nn.Module):
         p = f"model.layers.{l}."
         raw = lambda k: sd[k].to(device=self.dev, dtype=f32)
         W = QuantLayer(self.nf4, l)
-        self.nf4.put(l, "Wqkv_aug", torch.cat([raw(p + f"self_attn.{n}_proj.weight") for n in "qkv"], 0), tail_cols=self.Ra)
+        self.nf4.put(l, "Wqkv_aug", torch.cat([raw(p + f"self_attn.{n}_proj.weight") for n in "qkv"], 0))
         self.nf4.put(l, "Wo", raw(p + "self_attn.o_proj.weight"))
         gate, up = raw(p + "mlp.gate_proj.weight"), raw(p + "mlp.up_proj.weight")
         self.nf4.put(l, "Wgu", ops.interleave_gate_up(gate, up, self.gu_il) if self.gu_il else torch.cat([gate, up], 0))
         self.nf4.put(l, "Wd", raw(p + "mlp.down_proj.weight"))
-        if lora:
-            W["A_stack"] = torch.zeros(64, self.H, dtype=bf16, device=self.dev)
-            W["Bblk"] = torch.zeros(64, self.Nqkv, dtype=bf16, device=self.dev)
-        W["g1"] = g(p + "input_layernorm.weight", f32)
-        W["g2"] = g(p + "post_attention_layernorm.weight", f32)
-        self._frozen_biases(W, p, g)
+        self._frozen_vectors(W, l, g)
         return W
 
-    def _frozen_biases(self, W, p: str, g) -> None:
-        """frozen / LoRA modes: the attention biases (and Qwen3's q / k norm weights) are forward-only fp32 vectors (under use_bnb they take the fp16 cast of every
-        non-Linear-weight tensor, never the NF4 round trip)"""
-        W["bqkv"] = torch.cat([g(p + f"self_attn.{n}_proj.bias", f32) for n in "qkv"]) if self.qkv_bias else None
-        W["bo"] = g(p + "self_attn.o_proj.bias", f32) if self.o_bias else None
-        # Qwen3's q / k norm weights: forward-only fp32 vectors here too (use_bnb: the fp16 cast, as every norm weight)
-        W["qn"] = g(p + "self_attn.q_norm.weight", f32) if self.qk_norm or self.fullnorm else None
-        W["kn"] = g(p + "self_attn.k_norm.weight", f32) if self.qk_norm or self.fullnorm else None
+    def _frozen_vectors(self, W, l: int, g) -> None:
+        """frozen / LoRA modes: norm gains, attention biases and q / k norm weights are forward-only fp32 vectors (under
+        use_bnb they take the fp16 cast of every non-Linear-weight tensor, never the NF4 round trip)"""
+        W.update(dict.fromkeys(self.OPTIONAL))
+        for slot, kind, names in self._layer_tensors():
+            if kind == "acc":
+                W[slot] = torch.cat([g(f"model.layers.{l}." + n, f32) for n in names])
 
     def _drop(self, training: bool, call: int, layer: int):
         if not training or self.p_lora <= 0.0:
@@ -416,7 +368,7 @@ class LlamaDecoder(torch.nn.Module):
     def repack_lora(self) -> None:
         if self.lora is None:
             return
-        if getattr(self, "_pack_tab", None) is None:
+        if self._pack_tab is None:
             self._pack_tab = ops.build_pack_table(list(self._pack_entries()), self.dev)
         ops.pack_table_(self._pack_tab)
 
@@ -490,84 +442,122 @@ class LlamaDecoder(torch.nn.Module):
         """pos / rope_tables / kv_sink serve `generate`'s prefill: explicit position ids (int64 [B*L]) into cos / sin tables
         [T, hd/2], and a callback (layer, qkv) that copies the rotated K / V columns into the KV cache"""
         B, L = ids.shape
-        M, H, F, Ra = B * L, self.H, self.F, self.Ra
+        M, F = B * L, self.F
         cos_t, sin_t = self._rope(L) if rope_tables is None else rope_tables
         ctx = _Ctx()
         ctx.B, ctx.L, ctx.mask, ctx.layers = B, L, mask.contiguous(), []
         ctx.ids = ids.contiguous()
         self._call += 1
         ctx.call, ctx.training = self._call, self.training
-        x = ops.embed_gather(ids, self.embed)                                    # fp32 residual stream [M,H]
-        if self.post_norm:                                                       # the first QKV GEMM reads bf16(embeddings)
-            h_next = _aug_buf(M, H, Ra, self.dev)
-            ops.cast_f32_bf16(x, h_next[:, :H])
+        x, h_next = ops.embed_gather(ids, self.embed), None                     # fp32 residual stream [M,H]
         for li, W in enumerate(self.layers):
             a = _Ctx()
-            if self.post_norm:                   # no pre-norm: bf16(x), written by the layer below's postnorm (or the cast)
-                a.h1_aug = h_next
-            else:
-                a.x_in = x
-                a.h1_aug = _aug_buf(M, H, Ra, self.dev)
-                _, a.rstd1 = ops.rmsnorm_fwd(x, W["g1"], self.eps, h=a.h1_aug[:, :H])
-            if Ra:
-                ops.skinny_gemm(a.h1_aug[:, :H], W["A_stack"], a.h1_aug[:, H:], K=H, R=Ra,   # u = dropout(h1) A^T [M,2r]
-                                dropx=self._drop(ctx.training, ctx.call, li))
+            a.h1_aug = self._layer_in(x, W, h_next, a, self._drop(ctx.training, ctx.call, li))
             rope_cols = (self.nh + self.nkv) * self.hd
             a.pre = a.qk_rstd = None
-            if (self.qk_norm or self.fullnorm) and save and self.trainable:      # what the q/k norm backward reads
+            if self.qk_norm and save and self.trainable:                          # what the q/k norm backward reads
                 a.pre = torch.empty(M, rope_cols, dtype=bf16, device=self.dev)
-                a.qk_rstd = torch.empty(M, 2 if self.fullnorm else self.nh + self.nkv, dtype=f32, device=self.dev)
-            if self.fullnorm:
-                a.qkv = ops.gemm(a.h1_aug, W["Wqkv_aug"])                         # [M, Nq+2Nkv], then q/k norm + RoPE
-                ops.qk_fullnorm_rope_(a.qkv, self.nh, self.nkv, self.hd, W["qn"], W["kn"], self.eps, cos_t, sin_t,
-                                      L=L if pos is None else 0, pos=pos, pre=a.pre, rstd=a.qk_rstd, round_first=self.kind == "olmoe")
-            elif pos is None and self.fuse_rope and rope_cols % 256 == 0:
+                a.qk_rstd = torch.empty(M, 2 if self.qk_norm == "full" else self.nh + self.nkv, dtype=f32, device=self.dev)
+            if pos is None and self.fuse_rope and rope_cols % 256 == 0:
                 norm = dict(q_norm=W["qn"], k_norm=W["kn"], nq_heads=self.nh, eps=self.eps, pre_out=a.pre,
                             rstd_out=a.qk_rstd) if self.qk_norm else {}
                 a.qkv = ops.gemm_rope(a.h1_aug, W["Wqkv_aug"], cos_t, sin_t, L, rope_cols,   # QKV (+LoRA, + bias) with (q/k norm
                                       bias=W["bqkv"], **norm)                                # and) RoPE in the epilogue
             else:
                 a.qkv = ops.gemm(a.h1_aug, W["Wqkv_aug"], bias=W["bqkv"])        # [M, Nq+2Nkv]
-                if self.qk_norm:
-                    ops.qk_norm_rope_(a.qkv, self.nh + self.nkv, self.nh, W["qn"], W["kn"], self.eps, cos_t, sin_t,
-                                      L=L if pos is None else 0, pos=pos, pre=a.pre, rstd=a.qk_rstd)
-                elif pos is None:
-                    ops.rope_(a.qkv, 0, self.nh + self.nkv, self.hd, cos_t, sin_t, L)    # q heads then k heads are adjacent
-                else:
-                    ops.rope_pos_(a.qkv, 0, self.nh + self.nkv, self.hd, cos_t, sin_t, pos)
+                self._qk_rope(a.qkv, W, cos_t, sin_t, L, pos, a.pre, a.qk_rstd)
             if kv_sink is not None:
                 kv_sink(li, a.qkv)
             a.att, a.lse = ops.attention_auto_fwd(a.qkv[:, :self.Nq], a.qkv[:, self.Nq:self.Nq + self.Nkv],
                                                   a.qkv[:, self.Nq + self.Nkv:], ctx.mask, B, L, self.nh, self.nkv, self.hd, causal=True,
                                                   window=self.windows[li])
-            if self.post_norm:                   # x_mid = x + post_attention_layernorm(o_proj(att)); h2 = bf16(x_mid)
-                a.yo = ops.gemm(a.att, W["Wo"])
-                a.h2 = torch.empty(M, H, dtype=bf16, device=self.dev)
-                x_mid, a.rstd2 = ops.postnorm_fwd(a.yo, W["g2"], x, self.eps, out16=a.h2)
-            else:
-                x_mid = a.x_mid = ops.gemm(a.att, W["Wo"], out_dtype=f32, resid=x, bias=W["bo"])
-                a.h2, a.rstd2 = ops.rmsnorm_fwd(x_mid, W["g2"], self.eps)
+            x_mid, a.h2 = self._attn_out(a.att, W, x, ops.gemm, a)
             if "moe" in W:
                 x, a.moe = moe.forward(a.h2, W["moe"], resid=x_mid)
-                if save:
-                    ctx.layers.append(a)
-                continue
-            if self.gu_il:
-                a.gu, a.act = ops.gemm_swiglu(a.h2, W["Wgu"])                     # [M,2F] (interleaved) + silu(gate)*up [M,F]: one launch
             else:
-                a.gu = ops.gemm(a.h2, W["Wgu"])                                   # [M,2F]
-                a.act = ops.swiglu_fwd(a.gu, F)
-            if self.post_norm:                   # x = x_mid + post_feedforward_layernorm(down(act)), bf16(x) into the next QKV operand
-                a.yd = ops.gemm(a.act, W["Wd"])
-                h_next = _aug_buf(M, H, Ra, self.dev) if li + 1 < self.nl else None
-                x, a.rstd3 = ops.postnorm_fwd(a.yd, W["g3"], x_mid, self.eps, out16=h_next[:, :H] if h_next is not None else None)
-            else:
-                x = ops.gemm(a.act, W["Wd"], out_dtype=f32, resid=x_mid)
+                if self.gu_il:
+                    a.gu, a.act = ops.gemm_swiglu(a.h2, W["Wgu"])                 # [M,2F] (interleaved) + silu(gate)*up [M,F]: one launch
+                else:
+                    a.gu = ops.gemm(a.h2, W["Wgu"])                               # [M,2F]
+                    a.act = ops.swiglu_fwd(a.gu, F)
+                x, h_next = self._mlp_out(a.act, W, x_mid, li + 1 < self.nl, ops.gemm, a)
             if save:
                 ctx.layers.append(a)
         ctx.x_final = x
         ctx.hf, ctx.rstdf = ops.rmsnorm_fwd(x, self.norm_g, self.eps)
         return ctx
+
+    # ---- one implementation of each layer choice, shared by the forward, the prefill, the decode step and the backward --
+    def _layer_in(self, x: torch.Tensor, W, h_prev: Optional[torch.Tensor], a: _Ctx, drop) -> torch.Tensor:
+        """the QKV operand [M, H+Ra]: RMSNorm(x) (pre-norm), or bf16(x) as the layer below's post-norm wrote it (h_prev) or
+        cast from the embeddings; then the LoRA down-projection u = dropout(h1) A^T [M, 2r] into its last Ra columns"""
+        H, h1 = self.H, h_prev
+        if h1 is None:
+            h1 = _aug_buf(x.shape[0], H, self.Ra, self.dev)
+            if self.post_norm:
+                ops.cast_f32_bf16(x, h1[:, :H])
+            else:
+                a.x_in = x
+                _, a.rstd1 = ops.rmsnorm_fwd(x, W["g1"], self.eps, h=h1[:, :H])
+        if self.Ra:
+            ops.skinny_gemm(h1[:, :H], W["A_stack"], h1[:, H:], K=H, R=self.Ra, dropx=drop)
+        return h1
+
+    def _qk_rope(self, qkv: torch.Tensor, W, cos_t, sin_t, L: int, pos: Optional[torch.Tensor], pre=None, rstd=None) -> None:
+        """in place on qkv's q|k heads: the q/k norm (if any), then RoPE at positions row % L, or at `pos` (int64 [M]) when
+        given; pre / rstd receive what the q/k norm backward reads"""
+        nh, nkv, hd = self.nh, self.nkv, self.hd
+        kw = dict(L=L if pos is None else 0, pos=pos, pre=pre, rstd=rstd)
+        if self.qk_norm == "full":
+            ops.qk_fullnorm_rope_(qkv, nh, nkv, hd, W["qn"], W["kn"], self.eps, cos_t, sin_t, round_first=self.arch.traits.round_first, **kw)
+        elif self.qk_norm == "head":
+            ops.qk_norm_rope_(qkv, nh + nkv, nh, W["qn"], W["kn"], self.eps, cos_t, sin_t, **kw)
+        elif pos is None:
+            ops.rope_(qkv, 0, nh + nkv, hd, cos_t, sin_t, L)                      # q heads then k heads are adjacent
+        else:
+            ops.rope_pos_(qkv, 0, nh + nkv, hd, cos_t, sin_t, pos)
+
+    def _qk_rope_bwd(self, l: int, dqkv: torch.Tensor, W, a: _Ctx, cos_t, sin_t, L: int) -> None:
+        """backward of `_qk_rope` / the fused epilogue in place on d(qkv): un-rotate, then the q/k norm (and its weights) backward"""
+        dw = dict(dw_q=self.full.g(f"L{l}.qn"), dw_k=self.full.g(f"L{l}.kn")) if self.qk_norm and self.full is not None else {}
+        if self.qk_norm == "full":
+            ops.qk_fullnorm_rope_bwd_(dqkv, self.nh, self.nkv, self.hd, W["qn"], W["kn"], cos_t, sin_t, L, a.pre, a.qk_rstd, **dw)
+        elif self.qk_norm == "head":
+            ops.qk_norm_rope_bwd_(dqkv, self.nh + self.nkv, self.nh, W["qn"], W["kn"], cos_t, sin_t, L, a.pre, a.qk_rstd, **dw)
+        else:
+            ops.rope_(dqkv, 0, self.nh + self.nkv, self.hd, cos_t, sin_t, L, backward=True)
+
+    def _attn_out(self, att: torch.Tensor, W, x: torch.Tensor, gemm, a: _Ctx):
+        """o_proj and the residual -> (x_mid fp32, h2 bf16: the MLP operand). Pre-norm: x_mid = x + o_proj(att),
+        h2 = RMSNorm(x_mid). Post-norm: x_mid = x + post_attention_layernorm(o_proj(att)), h2 = bf16(x_mid)"""
+        if self.post_norm:
+            a.yo = gemm(att, W["Wo"])
+            a.h2 = torch.empty(x.shape[0], self.H, dtype=bf16, device=self.dev)
+            x_mid, a.rstd2 = ops.postnorm_fwd(a.yo, W["g2"], x, self.eps, out16=a.h2)
+        else:
+            x_mid = a.x_mid = gemm(att, W["Wo"], out_dtype=f32, resid=x, bias=W["bo"])
+            a.h2, a.rstd2 = ops.rmsnorm_fwd(x_mid, W["g2"], self.eps)
+        return x_mid, a.h2
+
+    def _mlp_out(self, act: torch.Tensor, W, x_mid: torch.Tensor, more: bool, gemm, a: _Ctx):
+        """down_proj and the residual -> (next x fp32, next QKV operand or None). Pre-norm: x = x_mid + down(act). Post-norm:
+        x = x_mid + post_feedforward_layernorm(down(act)), bf16(x) written straight into the next (`more`) layer's QKV operand"""
+        if not self.post_norm:
+            return gemm(act, W["Wd"], out_dtype=f32, resid=x_mid), None
+        a.yd = gemm(act, W["Wd"])
+        h_next = _aug_buf(x_mid.shape[0], self.H, self.Ra, self.dev) if more else None
+        x, a.rstd3 = ops.postnorm_fwd(a.yd, W["g3"], x_mid, self.eps, out16=h_next[:, :self.H] if more else None)
+        return x, h_next
+
+    def _layer_in_bwd(self, l: int, a: _Ctx, W, dh1: torch.Tensor, dmid32: torch.Tensor):
+        """gradient through `_layer_in` -> (dx32, dx16, dpend) at the layer below's output. Post-norm passes d(bf16 x) up as
+        dpend, to join the residual gradient there; pre-norm runs the RMSNorm backward (and its gain's gradient)"""
+        if self.post_norm:
+            return dmid32, None, dh1
+        if self.full is not None:
+            ops.col_reduce_(dy_bf16=dh1, z=a.x_in, rstd=a.rstd1, out_prod=self.full.g(f"L{l}.g1"))
+        dx32, dx16 = ops.rmsnorm_bwd(a.x_in, W["g1"], a.rstd1, dh1, dres_in=dmid32)
+        return dx32, dx16, None
 
     # ------------------------------------------------------------------------------------------------------------
     # greedy decoding with a KV cache (evaluation: reference dalm/eval/eval_rag.py:126-140 calls HF `model.generate`)
@@ -575,46 +565,20 @@ class LlamaDecoder(torch.nn.Module):
     def _decode_step(self, ids: torch.Tensor, pos: torch.Tensor, caches, kmask: torch.Tensor, cur, tables) -> torch.Tensor:
         """one token per sequence: ids / pos int64 [B] (device) -> logits bf16 [B, Vp]; appends K / V at cache column `cur` (int, or the int32 [B] device tensor of per-row columns: CUDA-graph mode)"""
         B = ids.shape[0]
-        H, F, Ra = self.H, self.F, self.Ra
         cos_t, sin_t = tables
-        x = ops.embed_gather(ids, self.embed)                                    # fp32 residual stream [B,H]
-        if self.post_norm:
-            h_next = _aug_buf(B, H, Ra, self.dev)
-            ops.cast_f32_bf16(x, h_next[:, :H])
+        x, h_next = ops.embed_gather(ids, self.embed), None                     # fp32 residual stream [B,H]
         for li, W in enumerate(self.layers):
-            if self.post_norm:
-                h1_aug = h_next
-            else:
-                h1_aug = _aug_buf(B, H, Ra, self.dev)
-                ops.rmsnorm_fwd(x, W["g1"], self.eps, h=h1_aug[:, :H])
-            if Ra:
-                ops.skinny_gemm(h1_aug[:, :H], W["A_stack"], h1_aug[:, H:], K=H, R=Ra)
-            qkv = ops.gemm_rows(h1_aug, W["Wqkv_aug"], bias=W["bqkv"])                # [B, Nq+2Nkv]
-            if self.fullnorm:
-                ops.qk_fullnorm_rope_(qkv, self.nh, self.nkv, self.hd, W["qn"], W["kn"], self.eps, cos_t, sin_t, pos=pos,
-                                      round_first=self.kind == "olmoe")
-            elif self.qk_norm:
-                ops.qk_norm_rope_(qkv, self.nh + self.nkv, self.nh, W["qn"], W["kn"], self.eps, cos_t, sin_t, pos=pos)
-            else:
-                ops.rope_pos_(qkv, 0, self.nh + self.nkv, self.hd, cos_t, sin_t, pos)
+            a = _Ctx()
+            qkv = ops.gemm_rows(self._layer_in(x, W, h_next, a, None), W["Wqkv_aug"], bias=W["bqkv"])   # [B, Nq+2Nkv]
+            self._qk_rope(qkv, W, cos_t, sin_t, 0, pos)
             att = ops.attention_decode(qkv, 0, self.Nq, self.Nq + self.Nkv, caches[li][0], caches[li][1], kmask, cur,
                                        self.nh, self.nkv, self.hd, window=self.windows[li])
-            if self.post_norm:
-                h2 = torch.empty(B, H, dtype=bf16, device=self.dev)
-                x_mid, _ = ops.postnorm_fwd(ops.gemm_rows(att, W["Wo"]), W["g2"], x, self.eps, out16=h2)
-            else:
-                x_mid = ops.gemm_rows(att, W["Wo"], out_dtype=f32, resid=x, bias=W["bo"])
-                h2, _ = ops.rmsnorm_fwd(x_mid, W["g2"], self.eps)
+            x_mid, h2 = self._attn_out(att, W, x, ops.gemm_rows, a)
             if "moe" in W:
                 x, _ = moe.forward(h2, W["moe"], resid=x_mid)
-                continue
-            act = ops.swiglu_fwd(ops.gemm_rows(h2, W["Wgu"]), F, interleave=self.gu_il)
-            if self.post_norm:
-                h_next = _aug_buf(B, H, Ra, self.dev) if li + 1 < self.nl else None
-                x, _ = ops.postnorm_fwd(ops.gemm_rows(act, W["Wd"]), W["g3"], x_mid, self.eps,
-                                        out16=h_next[:, :H] if h_next is not None else None)
             else:
-                x = ops.gemm_rows(act, W["Wd"], out_dtype=f32, resid=x_mid)
+                act = ops.swiglu_fwd(ops.gemm_rows(h2, W["Wgu"]), self.F, interleave=self.gu_il)
+                x, h_next = self._mlp_out(act, W, x_mid, li + 1 < self.nl, ops.gemm_rows, a)
         hf, _ = ops.rmsnorm_fwd(x, self.norm_g, self.eps)
         return ops.gemm_rows(hf, self.lm_head)
 
@@ -641,8 +605,7 @@ class LlamaDecoder(torch.nn.Module):
         if not self.trainable:
             return
         B, L = ctx.B, ctx.L
-        M, H, F, Ra, r = B * L, self.H, self.F, self.Ra, self.r
-        cos_t, sin_t = self._rope(L)
+        M = B * L
         if dlogits.stride(-1) != 1 or dlogits.stride(-2) != self.Vp:             # a caller-made copy: re-pad to the GEMM layout
             pad = torch.zeros(B, L, self.Vp, dtype=bf16, device=self.dev)
             pad[:, :, :self.V] = dlogits
@@ -666,7 +629,7 @@ class LlamaDecoder(torch.nn.Module):
         cos_t, sin_t = self._rope(L)
         bank = self.full
         acc = getattr(ctx, "acc", False)
-        G = (lambda l, n: bank.g(f"L{l}.{n}")) if bank is not None else None
+        G = lambda l, n: bank.g(f"L{l}.{n}")
         if bank is not None:
             ops.col_reduce_(dy_bf16=dhf, z=ctx.x_final, rstd=ctx.rstdf, out_prod=bank.g("norm_g"))
         dx32, dx16 = ops.rmsnorm_bwd(ctx.x_final, self.norm_g, ctx.rstdf, dhf)
@@ -705,52 +668,37 @@ class LlamaDecoder(torch.nn.Module):
                      ctx.mask, a.att, a.lse, datt, B, L, self.nh, self.nkv, self.hd, causal=True,
                      dq=dqkv[:, :self.Nq], dk=dqkv[:, self.Nq:self.Nq + self.Nkv],
                      dv=dqkv[:, self.Nq + self.Nkv:self.Nqkv], window=self.windows[l])
-            if self.fullnorm:                                                      # un-rotate, then the full-width q/k norm backward
-                ops.qk_fullnorm_rope_bwd_(dqkv, self.nh, self.nkv, self.hd, W["qn"], W["kn"], cos_t, sin_t, L, a.pre, a.qk_rstd,
-                                          dw_q=G(l, "qn") if bank is not None else None,
-                                          dw_k=G(l, "kn") if bank is not None else None)
-            elif self.qk_norm:                                                     # un-rotate, then the q/k RMSNorm backward
-                ops.qk_norm_rope_bwd_(dqkv, self.nh + self.nkv, self.nh, W["qn"], W["kn"], cos_t, sin_t, L, a.pre, a.qk_rstd,
-                                      dw_q=G(l, "qn") if bank is not None else None, dw_k=G(l, "kn") if bank is not None else None)
-            else:
-                ops.rope_(dqkv, 0, self.nh + self.nkv, self.hd, cos_t, sin_t, L, backward=True)
+            self._qk_rope_bwd(l, dqkv, W, a, cos_t, sin_t, L)
             if bank is not None:
                 ops.wgrad_(dqkv, a.h1_aug[:, :H], G(l, "Wqkv"), acc)
                 if self.qkv_bias:                                                  # d bqkv = column sums of d(pre-RoPE qkv)
                     ops.col_reduce_(dy_bf16=dqkv, out_sum=G(l, "bqkv"))
                 dh1 = ops.gemm(dqkv, W["Wqkv_aug"], layout=1)
-                if self.post_norm:
-                    dx32, dpend = dmid32, dh1
+            else:
+                names = [f"model.layers.{l}.self_attn.{n}" for n in self.LORA_TARGETS]
+                for j, n in enumerate(self.LORA_TARGETS):
+                    c0, w = self._target_cols(n)
+                    ops.skinny_gemm(dqkv[:, c0:c0 + w], W["Bblk"][j * r:(j + 1) * r, c0:c0 + w], dqkv[:, self.Nqkv + j * r:], K=w, R=r)
+                # dA_q, dA_v in one pass over h1 (the 16-row MMA tile is exactly the two rank-8 adapters)
+                xdrop = self._drop(ctx.training, ctx.call, l)
+                ops.lora_wgrad_(a.h1_aug[:, :H], dqkv[:, self.Nqkv:], self.lora.gA[names[0]], H, 1, H, 2 * r, 1.0,
+                                out1=self.lora.gA[names[1]], dropx=xdrop)
+                for j, n in enumerate(self.LORA_TARGETS):
+                    c0, w = self._target_cols(n)
+                    ops.lora_wgrad_(dqkv[:, c0:c0 + w], a.h1_aug[:, H + j * r:], self.lora.gB[names[j]], 1, r, w, r, self.lora.scale)
+                if l == 0:
+                    break                                                          # embeddings frozen
+                if self.nf4 is not None:                                           # base path against the expanded W[out,in] + (g A)
+                    dh1 = ops.gemm(dqkv[:, :self.Nqkv], W["Wqkv_aug"][:, :H], layout=1)
+                    ops.lora_dx_(dh1, dqkv[:, self.Nqkv:], W["A_stack"], K=H, R=Ra, drop=xdrop)
+                elif xdrop is None:
+                    dh1 = ops.gemm(dqkv, W["WqkvT_aug"])                           # [M,H], LoRA's A-path folded into K
                 else:
-                    ops.col_reduce_(dy_bf16=dh1, z=a.x_in, rstd=a.rstd1, out_prod=G(l, "g1"))
-                    dx32, dx16 = ops.rmsnorm_bwd(a.x_in, W["g1"], a.rstd1, dh1, dres_in=dmid32)
+                    dh1 = ops.gemm(dqkv[:, :self.Nqkv], W["WqkvT_aug"][:, :self.Nqkv])
+                    ops.lora_dx_(dh1, dqkv[:, self.Nqkv:], W["A_stack"], K=H, R=Ra, drop=xdrop)
+            dx32, dx16, dpend = self._layer_in_bwd(l, a, W, dh1, dmid32)
+            if bank is not None:
                 bank.bucket_ready(f"L{l}.")                                        # this layer's four weight gradients are final
-                continue
-            names = [f"model.layers.{l}.self_attn.{n}" for n in self.LORA_TARGETS]
-            for j, n in enumerate(self.LORA_TARGETS):
-                c0, w = self._target_cols(n)
-                ops.skinny_gemm(dqkv[:, c0:c0 + w], W["Bblk"][j * r:(j + 1) * r, c0:c0 + w], dqkv[:, self.Nqkv + j * r:], K=w, R=r)
-            # dA_q, dA_v in one pass over h1 (the 16-row MMA tile is exactly the two rank-8 adapters)
-            xdrop = self._drop(ctx.training, ctx.call, l)
-            ops.lora_wgrad_(a.h1_aug[:, :H], dqkv[:, self.Nqkv:], self.lora.gA[names[0]], H, 1, H, 2 * r, 1.0,
-                            out1=self.lora.gA[names[1]], dropx=xdrop)
-            for j, n in enumerate(self.LORA_TARGETS):
-                c0, w = self._target_cols(n)
-                ops.lora_wgrad_(dqkv[:, c0:c0 + w], a.h1_aug[:, H + j * r:], self.lora.gB[names[j]], 1, r, w, r, self.lora.scale)
-            if l == 0:
-                break                                                              # embeddings frozen
-            if self.nf4 is not None:                                               # base path against the expanded W[out,in] + (g A)
-                dh1 = ops.gemm(dqkv[:, :self.Nqkv], W["Wqkv_aug"][:, :H], layout=1)
-                ops.lora_dx_(dh1, dqkv[:, self.Nqkv:], W["A_stack"], K=H, R=Ra, drop=xdrop)
-            elif xdrop is None:
-                dh1 = ops.gemm(dqkv, W["WqkvT_aug"])                               # [M,H], LoRA's A-path folded into K
-            else:
-                dh1 = ops.gemm(dqkv[:, :self.Nqkv], W["WqkvT_aug"][:, :self.Nqkv])
-                ops.lora_dx_(dh1, dqkv[:, self.Nqkv:], W["A_stack"], K=H, R=Ra, drop=xdrop)
-            if self.post_norm:
-                dx32, dpend = dmid32, dh1
-            else:
-                dx32, dx16 = ops.rmsnorm_bwd(a.x_in, W["g1"], a.rstd1, dh1, dres_in=dmid32)
         if bank is not None:
             if self.post_norm:                                                     # d(embeddings) = residual + QKV-input gradients
                 dx32 = ops.masked_add(a=dx32, b=dpend)

@@ -4,7 +4,8 @@ from __future__ import annotations
 import json
 import math
 import os
-from typing import Dict, List, Optional
+from dataclasses import dataclass
+from typing import Callable, Dict, List, Optional
 
 import torch
 
@@ -63,13 +64,13 @@ def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, 
             sd[p + "output.LayerNorm.bias"] = _normal(gen, (H,), std, dtype, device)
         sd["pooler.dense.weight"] = _normal(gen, (H, H), std, dtype, device)   # loaded by AutoModel, unused by the path
         sd["pooler.dense.bias"] = zeros(H)
-    elif kind in ("llama", "qwen2", "qwen3", "mistral", "qwen3_moe") + OLMO_KINDS:
+    elif kind in DECODER_TRAITS:
+        t = DECODER_TRAITS[kind]
         F, V = cfg.get("intermediate_size"), cfg["vocab_size"]
-        sparse = moe_layers(cfg) if kind in ("qwen3_moe", "olmoe") else [False] * cfg["num_hidden_layers"]
-        post_norm = kind in ("olmo2", "olmo3")
+        sparse = moe_layers(cfg) if t.routed else [False] * cfg["num_hidden_layers"]
         nh, nkv = cfg["num_attention_heads"], cfg.get("num_key_value_heads", cfg["num_attention_heads"])
         hd = cfg.get("head_dim") or H // nh
-        qkv_bias, o_bias = attention_biases(kind, cfg) if kind not in OLMO_KINDS else (False, False)
+        qkv_bias, o_bias = attention_biases(kind, cfg)
         bstd = std if bias_std is None else float(bias_std)
         sd["model.embed_tokens.weight"] = _normal(gen, (V, H), std, dtype, device)
         for l in range(cfg["num_hidden_layers"]):
@@ -84,14 +85,11 @@ def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, 
                 sd[p + "self_attn.v_proj.bias"] = _normal(gen, (nkv * hd,), bstd, dtype, device)
             if o_bias:
                 sd[p + "self_attn.o_proj.bias"] = _normal(gen, (H,), bstd, dtype, device)
-            if kind in ("qwen3", "qwen3_moe"):
+            if t.qk_norm:                                          # per head, or over the whole projection width
                 nstd = std if qk_norm_std is None else float(qk_norm_std)
-                sd[p + "self_attn.q_norm.weight"] = ones(hd) + _normal(gen, (hd,), nstd, dtype, device)
-                sd[p + "self_attn.k_norm.weight"] = ones(hd) + _normal(gen, (hd,), nstd, dtype, device)
-            if kind in OLMO_KINDS:                                 # q / k RMSNorm over the whole projection width
-                nstd = std if qk_norm_std is None else float(qk_norm_std)
-                sd[p + "self_attn.q_norm.weight"] = ones(nh * hd) + _normal(gen, (nh * hd,), nstd, dtype, device)
-                sd[p + "self_attn.k_norm.weight"] = ones(nkv * hd) + _normal(gen, (nkv * hd,), nstd, dtype, device)
+                nq, nk = (hd, hd) if t.qk_norm == "head" else (nh * hd, nkv * hd)
+                sd[p + "self_attn.q_norm.weight"] = ones(nq) + _normal(gen, (nq,), nstd, dtype, device)
+                sd[p + "self_attn.k_norm.weight"] = ones(nk) + _normal(gen, (nk,), nstd, dtype, device)
             if sparse[l]:
                 E, I = cfg["num_experts"], moe_intermediate_size(cfg)
                 sd[p + "mlp.gate.weight"] = _normal(gen, (E, H), std if router_std is None else float(router_std), dtype, device)
@@ -103,7 +101,7 @@ def random_state_dict(kind: str, cfg: Dict, seed: int = 0, dtype=torch.float32, 
                 sd[p + "mlp.gate_proj.weight"] = _normal(gen, (F, H), std, dtype, device)
                 sd[p + "mlp.up_proj.weight"] = _normal(gen, (F, H), std, dtype, device)
                 sd[p + "mlp.down_proj.weight"] = _normal(gen, (H, F), std, dtype, device)
-            if post_norm:                                          # OLMo 2 / 3: norms after each sublayer, none before
+            if t.post_norm:                                        # OLMo 2 / 3: norms after each sublayer, none before
                 sd[p + "post_attention_layernorm.weight"] = ones(H) + _normal(gen, (H,), std, dtype, device)
                 sd[p + "post_feedforward_layernorm.weight"] = ones(H) + _normal(gen, (H,), std, dtype, device)
             else:
@@ -192,12 +190,8 @@ def model_kind(cfg: Dict) -> str:
     if mt in ("roberta", "xlm-roberta"):
         check_roberta(cfg)
         return "roberta"
-    if mt in ("llama", "qwen2", "qwen3", "mistral", "qwen3_moe"):
-        check_llama_family(cfg)
-        return mt
-    if mt in OLMO_KINDS:
-        check_olmo(cfg)
-        return mt
+    if mt in DECODER_TRAITS:
+        return resolve_decoder(cfg).kind
     if mt == "modernbert":
         check_modernbert(cfg)
         return "modernbert"
@@ -334,10 +328,6 @@ def check_llama_family(cfg: Dict) -> None:
         raise NotImplementedError(f"{mt}: mlp_bias=true is not built (the fused SwiGLU MLP has no bias)")
     if mt == "qwen3_moe":
         check_qwen3_moe(cfg)
-    if mt in ("qwen3", "qwen3_moe"):
-        hd = cfg.get("head_dim") or cfg["hidden_size"] // cfg["num_attention_heads"]
-        if hd != 128:
-            raise NotImplementedError(f"{mt}: head_dim={hd} is not built (the q/k norm kernels take head_dim 128)")
     if mt == "qwen3_moe":
         rt = _rope_type(cfg)
         if rt != "default":
@@ -459,7 +449,6 @@ def sliding_windows(cfg: Dict) -> List[int]:
     return [0] * n
 
 
-OLMO_KINDS = ("olmo2", "olmo3", "olmoe")
 # keys without which transformers would fill in its config class's defaults (the 7B shapes); the shape is read from config.json
 OLMO_SHAPE_KEYS = ("hidden_size", "intermediate_size", "num_hidden_layers", "num_attention_heads", "vocab_size")
 
@@ -491,8 +480,94 @@ def check_olmo(cfg: Dict) -> None:
     check_rope_type(cfg)
     if mt == "olmoe":
         check_moe_bounds(cfg)
-    else:
-        sliding_windows(cfg)
+
+
+@dataclass(frozen=True)
+class DecoderTraits:
+    """what the layers of one Llama-family model type contain, whatever its config says"""
+    check: Callable[[Dict], None]        # refuses the configs of this type that LlamaDecoder would compute wrong or cannot run
+    qk_norm: str = ""                    # q/k RMSNorm before RoPE: "head" per head (Qwen3), "full" over the whole q / k width (OLMo)
+    round_first: bool = False            # OlmoeRMSNorm: q / k rounded to bf16 before the norm weight multiplies them
+    post_norm: bool = False              # norms after each sublayer (post_attention / post_feedforward), none before
+    routed: str = ""                     # the layers of `moe_layers` run routed SwiGLU experts; names the published checkpoint
+                                         # and what fully fine-tuning it would need (~18 bytes per parameter)
+    bias: Optional[tuple] = None         # fixed (q/k/v biases, o_proj bias); None: `attention_bias` on all four
+    retriever: bool = True               # may serve as an autoregressive retriever
+    nf4: bool = False                    # 4-bit storage (engine/nf4store.py) is built
+
+
+# MistralAttention ignores `attention_bias`; OLMo configs that set it are refused (check_olmo)
+DECODER_TRAITS = {
+    "llama": DecoderTraits(check_llama_family, nf4=True),
+    "mistral": DecoderTraits(check_llama_family, bias=(False, False)),
+    "qwen2": DecoderTraits(check_llama_family, bias=(True, False)),
+    "qwen3": DecoderTraits(check_llama_family, qk_norm="head"),
+    "qwen3_moe": DecoderTraits(check_llama_family, qk_norm="head", routed="Qwen3-30B-A3B would need ~550 GB", retriever=False),
+    "olmo2": DecoderTraits(check_olmo, qk_norm="full", post_norm=True, bias=(False, False)),
+    "olmo3": DecoderTraits(check_olmo, qk_norm="full", post_norm=True, bias=(False, False)),
+    "olmoe": DecoderTraits(check_olmo, qk_norm="full", round_first=True, routed="OLMoE-1B-7B would need ~125 GB",
+                           bias=(False, False), retriever=False),
+}
+
+
+@dataclass(frozen=True)
+class DecoderArch:
+    """a Llama-family config resolved once: its type's traits and what the config decides for every layer"""
+    kind: str
+    traits: DecoderTraits
+    H: int
+    F: int                               # width of the dense SwiGLU MLP (0: none)
+    nl: int
+    nh: int
+    nkv: int
+    hd: int
+    V: int
+    eps: float
+    qkv_bias: bool
+    o_bias: bool
+    sparse: List[bool]                   # the layers that run the routed MLP
+    windows: List[int]                   # key window of each layer, 0 = full causal attention
+    inv_freq: torch.Tensor               # RoPE frequencies: default, linear, llama3 or yarn (fp32, CPU)
+    rope_scale: float                    # yarn's attention factor on cos / sin, else 1
+
+
+def resolve_decoder(cfg: Dict) -> DecoderArch:
+    """the architecture of a Llama-family config; raises NotImplementedError for model types, and for settings of the built
+    ones, that the decoder does not build"""
+    mt = cfg.get("model_type", "")
+    t = DECODER_TRAITS.get(mt)
+    if t is None:
+        raise NotImplementedError(f"model_type {mt!r} is not a Llama-family decoder")
+    t.check(cfg)
+    H, nh = cfg["hidden_size"], cfg["num_attention_heads"]
+    hd = cfg.get("head_dim") or H // nh
+    if t.qk_norm == "head" and hd != 128:
+        raise NotImplementedError(f"{mt}: head_dim={hd} is not built (the q/k norm kernels take head_dim 128)")
+    if hd not in (32, 64, 128):
+        raise NotImplementedError(f"head_dim {hd} not supported by the attention kernels")
+    sparse = moe_layers(cfg) if t.routed else [False] * cfg["num_hidden_layers"]
+    qkv_bias, o_bias = attention_biases(mt, cfg)
+    # without dense layers, qwen3_moe may leave intermediate_size out and olmoe's sizes its experts
+    return DecoderArch(kind=mt, traits=t, H=H, F=0 if all(sparse) else cfg.get("intermediate_size") or 0, nl=len(sparse), nh=nh,
+                       nkv=cfg.get("num_key_value_heads", nh), hd=hd, V=cfg["vocab_size"],
+                       eps=float(cfg.get("rms_norm_eps", 1e-5)), qkv_bias=qkv_bias, o_bias=o_bias, sparse=sparse,
+                       windows=sliding_windows(cfg), inv_freq=rope_inv_freq(cfg, hd), rope_scale=rope_attention_factor(cfg, hd))
+
+
+def check_decoder_mode(kind: str, full: bool = False, bnb: bool = False, nf4_storage: bool = False) -> None:
+    """refuses the training and storage modes a decoder of this kind is not built for: full fine-tuning and use_bnb of the
+    routed-MoE kinds, and 4-bit storage outside the kinds that build it"""
+    t = DECODER_TRAITS.get(kind, DecoderTraits(check=None))           # not a Llama-family kind: no routed MLP, no 4-bit storage
+    if t.routed and full:
+        raise NotImplementedError(f"full fine-tuning of a {kind} generator is not built: grouped expert weight gradients are "
+                                  "not built, and at ~18 bytes per parameter (fp32 master, gradient, Adam moments, bf16 copy) "
+                                  f"{t.routed}; use LoRA (use_peft) on the generator")
+    if t.routed and (bnb or nf4_storage):
+        raise NotImplementedError(f"use_bnb on a {kind} generator is not built: the 4-bit treatment of the fused 3-D expert "
+                                  "weights differs across transformers versions, so no single reference exists to match")
+    if nf4_storage and not t.nf4:
+        raise NotImplementedError(f"DALM_B200_NF4_STORAGE=1: 4-bit storage is built for BERT / (XLM-)RoBERTa encoders and Llama "
+                                  f"decoders, not {kind!r}")
 
 
 def check_roberta(cfg: Dict) -> None:
@@ -582,15 +657,9 @@ def roberta_max_len(cfg: Dict) -> int:
 
 
 def attention_biases(kind: str, cfg: Dict):
-    """(q/k/v projections carry a bias, o_proj carries a bias) for a llama-family config: Qwen2 has q/k/v biases only, Llama
-    and Qwen3 have all four when `attention_bias` is set, Mistral has none (MistralAttention ignores the key)"""
-    if kind == "qwen2":
-        return True, False
-    if kind == "mistral":
-        return False, False
-    # qwen3_moe: Qwen3MoeAttention, Qwen3's attention (`attention_bias` on all four projections)
+    """(q/k/v projections carry a bias, o_proj carries a bias) for a llama-family config, by its kind's DecoderTraits.bias"""
     ab = bool(cfg.get("attention_bias", False))
-    return ab, ab
+    return DECODER_TRAITS[kind].bias or (ab, ab)
 
 
 def is_bnb_linear_weight(name: str) -> bool:

@@ -82,7 +82,7 @@ def build_encoder(name_or_path: str, lora: bool, device: torch.device, state_dic
     if not nf4:
         sd = _maybe_bnb(sd, bnb, full, device)
     if autoregressive:
-        if kind not in ("llama", "qwen2", "qwen3", "mistral", "olmo2", "olmo3"):
+        if kind not in params.DECODER_TRAITS or not params.DECODER_TRAITS[kind].retriever:
             raise NotImplementedError("autoregressive retrievers are built for Llama, Qwen2 and Qwen3 models only, and for OLMo 2 "
                                       "and OLMo 3; Mistral runs as Llama with a sliding window")
         return _named(LlamaDecoder(cfg, sd, device=device, lora=lora, lora_seed=0, full=full, nf4_storage=nf4), name_or_path)
@@ -114,22 +114,6 @@ def _named(engine_model, name_or_path: str):
     return engine_model
 
 
-# the published checkpoint of each routed-MoE kind and its full fine-tuning footprint at ~18 bytes per parameter
-_MOE_FULL_FT = {"qwen3_moe": "Qwen3-30B-A3B would need ~550 GB", "olmoe": "OLMoE-1B-7B would need ~125 GB"}
-
-
-def _check_moe_mode(kind: str, full: bool, bnb: bool) -> None:
-    """routed-MoE generators (Qwen3-MoE, OLMoE) run frozen or with LoRA on q_proj / v_proj; every other mode is refused, naming
-    why"""
-    if full:
-        raise NotImplementedError(f"full fine-tuning of a {kind} generator is not built: grouped expert weight gradients are "
-                                  "not built, and at ~18 bytes per parameter (fp32 master, gradient, Adam moments, bf16 copy) "
-                                  f"{_MOE_FULL_FT[kind]}; use LoRA (use_peft) on the generator")
-    if bnb:
-        raise NotImplementedError(f"use_bnb on a {kind} generator is not built: the 4-bit treatment of the fused 3-D expert "
-                                  "weights differs across transformers versions, so no single reference exists to match")
-
-
 def _nf4_storage(bnb: bool, full: bool, kind: str) -> bool:
     """use_bnb + DALM_B200_NF4_STORAGE=1: keep the sub-model's Linear weights as packed NF4 codes and expand them per use
     (engine/nf4store.py) instead of the dequantised-resident default. BERT / (XLM-)RoBERTa encoders and Llama decoders."""
@@ -138,9 +122,8 @@ def _nf4_storage(bnb: bool, full: bool, kind: str) -> bool:
         return False
     if full:
         _maybe_bnb({}, True, True, None)                      # raises: 4-bit base weights cannot be fully fine-tuned
-    if kind not in ("bert", "roberta", "llama"):
-        raise NotImplementedError(f"DALM_B200_NF4_STORAGE=1: 4-bit storage is built for BERT / (XLM-)RoBERTa encoders and Llama "
-                                  f"decoders, not {kind!r}")
+    if kind not in ("bert", "roberta"):
+        params.check_decoder_mode(kind, nf4_storage=True)
     return True
 
 
@@ -167,15 +150,14 @@ def build_decoder(name_or_path: str, lora: bool, device: torch.device, state_dic
                   cfg: Optional[Dict] = None, full: bool = False, bnb: bool = False) -> LlamaDecoder:
     cfg = cfg or params.load_config(name_or_path)
     kind = params.model_kind(cfg)                # raises for unsupported families
-    if kind in _MOE_FULL_FT:
-        _check_moe_mode(kind, full, bnb)
+    params.check_decoder_mode(kind, full, bnb)
     sd = state_dict if state_dict is not None else params.load_state_dict(name_or_path)
     nf4 = _nf4_storage(bnb, full, kind)
     if not nf4:
         sd = _maybe_bnb(sd, bnb, full, device)
     if kind == "falcon":
         dec = FalconDecoder(cfg, sd, device=device, lora=lora, full=full)      # raises for lora=True, like peft would
-    elif kind not in ("llama", "qwen2", "qwen3", "mistral", "qwen3_moe", "olmo2", "olmo3", "olmoe"):
+    elif kind not in params.DECODER_TRAITS:
         raise NotImplementedError(f"generator of kind {kind!r} is not a causal decoder")
     else:
         dec = LlamaDecoder(cfg, sd, device=device, lora=lora, full=full, nf4_storage=nf4)
